@@ -1,6 +1,6 @@
-# Builds libdph_b200.so (sm_100a only) and the CPU oracle. `python -c "import __graft_entry__ as g; g.build()"` calls this.
+# Builds libdph_b200.so (sm_90a, H100 only) and the CPU oracle. `python -c "import __graft_entry__ as g; g.build()"` calls this.
 NVCC ?= nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC -Xcompiler -fvisibility=hidden --expt-relaxed-constexpr -Xptxas -v
 CSRC := densephrases_b200/csrc
 OBJDIR := build/obj

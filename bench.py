@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- queries/sec top-10 over the synthetic PQ96 phrase index (BASELINE.json metric), one process per GPU.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--dump-outputs DIR]   # this repo's CUDA path
   python bench.py --impl reference [...]                          # the reference's CPU path (FAISS-equivalent restatement)
 
 A *step* is one pass of the hot path (OPQ rotation -> coarse top-nprobe -> LUT -> PQ96 scan -> top-k merge) over one
@@ -9,11 +9,14 @@ batch of synthetic d=768 vector queries (SURVEY.md 8d: seed 1234 index, seed 432
 
   N = 1   C2 (BASELINE.json configs[1]): 100M phrases, IVF4096,PQ96, batch 64, nprobe 256 (the reference's fixed value,
           densephrases/index.py:53,62).  Extra legs in the same line: C1 (configs[0]), the encoder + C3 (configs[2]), and C4's
-          1B-phrase index held by this ONE GPU (96 GB) so that the metric's "@1/2/4/8 B200" series has its N=1 point.
+          index shape (IVF65536, batch 1024) on this ONE GPU with half of C4's phrases (500M, 48 GB of codes: the 1B-phrase index
+          needs 96 GB, more than an 80 GB H100 holds).
   N >= 2  C4 (configs[3]): 1B phrases, IVF65536,PQ96, batch 1024, list-range shards over the N ranks (strong scaling: the
           index and the batch are fixed), `value` at the reference's nprobe 256; the `nprobe32` object holds the same
           measurement at nprobe 32 (BASELINE.md: C4 is reported at nprobe 256 AND 32).
 Both arms draw the SAME query vectors (make_query_plan / finish_queries).  Prints ONE JSON line on rank 0.
+--dump-outputs DIR writes what the timed search returned in its last step (scores.npy float32, labels.npy float64, [batch, k]) and,
+with the encoder leg, the [CLS] vectors of each precision mode (encoder_<mode>.npy float32, start rows then end rows).
 """
 import argparse
 import hashlib
@@ -71,11 +74,11 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1412.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback"          # H100 SXM data sheet (dense bf16), not measured
 
 
 def csrc_sha():
-    """Hash of the CUDA sources: ties an ncu-derived number under profiles/ to the tree it was measured on."""
+    """Hash of the CUDA sources: ties a stored traffic measurement to the tree it was measured on."""
     h = hashlib.sha256()
     d = os.path.join(ROOT, "densephrases_b200", "csrc")
     for f in sorted(os.listdir(d)):
@@ -397,12 +400,11 @@ def measure_search(cx, ix, wl, Q, Qh, nprobe, sample_clocks=False):
     if pair_mode:
         roofline["note"] = ("algorithmic bytes count every (query, probed vector) pair; the kernel serves the 2 / 4 queries of a group from one code read and "
                             "later readers of a list from L2, so achieved > DRAM traffic and frac may exceed 1; the kernel's own limiters are the LSU "
-                            "data pipe (shared-memory gathers) and the issue slots, see profiles/ and DESIGN.md 4.1")
+                            "data pipe (shared-memory gathers) and the issue slots, see DESIGN.md 4.1")
     # step-level fraction of the HBM roofline: all ranks' algorithmic bytes / (step time x N x peak)
     tot_bytes = cx.sum_over_ranks(mean_bytes)
     step_frac = tot_bytes / (ms_dev / K / 1000.0) / 1e9 / (cx.world * pk["hbm_gbs"])
-    # kernels of this repo launched per search step (counted from the per-launch lists in profiles/: r2q_launches_c2.csv,
-    # r2q_launches_shard_c4_np*.csv): one GPU: rotation, coarse quantizer, tables, plan, scan, merge, 4 early-exit fallback launches;
+    # kernels of this repo launched per search step (counted from per-launch lists of one step): one GPU: rotation, coarse quantizer, tables, plan, scan, merge, 4 early-exit fallback launches;
     # sharded: + record pack / unpack (query-split) or coarse merge (list-split), + top-k pack and merge
     from densephrases_b200.sharded import use_query_split
     if cx.world == 1:
@@ -420,7 +422,7 @@ def measure_search(cx, ix, wl, Q, Qh, nprobe, sample_clocks=False):
 
 
 def lookup_traffic(kernel, wl_name, nprobe, world):
-    """dram bytes per launch of `kernel` from the ncu pass tools/profile.sh made on THIS tree (profiles/traffic.json, keyed by the
+    """dram bytes per launch of `kernel` from a profiler pass made on THIS tree (profiles/traffic.json, keyed by the
     hash of csrc/); null when the sources changed since."""
     tp = os.path.join(ROOT, "profiles", "traffic.json")
     if not os.path.exists(tp):
@@ -532,6 +534,8 @@ def run_ours(args):
     Q, Qh = queries(ix, wl, W + K)
     stage(f"{wl['name']} index built ({ix.local.device_bytes / 1e9:.1f} GB on this rank), queries made")
     main = measure_search(cx, ix, wl, Q, Qh, wl["nprobe"], sample_clocks=True)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, scores=main["_last"][0], labels=main["_last"][1])
     second = None
     if wl["name"] == "C4":
         second = measure_search(cx, ix, wl, Q, Qh, 32)
@@ -571,6 +575,8 @@ def run_ours(args):
     if world == 1:
         if not args.no_encoder:
             line["encoder"] = encoder_leg(cx, ix, wl)
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, **{f"encoder_{m}": o for m, o in line["encoder"].pop("_outputs").items()})
             stage("encoder leg done")
         del ix, Q
         torch.cuda.empty_cache()
@@ -628,11 +634,12 @@ def c1_leg(cx, build, queries, args):
 
 
 def c4_single_gpu_leg(cx, build, queries, args):
-    """C4's index (1B phrases, IVF65536, 96 GB of codes) held by ONE B200, batch 1024: the N = 1 point of the metric's 1/2/4/8 series."""
+    """C4's index shape (IVF65536, batch 1024) on ONE GPU with half of C4's phrases: 500M phrases, 48 GB of codes (the full 1B-phrase
+    index needs 96 GB, more than one 80 GB H100 holds)."""
     import torch
-    wl = workload("C4", args.scale)
+    wl = workload("C4", 0.5 * args.scale)
     save = (cx.W, cx.K)
-    cx.W, cx.K = 3, max(5, min(cx.K, 20))
+    cx.W, cx.K = 3, min(cx.K, 20)
     try:
         ix = build(wl)
         Q, Qh = queries(ix, wl, cx.W + cx.K)
@@ -728,6 +735,7 @@ def encoder_leg(cx, ix, wl):
     ms, _ = time_fn(c3, reps=10, warm=3)
     info["c3"] = {"mode": mode, "questions_per_s": 64000.0 / ms, "ms_per_64_questions": ms, "h2d_bytes_per_step": 3 * 64 * 64 * 8,
                   "d2h_bytes_per_step": 128 * k * 12, "what": "host token ids -> 2 towers -> stacked 128-vector search on the C2 index -> host top-10"}
+    info["_outputs"] = {m: o.cpu().numpy() for m, o in outs.items()}
     del enc
     return info
 
@@ -766,6 +774,14 @@ def emit(line):
         os.write(_REAL_STDOUT, data)
 
 
+def dump_outputs(d, **arrays):
+    """One DIR/<name>.npy per array: floating arrays as float32, integer arrays (labels) as float64 (exact below 2^53)."""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float32 if a.dtype.kind == "f" else np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -778,6 +794,7 @@ def main():
     ap.add_argument("--no-encoder", action="store_true", help="skip the C3 encoder leg")
     ap.add_argument("--no-c1", action="store_true", help="skip the C1 leg")
     ap.add_argument("--no-c4", action="store_true", help="N=1: skip the C4-on-one-GPU leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.steps is None:

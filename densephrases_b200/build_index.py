@@ -1,6 +1,6 @@
 """Index builder: train and fill an OPQ96 / IVF{nlist} / PQ96 inner-product phrase index without FAISS.
 
-Restates what /root/reference/build_phrase_index.py asks faiss to do (SURVEY.md 8f #4; offline, not on the serving hot path):
+Restates what reference build_phrase_index.py asks faiss to do (SURVEY.md 8f #4; offline, not on the serving hot path):
   train_index  (:96-142)   IndexPreTransform(OPQMatrix(768, 96; niter=10), IndexIVFPQ(IndexFlatIP(768), 768, nlist, 96, 8, IP))
   add_to_index (:145-150)  add_with_ids(vectors, ids = arange + offset + running_total)
 following the published faiss algorithms: OPQ (Ge et al., non-parametric variant: alternate PQ training with an orthogonal

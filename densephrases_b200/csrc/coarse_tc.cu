@@ -1,6 +1,6 @@
 // coarse_tc.cu -- coarse quantizer (faiss IndexFlatIP top-nprobe, reference call site densephrases/index.py:200) on the tensor
 // cores WITHOUT giving up the bit-exact sequential-FMA definition of the scores (oracle/ivfpq_ref.c):
-//   1. approximate scores  S~ = xr . C^T  with the 3xTF32 tcgen05 GEMM (gemm_tf32.cu), error <= B(q) = c |xr_q| max_l |C_l|;
+//   1. approximate scores  S~ = xr . C^T  with the 3xTF32 wgmma GEMM (gemm_tf32.cu), error <= B(q) = c |xr_q| max_l |C_l|;
 //   2. candidates = top-(nprobe + margin) of S~ per query;
 //   3. candidates are re-scored EXACTLY (one sequential fp32 FMA chain each, identical to sgemm_nt_seq / the oracle);
 //   4. top-nprobe of the exact scores, (score desc, list asc); the result is provably the global top-nprobe when
@@ -132,9 +132,9 @@ __global__ void cnorm_max_kernel(const float* C, long long nl, float* out) {
 int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, unsigned long long* keys64, int32_t* key, float* cd, cudaStream_t st) {
     const int margin = nprobe / 4 > 32 ? nprobe / 4 : 32;
     const int ncand = (int)std::min<int64_t>(nprobe + margin, nl);
-    // measured on B200 (tools/bench_shard.py): pays for small probe counts (C4 nprobe 32: 0.48 -> 0.28 ms per 1024 queries);
-    // at nprobe 256 the exact re-rank of 320 candidates costs what the tensor cores save, so the SIMT GEMM is kept there.
-    // With many lists per candidate (C5: 131 072 lists per shard, 320 candidates) the GEMM dominates again and the tensor cores win.
+    // pays for small probe counts; at nprobe 256 the exact re-rank of 320 candidates costs about what the tensor cores save, so the
+    // SIMT GEMM is kept there.  With many lists per candidate (131 072 lists per shard, 320 candidates) the GEMM dominates again
+    // and the tensor cores win.  Compare both paths with tools/bench_shard.py.
     const bool few_candidates = ncand <= 160 && nl > 4 * (int64_t)ncand;
     const bool many_lists = nl >= 32 * (int64_t)ncand;
     if (ncand > DPH_MAX_NPROBE || n < 32 || !(few_candidates || many_lists)) return 1;

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libdph_b200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libdph_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -49,6 +49,11 @@ struct DphPerDeviceOnce {
         return true;
     }
 };
+
+// Component-wise float2 FMA / add: two independent IEEE fp32 operations (Hopper has no packed f32x2 instructions), so each
+// component follows exactly the rounding chain of a scalar accumulator.
+__device__ __forceinline__ float2 dph_ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 dph_fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 
 // ---- counter-based generator: bit-identical to oracle/ivfpq_ref.c (mix64 / rnd64 / approx_normal) ----
 __host__ __device__ __forceinline__ uint64_t dph_mix64(uint64_t x) {

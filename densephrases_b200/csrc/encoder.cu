@@ -1,7 +1,7 @@
 // encoder.cu -- query-side encoder forward: two independent BERT-base towers on the same tokens, hidden state at
-// position 0 of each (Encoder.forward(return_query=True) -> embed_query, /root/reference/densephrases/encoder.py:146-152,
+// position 0 of each (Encoder.forward(return_query=True) -> embed_query, reference densephrases/encoder.py:146-152,
 // 101-118; HF BertModel semantics restated in SURVEY.md Appendix B).  Both towers run as one grouped problem:
-// every GEMM is one launch of the tcgen05 TF32 kernel (gemm_tf32.cu) with blockIdx.z = tower.
+// every GEMM is one launch of the wgmma GEMM (gemm_tf32.cu / gemm_bf16x3.cu) over the tiles of both towers.
 #include "common.cuh"
 #include "../../include/dph_b200.h"
 #include <cuda_bf16.h>
@@ -374,7 +374,7 @@ DPH_API int dph_encoder_create(dph_encoder** out, int device, int vocab_size, in
     DPH_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     DPH_CUDA(cudaGetDeviceProperties(&prop, device));
-    DPH_CHECK(prop.major == 10, "libdph_b200 is built for sm_100a (B200) only");
+    DPH_CHECK(prop.major == 9 && prop.minor == 0, "libdph_b200 is built for sm_90a (H100) only");
     dph_encoder* e = new dph_encoder();
     e->device = device; e->vocab = vocab_size; e->max_pos = max_pos; e->type_vocab = type_vocab;
     *out = e;
@@ -404,7 +404,7 @@ DPH_API int dph_encoder_set_attention(dph_encoder* e, int tensor_core) { e->atte
 DPH_API int dph_attention_bert(const float* qkv, const int64_t* mask, int B, int S, float* ctx, int tensor_core, void* cuda_stream) {
     DPH_CHECK(qkv && mask && ctx && B >= 1 && S >= 1 && S <= ENC_MAX_S, "attention: bad arguments");
     DPH_CHECK(!tensor_core || S <= 64, "tensor-core attention handles S <= 64");
-    DPH_CHECK(tensor_core >= 0 && tensor_core <= 2, "tensor_core: 0 SIMT fp32, 1 tcgen05 TF32, 2 tcgen05 bf16x3 planes (fp32-accurate)");
+    DPH_CHECK(tensor_core >= 0 && tensor_core <= 2, "tensor_core: 0 SIMT fp32, 1 wgmma TF32, 2 wgmma bf16x3 planes (fp32-accurate)");
     cudaStream_t st = (cudaStream_t)cuda_stream;
     float* scratch = nullptr;                            // the launchers run two towers: the second one repeats the first into scratch
     DPH_CUDA(cudaMalloc((void**)&scratch, (size_t)B * S * ENC_H * 4));

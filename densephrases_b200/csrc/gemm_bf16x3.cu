@@ -1,190 +1,22 @@
-// gemm_bf16x3.cu -- fp32-in / fp32-out dense layer on the tcgen05 tensor cores at bf16 MMA rate with ~2^-17 relative accuracy:
+// gemm_bf16x3.cu -- fp32-in / fp32-out dense layer on the Hopper tensor cores at bf16 MMA rate with ~2^-17 relative accuracy:
 // every fp32 operand x is carried as TWO bf16 planes (hi = bf16(x), lo = bf16(x - hi), x = hi + lo up to 2^-18 |x|) and the kernel
-// accumulates  a_hi.b_lo + a_lo.b_hi + a_hi.b_hi  in one fp32 TMEM accumulator (each bf16 x bf16 product is exact in fp32; the
-// dropped lo.lo term is 2^-18 relative).  Three kind::f16 MMAs cost 1.5 TF32 MMAs and the operand stream is the same 4 bytes per
-// element as fp32, so the layer runs at the speed of the 1xTF32 kernel (both are bound by the L2 -> SM operand stream, DESIGN.md 4.2)
-// while meeting the 1e-3 tolerance the north star sets for the query vectors (tests/test_encoder.py) -- the 3xTF32 kernel
-// (gemm_tf32.cu, 2^-22) needs 3 TF32 MMAs and twice the operand bytes for that.
+// accumulates  a_hi.b_lo + a_lo.b_hi + a_hi.b_hi  in one fp32 register accumulator (each bf16 x bf16 product is exact in fp32; the
+// dropped lo.lo term is 2^-18 relative).  Three bf16 wgmmas cost 1.5 TF32 wgmmas and the operand stream is the same 4 bytes per
+// element as fp32, while meeting the 1e-3 tolerance the north star sets for the query vectors (tests/test_encoder.py) -- the
+// 3xTF32 kernel (2^-22) needs 3 TF32 wgmmas and twice the operand bytes for that.
 //
-// Same persistent schedule as gemm_tf32_persist_kernel: one CTA per SM walks 128 x 256 output tiles, warp 0 = TMA producer
-// (4-stage ring; a stage is a 32-element k block: A_hi, A_lo 128 x 32 and B_hi, B_lo 256 x 32 bf16, SWIZZLE_64B, 48 KB), warp 1 = one
-// elected thread issuing 2 x 3 tcgen05.mma.kind::f16 128x256x16 per stage into one of two 256-column TMEM accumulators, warps 4-15 =
-// epilogue (tcgen05.ld -> bias / erf-GELU / residual -> fp32 rows and/or the (hi, lo) bf16 planes the NEXT layer consumes).
-// Reference op: torch.nn.functional.linear inside HF BertModel (densephrases/encoder.py:101-118).
-#include "umma.cuh"
+// Persistent schedule of gemm_wgmma_kernel (gemm_wgmma.cuh): one CTA per SM walks 128 x BN output tiles; a stage is a 32-element
+// k block (A_hi, A_lo 128 x 32 and B_hi, B_lo BN x 32 bf16, SWIZZLE_64B); the epilogue writes fp32 rows and/or the (hi, lo) bf16
+// planes the NEXT layer consumes.  Reference op: torch.nn.functional.linear inside HF BertModel (densephrases/encoder.py:101-118).
+#include "gemm_wgmma.cuh"
 #include "../../include/dph_b200.h"
-#include <cuda_bf16.h>
 
-#define BX_BM 128
-#define BX_BK 32                    // bf16 elements per stage row = 64 bytes = one SWIZZLE_64B row
-#define BX_STAGES 4
-#define BX_EPI_WARPS 12
-#define BX_THREADS (128 + 32 * BX_EPI_WARPS)
-#define BX_A_BYTES (BX_BM * BX_BK * 2)          // 8 KB per plane
-#define BX_B_BYTES(BN) ((BN) * BX_BK * 2)       // 16 KB per plane at BN = 256
-#define BX_STAGE_BYTES(BN) (2 * BX_A_BYTES + 2 * BX_B_BYTES(BN))   // 48 KB at BN = 256, 40 KB at BN = 192
-#define BX_MAX_GROUP 2
-// Tile width BN: 256 by default; 192 for N = 768 (the attention-output and FFN-output projections): 2 towers x 32 x 3 = 192 tiles of
-// 128 x 256 fill 148 SMs 1.3 times (65 % of two waves), 256 tiles of 128 x 192 fill them 1.73 times (86 %).
-
-struct BxMaps { CUtensorMap a_hi[BX_MAX_GROUP], a_lo[BX_MAX_GROUP], b_hi[BX_MAX_GROUP], b_lo[BX_MAX_GROUP]; };
-struct BxArgs {
-    const float* bias[BX_MAX_GROUP]; const float* residual[BX_MAX_GROUP];
-    float* out[BX_MAX_GROUP];                       // fp32 result (nullable)
-    __nv_bfloat16* out_hi[BX_MAX_GROUP];            // (hi, lo) planes of the result for the next bf16x3 layer (nullable)
-    __nv_bfloat16* out_lo[BX_MAX_GROUP];
-    int M, N, K, act;
-};
-
-__device__ __forceinline__ void bx_mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+// Tile width BN: 256 by default; 192 when it fills the last wave of the SMs better (N = 768, the attention-output and FFN-output
+// projections: at B = 64, S = 64, 2 towers x 32 x 3 = 192 tiles of 128 x 256 fill 132 SMs 1.45 times (73 % of two waves),
+// 256 tiles of 128 x 192 fill them 1.94 times (97 %)).
 __device__ __forceinline__ void bx_split(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(x);
     lo = __float2bfloat16_rn(x - __bfloat162float(hi));
-}
-
-template <int BX_BN>
-__global__ void __launch_bounds__(BX_THREADS, 1) gemm_bf16x3_persist_kernel(const __grid_constant__ BxMaps maps, const BxArgs args, int tiles_m, int tiles_n,
-                                                                        int total_tiles) {
-    constexpr int BX_STAGE = BX_STAGE_BYTES(BX_BN);
-    constexpr int BX_BB = BX_B_BYTES(BX_BN);
-    constexpr int CHUNKS = BX_BN / 32;                       // 32-column chunks of an accumulator: 8 or 6, shared by three epilogue warp groups
-    extern __shared__ __align__(1024) unsigned char gsm[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    unsigned char* tail = gsm + BX_STAGES * BX_STAGE;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(tail);        // full[4], empty[4], tfull[2], tempty[2]
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(tail + 128);
-    const unsigned full0 = smem_u32(bars), empty0 = smem_u32(bars + BX_STAGES), tfull0 = smem_u32(bars + 2 * BX_STAGES), tempty0 = smem_u32(bars + 2 * BX_STAGES + 2);
-    const unsigned stage0 = smem_u32(gsm);
-    const int num_k = args.K / BX_BK;
-    const int per_group = tiles_m * tiles_n;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.a_hi[0]) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.b_hi[0]) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < BX_STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(tfull0 + 8 * b, 1); mbar_init(tempty0 + 8 * b, BX_EPI_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            unsigned it = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                const int g = t / per_group, r = t - g * per_group, m_blk = r / tiles_n, n_blk = r - m_blk * tiles_n;
-                for (int kb = 0; kb < num_k; kb++, it++) {
-                    const unsigned s = it % BX_STAGES, ph = (it / BX_STAGES) & 1u;
-                    mbar_wait(empty0 + 8 * s, ph ^ 1u);
-                    mbar_expect_tx(full0 + 8 * s, BX_STAGE);
-                    const unsigned dst = stage0 + s * BX_STAGE;
-                    tma_load_2d(dst, &maps.a_hi[g], kb * BX_BK, m_blk * BX_BM, full0 + 8 * s);
-                    tma_load_2d(dst + BX_A_BYTES, &maps.a_lo[g], kb * BX_BK, m_blk * BX_BM, full0 + 8 * s);
-                    tma_load_2d(dst + 2 * BX_A_BYTES, &maps.b_hi[g], kb * BX_BK, n_blk * BX_BN, full0 + 8 * s);
-                    tma_load_2d(dst + 2 * BX_A_BYTES + BX_BB, &maps.b_lo[g], kb * BX_BK, n_blk * BX_BN, full0 + 8 * s);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // instruction descriptor: D = F32 (1 at bit 4), A = B = BF16 (1 at bits 7 and 10), both K-major, N>>3 at bit 17, M>>4 at bit 24
-        const unsigned idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((unsigned)(BX_BN >> 3) << 17) | ((unsigned)(BX_BM >> 4) << 24);
-        unsigned it = 0, i = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, i++) {
-            const unsigned buf = i & 1u, use = i >> 1;
-            mbar_wait(tempty0 + 8 * buf, (use & 1u) ^ 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const unsigned d_tmem = tmem_base + buf * 256u;
-            for (int kb = 0; kb < num_k; kb++, it++) {
-                const unsigned s = it % BX_STAGES, ph = (it / BX_STAGES) & 1u;
-                mbar_wait(full0 + 8 * s, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const unsigned base = stage0 + s * BX_STAGE;
-                    const unsigned long long ahi = make_sw64_desc(base), alo = make_sw64_desc(base + BX_A_BYTES);
-                    const unsigned long long bhi = make_sw64_desc(base + 2 * BX_A_BYTES), blo = make_sw64_desc(base + 2 * BX_A_BYTES + BX_BB);
-#pragma unroll
-                    for (int k = 0; k < BX_BK / 16; k++) {          // UMMA_K = 16 bf16 = 32 bytes: advance the start address inside the swizzle atom
-                        const unsigned long long ko = (unsigned long long)(k * 2);
-                        umma_bf16(d_tmem, ahi + ko, blo + ko, idesc, (kb | k) ? 1u : 0u);      // small cross terms first, then hi.hi
-                        umma_bf16(d_tmem, alo + ko, bhi + ko, idesc, 1u);
-                        umma_bf16(d_tmem, ahi + ko, bhi + ko, idesc, 1u);
-                    }
-                    umma_commit(empty0 + 8 * s);
-                    if (kb == num_k - 1) umma_commit(tfull0 + 8 * buf);
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        const int q = warp & 3;
-        const int eg = (warp >> 2) - 1;
-        const int c_lo = eg * ((CHUNKS + 2) / 3), c_hi = (eg == 2) ? CHUNKS : c_lo + (CHUNKS + 2) / 3;
-        unsigned i = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, i++) {
-            const int g = t / per_group, r = t - g * per_group, m_blk = r / tiles_n, n_blk = r - m_blk * tiles_n;
-            const unsigned buf = i & 1u, use = i >> 1;
-            mbar_wait(tfull0 + 8 * buf, use & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const long long row = (long long)m_blk * BX_BM + q * 32 + lane;
-            const float* bias = args.bias[g];
-            const float* resid = args.residual[g];
-            float* out = args.out[g];
-            __nv_bfloat16* ohi = args.out_hi[g];
-            __nv_bfloat16* olo = args.out_lo[g];
-#pragma unroll 1
-            for (int c = c_lo; c < c_hi; c++) {
-                unsigned v[32];
-                tmem_ld32(tmem_base + ((unsigned)(q * 32) << 16) + buf * 256u + (unsigned)(c * 32), v);
-                if (c == c_hi - 1) {
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) bx_mbar_arrive(tempty0 + 8 * buf);
-                }
-                const int col0 = n_blk * BX_BN + c * 32;
-                if (row < args.M) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 8) {
-                        float o[8];
-#pragma unroll
-                        for (int h = 0; h < 2; h++) {
-                            const float4 b4 = bias ? *reinterpret_cast<const float4*>(bias + col0 + j + 4 * h) : make_float4(0.f, 0.f, 0.f, 0.f);
-                            float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (resid) r4 = *reinterpret_cast<const float4*>(resid + row * args.N + col0 + j + 4 * h);
-                            const float* pb = &b4.x; const float* pr = &r4.x;
-#pragma unroll
-                            for (int e = 0; e < 4; e++) {
-                                float x = __uint_as_float(v[j + 4 * h + e]) + pb[e];
-                                if (args.act == 1) x = 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
-                                o[4 * h + e] = x + pr[e];
-                            }
-                        }
-                        if (out) {
-                            *reinterpret_cast<float4*>(out + row * args.N + col0 + j) = make_float4(o[0], o[1], o[2], o[3]);
-                            *reinterpret_cast<float4*>(out + row * args.N + col0 + j + 4) = make_float4(o[4], o[5], o[6], o[7]);
-                        }
-                        if (ohi) {
-                            __align__(16) __nv_bfloat16 h8[8], l8[8];
-#pragma unroll
-                            for (int e = 0; e < 8; e++) bx_split(o[e], h8[e], l8[e]);
-                            *reinterpret_cast<uint4*>(ohi + row * args.N + col0 + j) = *reinterpret_cast<const uint4*>(h8);
-                            *reinterpret_cast<uint4*>(olo + row * args.N + col0 + j) = *reinterpret_cast<const uint4*>(l8);
-                        }
-                    }
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
 }
 
 // ---- host side ---------------------------------------------------------------------------------------
@@ -225,30 +57,24 @@ int dph_launch_split_bf16(const float* x, void* hi, void* lo, long long n, cudaS
 int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const* A_lo, const void* const* W_hi, const void* const* W_lo,
                            const float* const* bias, const float* const* residual, float* const* out, void* const* out_hi, void* const* out_lo,
                            int M, int N, int K, int act, cudaStream_t st) {
-    DPH_CHECK(group >= 1 && group <= BX_MAX_GROUP, "gemm group size");
-    DPH_CHECK((N % 256 == 0 || N % 192 == 0) && K % BX_BK == 0 && M >= 1, "gemm_bf16x3 needs N % 256 == 0 (or N % 192 == 0) and K % 32 == 0");
-    static DphPerDeviceOnce once;
-    if (once.first()) {
-        DPH_CUDA(cudaFuncSetAttribute(gemm_bf16x3_persist_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, BX_STAGES * BX_STAGE_BYTES(256) + 1024));
-        DPH_CUDA(cudaFuncSetAttribute(gemm_bf16x3_persist_kernel<192>, cudaFuncAttributeMaxDynamicSharedMemorySize, BX_STAGES * BX_STAGE_BYTES(192) + 1024));
-    }
+    DPH_CHECK(group >= 1 && group <= GW_MAX_GROUP, "gemm group size");
+    DPH_CHECK((N % 256 == 0 || N % 192 == 0) && K % GW_BK == 0 && M >= 1, "gemm_bf16x3 needs N % 256 == 0 (or N % 192 == 0) and K % 32 == 0");
     int dev = 0, num_sms = 0;
     DPH_CUDA(cudaGetDevice(&dev));
     DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
     // tile width: the one that wastes less of the last wave (ties -> 256, the higher arithmetic intensity)
-    const int tm = (M + BX_BM - 1) / BX_BM;
+    const int tm = (M + GW_BM - 1) / GW_BM;
     auto waste = [&](int bn) { const long long t = (long long)group * tm * (N / bn); const long long w = (t + num_sms - 1) / num_sms; return (double)(w * num_sms) * bn / ((double)t * bn) ; };
     int BN = 256;
     if (N % 256 != 0 || (N % 192 == 0 && waste(192) + 0.2 < waste(256))) BN = 192;
-    const int smem = BX_STAGES * BX_STAGE_BYTES(BN) + 1024;
-    BxMaps mp;
-    BxArgs ap;
-    for (int g = 0; g < BX_MAX_GROUP; g++) {
+    GwMaps mp;
+    GwArgs ap;
+    for (int g = 0; g < GW_MAX_GROUP; g++) {
         const int s = g < group ? g : 0;
-        DPH_TRY(dph_make_map_bf16(&mp.a_hi[g], A_hi[s], M, K, K, BX_BM));
-        DPH_TRY(dph_make_map_bf16(&mp.a_lo[g], A_lo[s], M, K, K, BX_BM));
-        DPH_TRY(dph_make_map_bf16(&mp.b_hi[g], W_hi[s], N, K, K, BN));
-        DPH_TRY(dph_make_map_bf16(&mp.b_lo[g], W_lo[s], N, K, K, BN));
+        DPH_TRY(dph_make_map_bf16(&mp.a[g], A_hi[s], M, K, K, GW_BM));
+        DPH_TRY(dph_make_map_bf16(&mp.a2[g], A_lo[s], M, K, K, GW_BM));
+        DPH_TRY(dph_make_map_bf16(&mp.b[g], W_hi[s], N, K, K, BN));
+        DPH_TRY(dph_make_map_bf16(&mp.b2[g], W_lo[s], N, K, K, BN));
         ap.bias[g] = bias ? bias[s] : nullptr;
         ap.residual[g] = residual ? residual[s] : nullptr;
         ap.out[g] = out ? out[s] : nullptr;
@@ -256,9 +82,8 @@ int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const
         ap.out_lo[g] = out_lo ? (__nv_bfloat16*)out_lo[s] : nullptr;
     }
     ap.M = M; ap.N = N; ap.K = K; ap.act = act;
-    const int tiles_m = tm, tiles_n = N / BN, total = group * tiles_m * tiles_n;
-    if (BN == 256) gemm_bf16x3_persist_kernel<256><<<total < num_sms ? total : num_sms, BX_THREADS, smem, st>>>(mp, ap, tiles_m, tiles_n, total);
-    else gemm_bf16x3_persist_kernel<192><<<total < num_sms ? total : num_sms, BX_THREADS, smem, st>>>(mp, ap, tiles_m, tiles_n, total);
-    DPH_CUDA(cudaGetLastError());
-    return 0;
+    ap.tiles_m = tm; ap.tiles_n = N / BN; ap.total_tiles = group * tm * ap.tiles_n;
+    const int grid = ap.total_tiles < num_sms ? ap.total_tiles : num_sms;
+    if (BN == 256) return gw_launch<GW_BF16X3, 128, 2, 1, 4>(mp, ap, grid, st);
+    return gw_launch<GW_BF16X3, 192, 1, 1, 4>(mp, ap, grid, st);
 }

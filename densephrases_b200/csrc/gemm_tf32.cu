@@ -1,301 +1,14 @@
-// gemm_tf32.cu -- out[g] = epilogue(A[g] . W[g]^T + bias[g] (+ residual[g]))  on the 5th-gen tensor cores.
+// gemm_tf32.cu -- out[g] = epilogue(A[g] . W[g]^T + bias[g] (+ residual[g])) on the Hopper tensor cores.
 //
-// The dense contractions of the SpanBERT query towers (HF BertModel behind Encoder.embed_query,
-// /root/reference/densephrases/encoder.py:101-118; QKV / attention-output / FFN projections, SURVEY.md Appendix B).
-// fp32 operands in shared memory, tcgen05.mma kind::tf32 (the precision torch 1.9 -- the reference's pin -- used for
-// fp32 matmuls on Ampere+ by default), fp32 accumulators in TMEM.
+// The dense contractions of the SpanBERT query towers (HF BertModel behind Encoder.embed_query, reference
+// densephrases/encoder.py:101-118; QKV / attention-output / FFN projections, SURVEY.md Appendix B).
+// fp32 operands in shared memory, wgmma kind tf32 (the precision torch 1.9 -- the reference's pin -- used for fp32 matmuls on
+// Ampere+ by default), fp32 accumulators in registers; the kernel itself is gemm_wgmma_kernel (gemm_wgmma.cuh).
 //
-// Three schedules of the same MMA sequence (dph_gemm_tf32_set_mode; bit-identical outputs): the tile-per-CTA kernel below (also the
-// 3xTF32 split kernel and, with CL = 2, the multicast-cluster variant) and the persistent 128 x 256 kernel further down (default).
-//
-// Tile per CTA: one CTA computes a 128 x 128 output tile:  warp 0 = TMA producer (cp.async.bulk.tensor, SWIZZLE_128B, 3-stage
-// mbarrier ring), warp 1 = MMA issuer (one elected thread, 4 x UMMA 128x128x8 per 32-float k block), warp 2 = TMEM
-// allocator, warps 4-7 = epilogue (tcgen05.ld 32x32b -> bias / erf-GELU / residual -> 128-byte row segments to global).
-// ~97 KB of shared memory and 128 TMEM columns per CTA -> two CTAs per SM, so one tile's epilogue overlaps the
-// neighbour's main loop.  blockIdx.z selects the problem of a group (the two towers run as one launch).
-#include "umma.cuh"
+// Three schedules of the same wgmma sequence (dph_gemm_tf32_set_mode; bit-identical outputs): one 128 x 128 tile per CTA (also
+// the 3xTF32 split kernel), the same as 2-CTA clusters sharing the A tile by TMA multicast, and persistent 128 x 256 tiles (default).
+#include "gemm_wgmma.cuh"
 #include "../../include/dph_b200.h"
-
-#define GM_BM 128
-#define GM_BN 128
-#define GM_BK 32                   // fp32 elements = 128 bytes = one SWIZZLE_128B row
-#define GM_STAGES 3
-#define GM_TILE_BYTES (GM_BM * GM_BK * 4)                   // 16384 (BM == BN)
-#define GM_MAX_GROUP 2
-
-// SPLIT = 1 ("3xTF32", fp32-accurate): every operand arrives as an exact-TF32 pair (hi, lo) with x ~= hi + lo, and the
-// kernel accumulates hi.hi + hi.lo + lo.hi in the same fp32 TMEM accumulator (the dropped lo.lo term is ~2^-22 relative).
-// a_lo doubles as the 64-row-box map of A in the cluster variant (CL == 2 is only built for SPLIT == 0)
-struct GemmMaps { CUtensorMap a[GM_MAX_GROUP]; CUtensorMap b[GM_MAX_GROUP]; CUtensorMap a_lo[GM_MAX_GROUP]; CUtensorMap b_lo[GM_MAX_GROUP]; };
-struct GemmArgs {
-    const float* bias[GM_MAX_GROUP]; const float* residual[GM_MAX_GROUP]; float* out[GM_MAX_GROUP];
-    int M, N, K, act;     // act: 0 none, 1 erf-GELU
-};
-
-// CL == 2: the two CTAs of a cluster are neighbours along N (same m_blk): each loads HALF of the shared A tile and multicasts it to
-// both, so the cluster reads A from L2 once (24 KB instead of 32 KB of L2 reads per CTA and k block).  A stage may be refilled only
-// when BOTH consumers have released it (empty barriers count CL arrivals, released with a multicast tcgen05.commit).
-template <int SPLIT, int CL>
-__global__ void __launch_bounds__(256, SPLIT ? 1 : 2) gemm_tf32_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs args) {
-    static_assert(CL == 1 || (CL == 2 && SPLIT == 0), "cluster variant: 1xTF32 only");
-    constexpr int GM_STAGE_BYTES = (SPLIT ? 4 : 2) * GM_TILE_BYTES;
-    extern __shared__ __align__(1024) unsigned char gsm[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int g = blockIdx.z, m_blk = blockIdx.y, n_blk = blockIdx.x;
-    unsigned char* tail = gsm + GM_STAGES * GM_STAGE_BYTES;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(tail);        // full[3], empty[3], tmem_full
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(tail + 64);
-    const unsigned full0 = smem_u32(bars), empty0 = smem_u32(bars + GM_STAGES), tmem_full = smem_u32(bars + 2 * GM_STAGES);
-    const unsigned stage0 = smem_u32(gsm);
-    const CUtensorMap* map_a = &maps.a[g];
-    const CUtensorMap* map_b = &maps.b[g];
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(map_a) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(map_b) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < GM_STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, CL); }
-        mbar_init(tmem_full, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(GM_BN) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem_base = *tmem_slot;
-    const int num_k = args.K / GM_BK;
-    unsigned crank = 0;
-    if (CL == 2) { crank = cluster_ctarank(); cluster_sync_all(); }      // peer's barriers are initialised before anything signals them
-
-    if (warp == 0) {
-        if (lane == 0) {
-            for (int kb = 0; kb < num_k; kb++) {
-                const int s = kb % GM_STAGES;
-                const unsigned ph = (kb / GM_STAGES) & 1;
-                mbar_wait(empty0 + 8 * s, ph ^ 1);
-                mbar_expect_tx(full0 + 8 * s, GM_STAGE_BYTES);
-                const unsigned dst = stage0 + s * GM_STAGE_BYTES;
-                if (CL == 2) tma_load_2d_mc(dst + crank * (GM_TILE_BYTES / 2), &maps.a_lo[g], kb * GM_BK, m_blk * GM_BM + (int)crank * (GM_BM / 2), full0 + 8 * s, (unsigned short)3);
-                else tma_load_2d(dst, map_a, kb * GM_BK, m_blk * GM_BM, full0 + 8 * s);
-                tma_load_2d(dst + GM_TILE_BYTES, map_b, kb * GM_BK, n_blk * GM_BN, full0 + 8 * s);
-                if (SPLIT) {
-                    tma_load_2d(dst + 2 * GM_TILE_BYTES, &maps.a_lo[g], kb * GM_BK, m_blk * GM_BM, full0 + 8 * s);
-                    tma_load_2d(dst + 3 * GM_TILE_BYTES, &maps.b_lo[g], kb * GM_BK, n_blk * GM_BN, full0 + 8 * s);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // instruction descriptor: D=F32, A=B=TF32, both K-major, N>>3 at bit 17, M>>4 at bit 24 (cute::UMMA::InstrDescriptor)
-        const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(GM_BN >> 3) << 17) | ((unsigned)(GM_BM >> 4) << 24);
-        for (int kb = 0; kb < num_k; kb++) {
-            const int s = kb % GM_STAGES;
-            const unsigned ph = (kb / GM_STAGES) & 1;
-            mbar_wait(full0 + 8 * s, ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (lane == 0) {
-                const unsigned a_addr = stage0 + s * GM_STAGE_BYTES, b_addr = a_addr + GM_TILE_BYTES;
-                const unsigned long long adesc = make_sw128_desc(a_addr), bdesc = make_sw128_desc(b_addr);
-                const unsigned long long alo = make_sw128_desc(a_addr + 2 * GM_TILE_BYTES), blo = make_sw128_desc(a_addr + 3 * GM_TILE_BYTES);
-#pragma unroll
-                for (int k = 0; k < GM_BK / 8; k++) {       // UMMA_K = 8 tf32 = 32 bytes: advance the start address inside the swizzle atom
-                    const unsigned long long ko = (unsigned long long)(k * 2);
-                    if (SPLIT) {                             // small cross terms first, then the hi.hi term
-                        umma_tf32(tmem_base, adesc + ko, blo + ko, idesc, (kb | k) ? 1u : 0u);
-                        umma_tf32(tmem_base, alo + ko, bdesc + ko, idesc, 1u);
-                        umma_tf32(tmem_base, adesc + ko, bdesc + ko, idesc, 1u);
-                    } else {
-                        umma_tf32(tmem_base, adesc + ko, bdesc + ko, idesc, (kb | k) ? 1u : 0u);
-                    }
-                }
-                if (CL == 2) umma_commit_mc(empty0 + 8 * s, (unsigned short)3);   // frees the stage in both CTAs (each still needs the peer's release)
-                else umma_commit(empty0 + 8 * s);            // frees the stage once these MMAs have read it
-                if (kb == num_k - 1) umma_commit(tmem_full); // accumulator complete
-            }
-            __syncwarp();
-        }
-    } else if (warp >= 4) {
-        const int q = warp & 3;                              // TMEM lane quarter this warp may access
-        mbar_wait(tmem_full, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const long long row = (long long)m_blk * GM_BM + q * 32 + lane;
-        const float* bias = args.bias[g];
-        const float* resid = args.residual[g];
-        float* out = args.out[g];
-#pragma unroll 1
-        for (int c = 0; c < GM_BN / 32; c++) {
-            unsigned v[32];
-            const unsigned taddr = tmem_base + ((unsigned)(q * 32) << 16) + (unsigned)(c * 32);
-            tmem_ld32(taddr, v);
-            const int col0 = n_blk * GM_BN + c * 32;
-            if (row < args.M) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4) {
-                    float4 o;
-                    float* po = &o.x;
-                    const float4 b4 = bias ? *reinterpret_cast<const float4*>(bias + col0 + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-                    const float* pb = &b4.x;
-                    float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (resid) r4 = *reinterpret_cast<const float4*>(resid + row * args.N + col0 + j);
-                    const float* pr = &r4.x;
-#pragma unroll
-                    for (int e = 0; e < 4; e++) {
-                        float x = __uint_as_float(v[j + e]) + pb[e];
-                        if (args.act == 1) x = 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
-                        po[e] = x + pr[e];
-                    }
-                    *reinterpret_cast<float4*>(out + row * args.N + col0 + j) = o;
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(GM_BN) : "memory");
-    if (CL == 2) cluster_sync_all();       // the peer may still multicast into this CTA's shared memory / barriers until it is done too
-}
-
-// ---- persistent variant (1xTF32, N % 256 == 0) ---------------------------------------------------------------------------
-// One CTA per SM walks a static list of 128 x 256 output tiles (tile = blockIdx.x + i * gridDim.x, n fastest so the CTAs that
-// run together share A and B tiles in L2).  Bigger tiles raise the arithmetic intensity of the operand stream from 32 to 43 flop
-// per L2 byte -- the chip-wide L2 -> SM throughput (~12 TB/s) is what bounds fp32-operand tiles, not the tensor pipe -- and the
-// roles never stop: warp 0 keeps the 4-stage TMA ring (48 KB per stage) full across tile boundaries, warp 1 issues
-// tcgen05.mma 128x256x8 into one of TWO 256-column TMEM accumulators, warps 4-15 drain the other one (three warps per TMEM lane quarter, 32-column chunks 0-2 / 3-5 / 6-7) (tcgen05.ld -> bias / GELU /
-// residual -> global), so a tile's epilogue overlaps the next tile's main loop.  Barriers: full/empty per stage, and per
-// accumulator tfull (MMA -> epilogue, tcgen05.commit) / tempty (epilogue -> MMA, one arrive per epilogue warp, 12 in all).
-#define GP_BN 256
-#define GP_STAGES 4
-#define GP_EPI_WARPS 12
-#define GP_THREADS (128 + 32 * GP_EPI_WARPS)
-#define GP_A_BYTES (GM_BM * GM_BK * 4)          // 16 KB
-#define GP_B_BYTES (GP_BN * GM_BK * 4)          // 32 KB
-#define GP_STAGE_BYTES (GP_A_BYTES + GP_B_BYTES)
-struct GemmMapsP { CUtensorMap a[GM_MAX_GROUP]; CUtensorMap b[GM_MAX_GROUP]; };
-
-__device__ __forceinline__ void mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-
-__global__ void __launch_bounds__(GP_THREADS, 1) gemm_tf32_persist_kernel(const __grid_constant__ GemmMapsP maps, const GemmArgs args, int tiles_m, int tiles_n,
-                                                                   int total_tiles) {
-    extern __shared__ __align__(1024) unsigned char gsm[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    unsigned char* tail = gsm + GP_STAGES * GP_STAGE_BYTES;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(tail);        // full[4], empty[4], tfull[2], tempty[2]
-    unsigned* tmem_slot = reinterpret_cast<unsigned*>(tail + 128);
-    const unsigned full0 = smem_u32(bars), empty0 = smem_u32(bars + GP_STAGES), tfull0 = smem_u32(bars + 2 * GP_STAGES), tempty0 = smem_u32(bars + 2 * GP_STAGES + 2);
-    const unsigned stage0 = smem_u32(gsm);
-    const int num_k = args.K / GM_BK;
-    const int per_group = tiles_m * tiles_n;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.a[0]) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.b[0]) : "memory");
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < GP_STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(tfull0 + 8 * b, 1); mbar_init(tempty0 + 8 * b, GP_EPI_WARPS); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            unsigned it = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                const int g = t / per_group, r = t - g * per_group, m_blk = r / tiles_n, n_blk = r - m_blk * tiles_n;
-                for (int kb = 0; kb < num_k; kb++, it++) {
-                    const unsigned s = it % GP_STAGES, ph = (it / GP_STAGES) & 1u;
-                    mbar_wait(empty0 + 8 * s, ph ^ 1u);
-                    mbar_expect_tx(full0 + 8 * s, GP_STAGE_BYTES);
-                    const unsigned dst = stage0 + s * GP_STAGE_BYTES;
-                    tma_load_2d(dst, &maps.a[g], kb * GM_BK, m_blk * GM_BM, full0 + 8 * s);
-                    tma_load_2d(dst + GP_A_BYTES, &maps.b[g], kb * GM_BK, n_blk * GP_BN, full0 + 8 * s);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        const unsigned idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(GP_BN >> 3) << 17) | ((unsigned)(GM_BM >> 4) << 24);
-        unsigned it = 0, i = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, i++) {
-            const unsigned buf = i & 1u, use = i >> 1;
-            mbar_wait(tempty0 + 8 * buf, (use & 1u) ^ 1u);         // the epilogue has drained this accumulator (first use: passes)
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const unsigned d_tmem = tmem_base + buf * GP_BN;
-            for (int kb = 0; kb < num_k; kb++, it++) {
-                const unsigned s = it % GP_STAGES, ph = (it / GP_STAGES) & 1u;
-                mbar_wait(full0 + 8 * s, ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) {
-                    const unsigned a_addr = stage0 + s * GP_STAGE_BYTES;
-                    const unsigned long long adesc = make_sw128_desc(a_addr), bdesc = make_sw128_desc(a_addr + GP_A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < GM_BK / 8; k++)
-                        umma_tf32(d_tmem, adesc + (unsigned long long)(k * 2), bdesc + (unsigned long long)(k * 2), idesc, (kb | k) ? 1u : 0u);
-                    umma_commit(empty0 + 8 * s);
-                    if (kb == num_k - 1) umma_commit(tfull0 + 8 * buf);
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp >= 4) {
-        const int q = warp & 3;                              // TMEM lane quarter; three warps share a quarter: 32-column chunks 0-2 / 3-5 / 6-7 of a tile
-        const int eg = (warp >> 2) - 1;                      // 0: warps 4-7, 1: warps 8-11, 2: warps 12-15
-        const int c_lo = eg * 3, c_hi = (eg == 2) ? 8 : c_lo + 3;
-        unsigned i = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, i++) {
-            const int g = t / per_group, r = t - g * per_group, m_blk = r / tiles_n, n_blk = r - m_blk * tiles_n;
-            const unsigned buf = i & 1u, use = i >> 1;
-            mbar_wait(tfull0 + 8 * buf, use & 1u);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const long long row = (long long)m_blk * GM_BM + q * 32 + lane;
-            const float* bias = args.bias[g];
-            const float* resid = args.residual[g];
-            float* out = args.out[g];
-#pragma unroll 1
-            for (int c = c_lo; c < c_hi; c++) {
-                unsigned v[32];
-                tmem_ld32(tmem_base + ((unsigned)(q * 32) << 16) + buf * GP_BN + (unsigned)(c * 32), v);
-                if (c == c_hi - 1) {                                // this warp's share is read: hand it back before the last stores
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tempty0 + 8 * buf);
-                }
-                const int col0 = n_blk * GP_BN + c * 32;
-                if (row < args.M) {
-#pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        float4 o;
-                        float* po = &o.x;
-                        const float4 b4 = bias ? *reinterpret_cast<const float4*>(bias + col0 + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-                        const float* pb = &b4.x;
-                        float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (resid) r4 = *reinterpret_cast<const float4*>(resid + row * args.N + col0 + j);
-                        const float* pr = &r4.x;
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            float x = __uint_as_float(v[j + e]) + pb[e];
-                            if (args.act == 1) x = 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f));
-                            po[e] = x + pr[e];
-                        }
-                        *reinterpret_cast<float4*>(out + row * args.N + col0 + j) = o;
-                    }
-                }
-            }
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
-}
 
 // ---- host side ---------------------------------------------------------------------------------------
 static dph_PFN_encodeTiled g_encode = nullptr;
@@ -321,9 +34,6 @@ int dph_make_map_f32(CUtensorMap* map, const float* ptr, long long rows, long lo
     DPH_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed");
     return 0;
 }
-// rows x K fp32 row-major matrix -> tensor map with a [GM_BK x 128] box
-static int make_map(CUtensorMap* map, const float* ptr, long long rows, int K) { return dph_make_map_f32(map, ptr, rows, K, K, 128); }
-
 // x -> (hi, lo): hi = round-to-nearest TF32 of x, lo = round-to-nearest TF32 of (x - hi)  (both exact TF32 values)
 __global__ void split_tf32_kernel(const float4* __restrict__ x, float4* __restrict__ hi, float4* __restrict__ lo, long long n4) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -354,76 +64,44 @@ int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const
                            const float* const* bias, const float* const* residual, float* const* out, void* const* out_hi, void* const* out_lo,
                            int M, int N, int K, int act, cudaStream_t st);
 
-// how 1xTF32 GEMMs are scheduled: 0 one 128x128 tile per CTA (2 CTAs/SM); 1 the same as 2-CTA clusters sharing the A tile by TMA
-// multicast (needs an even number of N tiles); 2 persistent 128x256 tiles with double-buffered TMEM (needs N % 256 == 0)
-static int g_gemm_mode = 2;      // measured on the encoder forward (B=64, S=64): mode 0 5.44 ms, mode 1 5.65 ms, mode 2 4.41 ms
+// how 1xTF32 GEMMs are scheduled: 0 one 128x128 tile per CTA; 1 the same as 2-CTA clusters sharing the A tile by TMA multicast
+// (needs an even number of N tiles); 2 persistent 128x256 tiles, one CTA per SM (needs N % 256 == 0)
+static int g_gemm_mode = 2;
 DPH_API int dph_gemm_tf32_set_mode(int mode) { DPH_CHECK(mode >= 0 && mode <= 2, "gemm mode 0..2"); g_gemm_mode = mode; return 0; }
 
 // Grouped launch used by the encoder: problems share M, N, K and the epilogue; pointers are device pointers.
 // A_lo / W_lo non-null -> 3xTF32 mode (A, W are then the hi parts).
 int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W, const float* const* bias, const float* const* residual,
                          float* const* out, int M, int N, int K, int act, cudaStream_t st, const float* const* A_lo, const float* const* W_lo) {
-    DPH_CHECK(group >= 1 && group <= GM_MAX_GROUP, "gemm group size");
-    DPH_CHECK(N % GM_BN == 0 && K % GM_BK == 0 && M >= 1, "gemm_tf32 needs N % 128 == 0 and K % 32 == 0");
+    DPH_CHECK(group >= 1 && group <= GW_MAX_GROUP, "gemm group size");
+    DPH_CHECK(N % 128 == 0 && K % GW_BK == 0 && M >= 1, "gemm_tf32 needs N % 128 == 0 and K % 32 == 0");
     const bool split = A_lo != nullptr && W_lo != nullptr;
-    const int smem_fast = GM_STAGES * 2 * GM_TILE_BYTES + 1024, smem_split = GM_STAGES * 4 * GM_TILE_BYTES + 1024;
-    static DphPerDeviceOnce once;
-    if (once.first()) {
-        DPH_CUDA(cudaFuncSetAttribute(gemm_tf32_kernel<0, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_fast));
-        DPH_CUDA(cudaFuncSetAttribute(gemm_tf32_kernel<0, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_fast));
-        DPH_CUDA(cudaFuncSetAttribute(gemm_tf32_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_split));
-    }
-    const bool cluster = !split && g_gemm_mode == 1 && ((N / GM_BN) % 2 == 0);
-    if (!split && g_gemm_mode == 2 && N % GP_BN == 0) {
-        const int smem_p = GP_STAGES * GP_STAGE_BYTES + 1024;
-        static DphPerDeviceOnce once_p;
-        if (once_p.first()) DPH_CUDA(cudaFuncSetAttribute(gemm_tf32_persist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_p));
-        int dev = 0, num_sms = 0;
-        DPH_CUDA(cudaGetDevice(&dev));
-        DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-        GemmMapsP mp;
-        GemmArgs ap;
-        for (int g = 0; g < GM_MAX_GROUP; g++) {
-            int s = g < group ? g : 0;
-            DPH_TRY(make_map(&mp.a[g], A[s], M, K));
-            DPH_TRY(dph_make_map_f32(&mp.b[g], W[s], N, K, K, GP_BN));
-            ap.bias[g] = bias ? bias[s] : nullptr;
-            ap.residual[g] = residual ? residual[s] : nullptr;
-            ap.out[g] = out[s];
-        }
-        ap.M = M; ap.N = N; ap.K = K; ap.act = act;
-        const int tiles_m = (M + GM_BM - 1) / GM_BM, tiles_n = N / GP_BN, total = group * tiles_m * tiles_n;
-        gemm_tf32_persist_kernel<<<total < num_sms ? total : num_sms, GP_THREADS, smem_p, st>>>(mp, ap, tiles_m, tiles_n, total);
-        DPH_CUDA(cudaGetLastError());
-        return 0;
-    }
-    GemmMaps maps;
-    GemmArgs args;
-    for (int g = 0; g < GM_MAX_GROUP; g++) {
-        int s = g < group ? g : 0;
-        DPH_TRY(make_map(&maps.a[g], A[s], M, K));
-        DPH_TRY(make_map(&maps.b[g], W[s], N, K));
-        if (cluster) DPH_TRY(dph_make_map_f32(&maps.a_lo[g], A[s], M, K, K, GM_BM / 2));
-        else DPH_TRY(make_map(&maps.a_lo[g], split ? A_lo[s] : A[s], M, K));
-        DPH_TRY(make_map(&maps.b_lo[g], split ? W_lo[s] : W[s], N, K));
+    const bool persist = !split && g_gemm_mode == 2 && N % 256 == 0;
+    const bool cluster = !split && g_gemm_mode == 1 && ((N / 128) % 2 == 0);
+    const int BN = persist ? 256 : 128;
+    GwMaps maps;
+    GwArgs args;
+    for (int g = 0; g < GW_MAX_GROUP; g++) {
+        const int s = g < group ? g : 0;
+        DPH_TRY(dph_make_map_f32(&maps.a[g], A[s], M, K, K, GW_BM));
+        DPH_TRY(dph_make_map_f32(&maps.b[g], W[s], N, K, K, BN));
+        if (cluster) DPH_TRY(dph_make_map_f32(&maps.a2[g], A[s], M, K, K, GW_BM / 2));
+        else DPH_TRY(dph_make_map_f32(&maps.a2[g], split ? A_lo[s] : A[s], M, K, K, GW_BM));
+        DPH_TRY(dph_make_map_f32(&maps.b2[g], split ? W_lo[s] : W[s], N, K, K, BN));
         args.bias[g] = bias ? bias[s] : nullptr;
         args.residual[g] = residual ? residual[s] : nullptr;
         args.out[g] = out[s];
+        args.out_hi[g] = nullptr; args.out_lo[g] = nullptr;
     }
     args.M = M; args.N = N; args.K = K; args.act = act;
-    dim3 grid(N / GM_BN, (M + GM_BM - 1) / GM_BM, group);
-    if (split) gemm_tf32_kernel<1, 1><<<grid, 256, smem_split, st>>>(maps, args);
-    else if (!cluster) gemm_tf32_kernel<0, 1><<<grid, 256, smem_fast, st>>>(maps, args);
-    else {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = grid; cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = (size_t)smem_fast; cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        DPH_CUDA(cudaLaunchKernelEx(&cfg, gemm_tf32_kernel<0, 2>, maps, args));
-    }
-    DPH_CUDA(cudaGetLastError());
-    return 0;
+    args.tiles_m = (M + GW_BM - 1) / GW_BM; args.tiles_n = N / BN; args.total_tiles = group * args.tiles_m * args.tiles_n;
+    if (split) return gw_launch<GW_TF32X3, 128, 1, 1, 3>(maps, args, args.total_tiles, st);
+    if (cluster) return gw_launch<GW_TF32, 128, 1, 2, 4>(maps, args, args.total_tiles, st);
+    if (!persist) return gw_launch<GW_TF32, 128, 1, 1, 4>(maps, args, args.total_tiles, st);
+    int dev = 0, num_sms = 0;
+    DPH_CUDA(cudaGetDevice(&dev));
+    DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+    return gw_launch<GW_TF32, 128, 2, 1, 4>(maps, args, args.total_tiles < num_sms ? args.total_tiles : num_sms, st);
 }
 
 // C ABI (test / standalone use): out [M,N] = act(A [M,K] . W[N,K]^T + bias) + residual, device pointers, fp32 in/out.

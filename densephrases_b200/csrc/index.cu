@@ -121,7 +121,7 @@ DPH_API int dph_index_create(dph_index** out, int d, int64_t nlist, int M, int n
     cudaDeviceProp prop;
     DPH_CUDA(cudaGetDeviceProperties(&prop, device));
     ix->num_sms = prop.multiProcessorCount;
-    if (prop.major != 10) { delete ix; dph_set_error("libdph_b200 is built for sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor)); return 1; }
+    if (prop.major != 9 || prop.minor != 0) { delete ix; dph_set_error("libdph_b200 is built for sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor)); return 1; }
     *out = ix;
     return 0;
 }

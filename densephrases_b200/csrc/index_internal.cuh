@@ -40,7 +40,7 @@ struct dph_index {
     int nprobe = 256;
     int scan_mode = DPH_SCAN_FAST;
     cudaStream_t stream = 0;
-    int num_sms = 148;
+    int num_sms = 132;
 
     // model
     float* A = nullptr;         // [d,d]

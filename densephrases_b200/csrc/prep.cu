@@ -1,7 +1,7 @@
 // prep.cu -- query preparation kernels of the IVF-PQ search (everything before the code scan):
 //   * sgemm_nt_seq : out = X W^T with ONE sequential fp32 FMA chain per output (k ascending) -- used for the
 //                    OPQ rotation (faiss LinearTransform::apply) and the coarse scores (IndexFlatIP::search),
-//                    replacing the sgemm faiss calls at /root/reference/densephrases/index.py:200.
+//                    replacing the sgemm faiss calls at reference densephrases/index.py:200.
 //   * coarse_select: top-nprobe lists per query, (score desc, list asc).
 //   * lut          : PQ inner-product tables (faiss ProductQuantizer::compute_inner_prod_table) in two layouts.
 //   * plan         : per (query, probe) segment descriptors + work partition for the scan kernel.
@@ -28,9 +28,8 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_kernel(const float* __restri
     const float4* ap = reinterpret_cast<const float4*>(X + (aok ? arow : 0) * K) + lk4;
     const float4* bp = reinterpret_cast<const float4*>(W + (bok ? brow : 0) * K) + lk4;
     const int tx = tid & 15, ty = tid >> 4;
-    // accumulators as float2 pairs along the output column: one packed FFMA2 (fma.rn.f32x2, two independent IEEE fp32 FMAs)
-    // advances two outputs -- the SIMT fp32 pipe issues a 3-register FFMA every other cycle, so this doubles the FMA rate while
-    // every output still sees exactly one fused multiply-add per k, k ascending (bit-identical to the scalar chain).
+    // accumulators as float2 pairs along the output column (dph_ffma2: two independent IEEE fp32 FMAs): every output sees
+    // exactly one fused multiply-add per k, k ascending (bit-identical to the scalar chain).
     float2 acc[8][4];
 #pragma unroll
     for (int i = 0; i < 8; i++)
@@ -60,7 +59,7 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_kernel(const float* __restri
             for (int i = 0; i < 8; i++) {
                 const float2 a2 = make_float2(a[i], a[i]);
 #pragma unroll
-                for (int j = 0; j < 4; j++) acc[i][j] = __ffma2_rn(a2, b[j], acc[i][j]);
+                for (int j = 0; j < 4; j++) acc[i][j] = dph_ffma2(a2, b[j], acc[i][j]);
             }
         }
         if (kt + 1 < ktiles) {
@@ -107,7 +106,7 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_small_kernel(const float* __
     const float4* ap = reinterpret_cast<const float4*>(X + (aok ? arow : 0) * K) + q4;
     const float4* bp = reinterpret_cast<const float4*>(W + (bok ? brow : 0) * K) + q4;
     const int tx = tid & 15, ty = tid >> 4;
-    float2 acc[4][2];                        // packed FFMA2 along the output column (see sgemm_nt_seq_kernel)
+    float2 acc[4][2];                        // float2 pairs along the output column (see sgemm_nt_seq_kernel)
 #pragma unroll
     for (int i = 0; i < 4; i++) { acc[i][0] = make_float2(0.0f, 0.0f); acc[i][1] = make_float2(0.0f, 0.0f); }
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -137,8 +136,8 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_small_kernel(const float* __
 #pragma unroll
             for (int i = 0; i < 4; i++) {
                 const float2 a2 = make_float2(a[i], a[i]);
-                acc[i][0] = __ffma2_rn(a2, b01, acc[i][0]);
-                acc[i][1] = __ffma2_rn(a2, b23, acc[i][1]);
+                acc[i][0] = dph_ffma2(a2, b01, acc[i][0]);
+                acc[i][1] = dph_ffma2(a2, b23, acc[i][1]);
             }
         }
         if (kt + 1 < ktiles) {
@@ -187,7 +186,7 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_rows_kernel(const float* __r
     const float4* ap = reinterpret_cast<const float4*>(X + (aok ? (row0 + ar) : 0) * K);
     const float4* bp = reinterpret_cast<const float4*>(W + (bok ? (col0 + br) : 0) * K);
     const int tx = tid & 15, ty = tid >> 4;
-    float2 acc[TM][2];                       // float2 pairs along the output column, advanced by packed FFMA2 (see sgemm_nt_seq_kernel)
+    float2 acc[TM][2];                       // float2 pairs along the output column, advanced by dph_ffma2 (see sgemm_nt_seq_kernel)
 #pragma unroll
     for (int i = 0; i < TM; i++) { acc[i][0] = make_float2(0.0f, 0.0f); acc[i][1] = make_float2(0.0f, 0.0f); }
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -227,8 +226,8 @@ __global__ void __launch_bounds__(256) sgemm_nt_seq_rows_kernel(const float* __r
 #pragma unroll
             for (int i = 0; i < TM; i++) {
                 const float2 a2 = make_float2(a[i], a[i]);
-                acc[i][0] = __ffma2_rn(a2, b01, acc[i][0]);
-                acc[i][1] = __ffma2_rn(a2, b23, acc[i][1]);
+                acc[i][0] = dph_ffma2(a2, b01, acc[i][0]);
+                acc[i][1] = dph_ffma2(a2, b23, acc[i][1]);
             }
         }
         if (kt + 1 < ktiles) {
@@ -259,13 +258,16 @@ int dph_launch_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m
     const bool k64 = (K % GRK) == 0;                       // the row-tiled kernels step k by 64
     dim3 grid((unsigned)((m + GBN - 1) / GBN), (unsigned)((n + GBM - 1) / GBM));
     const int variant = g_dph_tune[1];
-    if (variant == 1 || (variant == 0 && (long long)grid.x * grid.y >= 2 * 148)) {
+    int dev = 0, num_sms = 0;
+    DPH_CUDA(cudaGetDevice(&dev));
+    DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+    if (variant == 1 || (variant == 0 && (long long)grid.x * grid.y >= 2 * num_sms)) {
         sgemm_nt_seq_kernel<<<grid, 256, 0, st>>>(X, n, W, m, K, out);
         DPH_CUDA(cudaGetLastError());
         return 0;
     }
-    // pick the LARGEST tile that still gives >= 128 CTAs (measured on B200, tools/bench_variants.py sgemm: n x m = 1024 x 768: 64x64 76 us,
-    // 32x64 87, 16x64 160;  64 x 4096: 32x64 34 us, 64x64 43, 16x64 58;  64 x 768 and 128 x 768: 16x64 31 us, 32x64 33, 64x64 43)
+    // pick the LARGEST tile that still gives >= 128 CTAs: with fewer CTAs than SMs the smaller tiles' extra parallelism outweighs
+    // their lower reuse (compare the variants with tools/bench_variants.py sgemm)
     const long long ct = (m + 63) / 64;
     if (!k64 || variant == 2 || (variant == 0 && ct * ((n + 63) / 64) >= 128)) {
         sgemm_nt_seq_small_kernel<<<dim3((unsigned)ct, (unsigned)((n + 63) / 64)), 256, 0, st>>>(X, n, W, m, K, out);

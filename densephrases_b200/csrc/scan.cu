@@ -1,7 +1,7 @@
 // scan.cu -- the PQ asymmetric-distance scan over the probed inverted lists and the top-k merge.
 //
 // Replaces faiss IVFPQScanner::scan_codes + the result heap behind self.index.search(...) at
-// /root/reference/densephrases/index.py:200 (SURVEY.md 8a-10(iv), Appendix A).
+// reference densephrases/index.py:200 (SURVEY.md 8a-10(iv), Appendix A).
 //
 // Work decomposition: the plan kernel linearises all in-shard (query, probe, 32-vector block) triples in
 // canonical scan order; scan CTA c of G takes the contiguous range [T c/G, T (c+1)/G).  One persistent CTA
@@ -56,7 +56,7 @@ __device__ __forceinline__ void l2_prefetch_block(const void* p) {
 
 extern __shared__ __align__(1024) unsigned char dph_smem[];
 // The dynamic shared memory window of a kernel without static shared memory starts at this shared-space address on
-// sm_100 (1 KB is reserved by the system); probed once at library init (dph_scan_setup_attrs), a mismatch is fatal.
+// sm_90 (1 KB is reserved by the system); probed once at library init (dph_scan_setup_attrs), a mismatch is fatal.
 #define DPH_DYN_SMEM_BASE 0x400
 
 // One FAST lookup: PRMT builds (cta window bits | code << 8 | lane*4); the table base, the step offset and the window
@@ -66,16 +66,16 @@ template <int IMM> __device__ __forceinline__ float lds_imm(unsigned addr) {
     asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(v) : "r"(addr), "n"(IMM));
     return v;
 }
-// The four running sums live in two float2 registers and advance with packed FADD2 (add.rn.f32x2: two independent IEEE fp32 adds per
-// instruction) -- the same per-component summation order as four scalar accumulators, half the FP32-pipe instructions.
+// The four running sums live in two float2 registers (dph_fadd2: two independent IEEE fp32 adds) -- the same per-component
+// summation order as four scalar accumulators.
 template <int T0> __device__ __forceinline__ void fast_word(unsigned wv, unsigned y, float2& a01, float2& a23) {
     constexpr int TB = DPH_DYN_SMEM_BASE + (T0 >> 5) * 65536 + (T0 & 31) * 4;   // T0 % 4 == 0: the 4 bytes share a table
     const float v0 = lds_imm<TB + 0>(__byte_perm(wv, y, 0x7504));
     const float v1 = lds_imm<TB + 4>(__byte_perm(wv, y, 0x7514));
     const float v2 = lds_imm<TB + 8>(__byte_perm(wv, y, 0x7524));
     const float v3 = lds_imm<TB + 12>(__byte_perm(wv, y, 0x7534));
-    a01 = __fadd2_rn(a01, make_float2(v0, v1));
-    a23 = __fadd2_rn(a23, make_float2(v2, v3));
+    a01 = dph_fadd2(a01, make_float2(v0, v1));
+    a23 = dph_fadd2(a23, make_float2(v2, v3));
 }
 template <int C> __device__ __forceinline__ void fast_chunk(const uint4& v, unsigned y, float2& a01, float2& a23) {
     fast_word<C * 16 + 0>(v.x, y, a01, a23);

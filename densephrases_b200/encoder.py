@@ -1,11 +1,11 @@
-"""Encoder: query-side forward of the DensePhrases encoder on the B200 tensor cores.
+"""Encoder: query-side forward of the DensePhrases encoder on the H100 tensor cores.
 
-Mirror of the query path of /root/reference/densephrases/encoder.py (class Encoder): `embed_query` (:101-118) and
+Mirror of the query path of reference densephrases/encoder.py (class Encoder): `embed_query` (:101-118) and
 `forward(input_ids_=..., attention_mask_=..., token_type_ids_=..., return_query=True)` (:146-152) -> (query_start,
 query_end), each [B,1,768], computed by two independent BERT-base towers whose weights come from the
 `query_start_encoder.*` / `query_end_encoder.*` entries of the reference state dict (legacy names `bert_q_start.*` /
 `bert_q_end.*` are accepted like single_utils.backward_compat, :36-56).  The phrase tower, the filter head and the
-training losses are out of scope (SURVEY.md 8a).  Compute: libdph_b200 (tcgen05 kind::tf32 GEMMs, fp32 everything else)."""
+training losses are out of scope (SURVEY.md 8a).  Compute: libdph_b200 (wgmma TF32 / bf16 GEMMs, fp32 everything else)."""
 import ctypes as C
 
 import numpy as np
@@ -133,7 +133,7 @@ class Encoder(object):
     def forward(self, input_ids=None, attention_mask=None, token_type_ids=None, input_ids_=None, attention_mask_=None, token_type_ids_=None,
                 return_phrase=False, return_query=False, **unused):
         if input_ids is not None or not return_query:
-            raise NotImplementedError('only the query-side path (return_query=True, encoder.py:146-152) is on the B200 hot path')
+            raise NotImplementedError('only the query-side path (return_query=True, encoder.py:146-152) is on the GPU hot path')
         assert len(input_ids_.size()) == 2
         return self.embed_query(input_ids_, attention_mask_, token_type_ids_)
 

@@ -1,6 +1,6 @@
 """IvfPqIndex: Python handle over the C-ABI index (include/dph_b200.h).
 
-Mirrors the slice of the faiss Python API that /root/reference/densephrases/index.py uses on the hot path:
+Mirrors the slice of the faiss Python API that reference densephrases/index.py uses on the hot path:
 ``search(x, k) -> (D, I)`` (index.py:200), ``reconstruct`` (index.py:31,286,296), ``ntotal``, ``d``, ``nprobe``
 (index.py:33,53,62), the OPQ matrix (index.py:32).  numpy in -> numpy out through the C ABI with host buffers;
 torch CUDA tensors in -> torch CUDA tensors out (device pointers, asynchronous on the current stream)."""

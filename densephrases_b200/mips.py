@@ -1,6 +1,6 @@
-"""MIPS -- the phrase-index runtime of DensePhrases on the B200-native IVF-PQ index.
+"""MIPS -- the phrase-index runtime of DensePhrases on the H100-native IVF-PQ index.
 
-API mirror of the reference class `MIPS` (/root/reference/densephrases/index.py:23-482): same constructor and
+API mirror of the reference class `MIPS` (reference densephrases/index.py:23-482): same constructor and
 `search(...)` signature, same result dictionaries, same tolerance of missing ids / out-of-range labels, so the
 reference's callers (eval_phrase_retrieval.evaluate :57-77, DensePhrases.search model.py:82-87,
 train_query.get_top_phrases :187-201) work on top of it.  The internals are written for batches, not items:

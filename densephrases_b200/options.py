@@ -1,4 +1,4 @@
-"""Options: flag-compatible subset of /root/reference/densephrases/options.py (:20-251) for the retrieval hot path --
+"""Options: flag-compatible subset of reference densephrases/options.py (:20-251) for the retrieval hot path --
 every flag `eval_phrase_retrieval.py`, `DensePhrases.__init__` (model.py:30-43) and the Makefile eval targets
 (Makefile:169-181) pass is accepted with the reference's default; training/dump-only flags are accepted and ignored."""
 import argparse

@@ -1,8 +1,8 @@
 /*
- * dph_b200.h -- C ABI of libdph_b200.so: the B200-native replacement for the FAISS calls on the
+ * dph_b200.h -- C ABI of libdph_b200.so: the H100-native (sm_90a) replacement for the FAISS calls on the
  * DensePhrases retrieval hot path.  Plain pointers and sizes only (no torch / faiss types).
  *
- * Every entry point names the reference interface it replaces (paths relative to /root/reference):
+ * Every entry point names the reference interface it replaces (paths relative to the reference DensePhrases repository):
  *
  *   dph_index_search            <- faiss.IndexPreTransform.search(x, k)      densephrases/index.py:200
  *   dph_index_reconstruct_batch <- faiss IndexIVFPQ.reconstruct(id) per id   densephrases/index.py:31,282-300
@@ -159,8 +159,8 @@ int dph_encoder_set_precision(dph_encoder* e, int precise);
  * MMAs per contraction (fp32-accurate) in modes 1 and 2; fp32 accumulation and softmax.  0: always the fp32 SIMT attention kernels. */
 int dph_encoder_set_attention(dph_encoder* e, int tensor_core);
 /* One BERT-base self-attention (12 heads x 64; HF BertSelfAttention as used by encoder.py:101-118) on device buffers:
- * qkv fp32 [B*S, 2304] = (Q | K | V), mask int64 [B,S] -> ctx fp32 [B*S, 768].  tensor_core: 0 SIMT fp32, 1 tcgen05 TF32,
- * 2 tcgen05 on bf16 (hi, lo) operand planes, three MMAs per contraction (fp32-accurate); 1 and 2 need S <= 64. */
+ * qkv fp32 [B*S, 2304] = (Q | K | V), mask int64 [B,S] -> ctx fp32 [B*S, 768].  tensor_core: 0 SIMT fp32, 1 wgmma TF32,
+ * 2 wgmma on bf16 (hi, lo) operand planes, three MMAs per contraction (fp32-accurate); 1 and 2 need S <= 64. */
 int dph_attention_bert(const float* qkv, const int64_t* attention_mask, int B, int S, float* ctx, int tensor_core, void* cuda_stream);
 /* input_ids / attention_mask / token_type_ids int64 [B,S] (S <= 384); start_out / end_out fp32 [B,768] = hidden state at
  * position 0 of each tower (the reference returns them as [B,1,768]). */
@@ -171,16 +171,15 @@ int dph_encoder_embed_query(dph_encoder* e, const int64_t* input_ids, const int6
  * acc = fmaf(x[t], w[t], acc) for t ascending; device pointers; K % 32 == 0.  Used for the OPQ rotation and the coarse quantizer. */
 int dph_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m, int64_t K, float* out, void* cuda_stream);
 
-/* ---- dense fp32 GEMM on the tcgen05 tensor cores (kind::tf32), the encoder's building block ----
+/* ---- dense fp32 GEMM on the Hopper tensor cores (wgmma tf32), the encoder's building block ----
  * out [M,N] = act(A [M,K] . W [N,K]^T + bias [N]) + residual [M,N]; act: 0 none, 1 erf-GELU; device pointers;
  * N % 128 == 0, K % 32 == 0.  == torch.nn.functional.linear (HF BertSelfAttention/BertOutput/BertIntermediate). */
 int dph_gemm_tf32_nt(const float* A, const float* W, const float* bias, const float* residual, float* out, int64_t M, int64_t N,
                      int64_t K, int act, int precise /* 0: 1xTF32, 1: 3xTF32 split (fp32-accurate), 2: bf16x3 split (N % 256 == 0) */,
                      void* cuda_stream);
 /* Scheduling of the 1xTF32 GEMMs (process-wide; every mode issues the same MMAs in the same order -> bit-identical results):
- * 0: one 128x128 tile per CTA, two CTAs per SM;  1: the same as 2-CTA thread-block clusters sharing the A tile through TMA
- * multicast (N/128 even);  2 (default): persistent CTAs walking 128x256 tiles with double-buffered TMEM accumulators and twelve
- * epilogue warps (N % 256 == 0, else mode 0). */
+ * 0: one 128x128 tile per CTA;  1: the same as 2-CTA thread-block clusters sharing the A tile through TMA multicast (N/128 even);
+ * 2 (default): one persistent CTA per SM walking 128x256 tiles (N % 256 == 0, else mode 0). */
 int dph_gemm_tf32_set_mode(int mode);
 /* Measurement hook (process-wide): choose between kernel variants that compute bit-identical results, for A/B timing on hardware
  * (tools/bench_variants.py).  knob 0: additions of the quad scan issued on the FMA pipe (0 none .. 3 all; default 1);

@@ -1,9 +1,9 @@
 """oracle/encoder_ref.py -- TEST INFRASTRUCTURE.  Plain PyTorch fp32 restatement of the query-tower forward
 (HF BertModel, transformers 2.9.0 semantics, SURVEY.md Appendix B) used by Encoder.embed_query
-(/root/reference/densephrases/encoder.py:101-118).  It is pinned against the reference class itself:
-tests/golden/make_encoder_golden.py imports /root/reference/densephrases/encoder.py in the build container, runs it on
+(reference densephrases/encoder.py:101-118).  It is pinned against the reference class itself:
+tests/golden/make_encoder_golden.py imports the reference densephrases/encoder.py, runs it on
 seeded weights/inputs and stores the outputs; tests/test_encoder.py checks this restatement against those fixtures, so it
-can stand in for the reference on the GPU box (where /root/reference does not exist)."""
+can stand in for the reference wherever the reference repository is not present."""
 import math
 
 import torch

@@ -3,12 +3,12 @@
  *
  * CPU restatement of the search arithmetic DensePhrases delegates to FAISS:
  *   faiss.IndexPreTransform(OPQMatrix(768,96), IndexIVFPQ(IndexFlatIP(768), 768, nlist, 96, 8, IP))
- * built at /root/reference/build_phrase_index.py:113-116, searched at
- * /root/reference/densephrases/index.py:200 (self.index.search) and reconstructed from at
- * /root/reference/densephrases/index.py:31,286,296 (reconst_fn).
+ * built at reference build_phrase_index.py:113-116, searched at
+ * reference densephrases/index.py:200 (self.index.search) and reconstructed from at
+ * reference densephrases/index.py:31,286,296 (reconst_fn).
  *
  * The algorithm lives in the un-vendored third-party dependency faiss-gpu==1.6.5
- * (/root/reference/requirements.txt:2); it is restated here from its published algorithm
+ * (reference requirements.txt:2); it is restated here from its published algorithm
  * (IndexPreTransform::search -> LinearTransform::apply -> IndexIVF::search ->
  *  IndexFlatIP coarse top-nprobe -> IVFPQScanner<IP, CMin, PQDecoder8>::scan_codes with
  *  precompute_mode 2 -> heap_pop/heap_push/heap_reorder), see SURVEY.md Appendix A.

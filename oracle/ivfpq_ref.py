@@ -4,7 +4,7 @@ Two things live here:
 
 1. ``CRef`` / ``RefIndex``: ctypes binding of ``oracle/ivfpq_ref.c`` (the primary, OpenMP, bit-exact
    CPU restatement of the FAISS ``IndexPreTransform(OPQ) -> IndexIVFPQ(IP, by_residual)`` search that
-   /root/reference/densephrases/index.py:200 calls, and of ``reconstruct`` at index.py:31,286,296).
+   reference densephrases/index.py:200 calls, and of ``reconstruct`` at index.py:31,286,296).
 2. A *numpy* restatement of the same algorithm (``np_*`` functions; pure-Python heap loops, small cases
    only) plus an exhaustive fp64 scorer. tests/test_oracle.py holds the C and numpy versions to
    bit-equality and both to the fp64 brute force.

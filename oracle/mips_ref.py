@@ -1,5 +1,5 @@
 """oracle/mips_ref.py -- TEST INFRASTRUCTURE.  Item-by-item restatement of the reference's phrase stage
-(/root/reference/densephrases/index.py:220-448: search_phrase + aggregate_results) over the oracle IVF-PQ index,
+(reference densephrases/index.py:220-448: search_phrase + aggregate_results) over the oracle IVF-PQ index,
 written the way the reference runs it (one reconstruct per id, one validity test per candidate, python sorting) so the
 batched product implementation (densephrases_b200/mips.py) can be compared result-by-result.
 PINNED against the reference itself: tests/golden/mips_search.json holds the outputs of the UNMODIFIED reference `MIPS.search`

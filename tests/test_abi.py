@@ -25,7 +25,7 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_no_cpu_fallback_without_gpu():
-    """The product path must fail loudly when there is no B200 (no silent CPU fallback)."""
+    """The product path must fail loudly when there is no H100 (no silent CPU fallback)."""
     import pytest
     import torch
     if torch.cuda.is_available():

@@ -6,16 +6,30 @@ import os
 import numpy as np
 import pytest
 
+HERE = os.path.dirname(os.path.abspath(__file__))
+TRUECASE_DIST = os.path.join(HERE, "golden", "truecase.dist")
+
+
+def reference_golden():
+    """Outputs of the unmodified reference code on the inputs below (tests/golden/make_api_golden.py)."""
+    return json.load(open(os.path.join(HERE, "golden", "api_reference.json")))
+
+
+def as_json(x):
+    """The value as it reads back from the golden JSON file (tuples -> lists, numpy scalars -> Python numbers)."""
+    return json.loads(json.dumps(x, sort_keys=True, default=lambda v: v.item() if isinstance(v, np.generic) else str(v)))
+
 
 def test_reference_eval_script_imports_against_facade():
-    ref = "/root/reference/eval_phrase_retrieval.py"
-    if not os.path.exists(ref):
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib.util
-    spec = importlib.util.spec_from_file_location("ref_eval_phrase_retrieval", ref)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)                       # executes its `import faiss`, `from densephrases... import ...` lines (:12,:19-25)
-    assert callable(mod.evaluate) and callable(mod.embed_all_query)
+    """Every `import faiss` / `from densephrases... import ...` line of the reference eval_phrase_retrieval.py (:12,:19-25, recorded
+    in the golden file) resolves against this repository's facade."""
+    import importlib
+    imports = reference_golden()["imports"]
+    assert any(m == "faiss" for m, _ in imports) and any(m == "densephrases" for m, _ in imports)
+    for module, names in imports:
+        mod = importlib.import_module(module)
+        for n in names:
+            assert getattr(mod, n) is not None, (module, n)
     import faiss
     with pytest.raises(RuntimeError):
         faiss.read_index
@@ -157,28 +171,17 @@ def test_metrics_match_reference_golden():
         assert bool(R.drqa_metric_max_over_ground_truths(R.drqa_exact_match_score, c["prediction"], c["truths"])) == c["em"]
 
 
-def test_unmodified_reference_evaluate_runs_on_the_facade(tmp_path):
-    """The reference's own `eval_phrase_retrieval.evaluate` (:49-91) + `evaluate_results` (:94-204), UNMODIFIED, executed over this
-    repo's drop-in surface: `Options`, `load_qa_pairs`, `get_query2vec` (+ tokenizer) and the metric functions come from the
-    `densephrases` facade; only the phrase index and the encoder are CPU stand-ins with the documented call signatures.  Its
-    numbers equal densephrases_b200.runtime.evaluate on the same inputs (the reference reports percentages)."""
-    ref = "/root/reference/eval_phrase_retrieval.py"
-    if not os.path.exists(ref):
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib.util
+def reference_evaluate_inputs(tmp):
+    """Options, canned MIPS / encoder stand-ins with the documented call signatures and the tokenizer the evaluate loop runs on."""
     import torch
     from densephrases import Options
-    from densephrases_b200 import runtime as R
     from densephrases_b200.tokenization import WordPieceTokenizer
-    spec = importlib.util.spec_from_file_location("ref_eval_phrase_retrieval_run", ref)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
     qa = [("which river crosses the city", ["the Seine", "Seine"]), ("who signed the treaty", ["Louis XIV"]), ("what year", ["1648", "in 1648"]),
           ("where", ["Paris"]), ("what is the a an the", ["yes"])]
-    json.dump({"data": [{"id": str(i), "question": q, "answers": a} for i, (q, a) in enumerate(qa)]}, open(tmp_path / "test.json", "w"))
+    json.dump({"data": [{"id": str(i), "question": q, "answers": a} for i, (q, a) in enumerate(qa)]}, open(os.path.join(tmp, "test.json"), "w"))
     o = Options()
     o.add_model_options(); o.add_index_options(); o.add_retrieval_options(); o.add_data_options()
-    args = o.parse(["--test_path", str(tmp_path / "test.json"), "--load_dir", str(tmp_path), "--top_k", "3", "--eval_batch_size", "2", "--save_pred"])
+    args = o.parse(["--test_path", os.path.join(tmp, "test.json"), "--load_dir", str(tmp), "--top_k", "3", "--eval_batch_size", "2", "--save_pred"])
     canned = {"which river crosses the city": ["Seine", "Loire"], "who signed the treaty": ["Louis XV", "Louis XIV", "x"], "what year": [],
               "where": ["paris.", "Lyon"], "what is the a an the": ["no", "Yes!"]}
 
@@ -199,41 +202,32 @@ def test_unmodified_reference_evaluate_runs_on_the_facade(tmp_path):
             return [[{"answer": a, "context": "ctx " + a, "title": ["T"], "score": 10.0 - j, "start_pos": 4, "end_pos": 4 + len(a)}
                      for j, a in enumerate(canned[q])] for q in q_texts]
 
-    tok = WordPieceTokenizer.from_pretrained_or_synthetic(None)
-    em1, f11, emk, f1k = mod.evaluate(args, mips=FakeMips(), query_encoder=FakeEncoder(), tokenizer=tok)
-    mine = R.evaluate(args, mips=FakeMips(), query_encoder=FakeEncoder(), tokenizer=tok)
-    assert (em1, f11, emk, f1k) == pytest.approx((100 * mine["exact_match_top1"], 100 * mine["f1_score_top1"], 100 * mine["exact_match_top3"],
-                                                  100 * mine["f1_score_top3"]))
-    assert em1 == pytest.approx(40.0) and emk == pytest.approx(80.0)
-    pred = json.load(open(tmp_path / "pred" / "test_5_top3.pred"))                       # written by the reference (:187-196)
-    assert pred["1"]["prediction"] == canned["who signed the treaty"] and pred["2"]["prediction"] == [""]
+    return args, FakeMips(), FakeEncoder(), WordPieceTokenizer.from_pretrained_or_synthetic(None)
 
 
-@pytest.mark.parametrize("unit", ["phrase", "sentence", "paragraph", "document"])
-def test_densephrases_search_wrapper_equals_unmodified_reference_class(oracle, unit):
-    """model.py:55-109 (`DensePhrases.search`: query2vec -> stacked vectors -> MIPS.search with the unit's aggregation -> field
-    selection) run UNMODIFIED over this repo's MIPS / query2vec gives exactly what densephrases_b200's DensePhrases.search returns."""
-    ref_path = "/root/reference/densephrases/model.py"
-    if not os.path.exists(ref_path):
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib.util
-    import sys
-    import types
+def test_unmodified_reference_evaluate_runs_on_the_facade(tmp_path):
+    """The reference's own `eval_phrase_retrieval.evaluate` (:49-91) + `evaluate_results` (:94-204), UNMODIFIED, executed over this
+    repo's drop-in surface (`Options`, `load_qa_pairs`, `get_query2vec` + tokenizer, the metric functions; only the phrase index
+    and the encoder are CPU stand-ins) produced the golden numbers and prediction file; densephrases_b200.runtime.evaluate on the
+    same inputs gives the same numbers (the reference reports percentages)."""
+    from densephrases_b200 import runtime as R
+    want = reference_golden()["evaluate"]
+    args, mips, enc, tok = reference_evaluate_inputs(str(tmp_path))
+    mine = R.evaluate(args, mips=mips, query_encoder=enc, tokenizer=tok)
+    assert (want["em1"], want["f1_1"], want["emk"], want["f1_k"]) == pytest.approx(
+        (100 * mine["exact_match_top1"], 100 * mine["f1_score_top1"], 100 * mine["exact_match_top3"], 100 * mine["f1_score_top3"]))
+    assert want["em1"] == pytest.approx(40.0) and want["emk"] == pytest.approx(80.0)
+    assert want["pred"]["1"]["prediction"] == ["Louis XV", "Louis XIV", "x"] and want["pred"]["2"]["prediction"] == [""]
+
+
+def search_wrapper_setup(oracle, obj):
+    """Give a DensePhrases object (ours or the reference class) this repo's query2vec and a MIPS over the oracle index; returns the questions."""
     import torch
-    from densephrases import DensePhrases, Options
+    from densephrases import Options
     from densephrases_b200 import runtime as R
     from densephrases_b200.mips import MIPS
     from densephrases_b200.tokenization import WordPieceTokenizer
     from tests.test_mips import OracleIndexAdapter, build
-    stub = types.ModuleType("densephrases.utils.squad_utils")
-    stub.TrueCaser = type("TrueCaser", (), {})
-    sys.modules["densephrases.utils.squad_utils"] = stub
-    try:
-        spec = importlib.util.spec_from_file_location("ref_densephrases_model", ref_path)
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-    finally:
-        del sys.modules["densephrases.utils.squad_utils"]
     doc_groups, idx_f, _, ref, query = build(oracle)
     mips = MIPS.from_components(OracleIndexAdapter(ref), idx_f, doc_groups, cuda=False)
     qvec = torch.from_numpy(query.astype(np.float32))
@@ -246,84 +240,81 @@ def test_densephrases_search_wrapper_equals_unmodified_reference_class(oracle, u
     o = Options()
     o.add_model_options(); o.add_index_options(); o.add_retrieval_options(); o.add_data_options()
     args = o.parse([])
-    q2v = R.get_query2vec(query_encoder=FakeEncoder(), tokenizer=WordPieceTokenizer.from_pretrained_or_synthetic(None), args=args, batch_size=64)
-    theirs, ours = mod.DensePhrases.__new__(mod.DensePhrases), DensePhrases.__new__(DensePhrases)
-    for obj in (theirs, ours):
-        obj.query2vec, obj.mips, obj.truecase, obj.args = q2v, mips, None, args
-    qs = ["first question", "second question", "third"]
-    a = theirs.search(qs, retrieval_unit=unit, top_k=3, truecase=False, return_meta=True)
+    obj.query2vec = R.get_query2vec(query_encoder=FakeEncoder(), tokenizer=WordPieceTokenizer.from_pretrained_or_synthetic(None), args=args, batch_size=64)
+    obj.mips, obj.truecase, obj.args = mips, None, args
+    return ["first question", "second question", "third"]
+
+
+def strip_vectors(rets):
+    return [[{k: v for k, v in r.items() if k not in ("start_vec", "end_vec")} for r in ret] for ret in rets]
+
+
+@pytest.mark.parametrize("unit", ["phrase", "sentence", "paragraph", "document"])
+def test_densephrases_search_wrapper_equals_unmodified_reference_class(oracle, unit):
+    """model.py:55-109 (`DensePhrases.search`: query2vec -> stacked vectors -> MIPS.search with the unit's aggregation -> field
+    selection) run UNMODIFIED over this repo's MIPS / query2vec gave the golden results; densephrases_b200's DensePhrases.search
+    returns exactly the same."""
+    from densephrases import DensePhrases
+    want = reference_golden()["search"][unit]
+    ours = DensePhrases.__new__(DensePhrases)
+    qs = search_wrapper_setup(oracle, ours)
     b = ours.search(qs, retrieval_unit=unit, top_k=3, truecase=False, return_meta=True)
-    assert a[0] == b[0] and len(a[0]) == 3 and all(len(x) <= 3 for x in a[0])
-    strip = lambda rets: [[{k: v for k, v in r.items() if k not in ("start_vec", "end_vec")} for r in ret] for ret in rets]
-    assert strip(a[1]) == strip(b[1])
-    assert theirs.search(qs[0], retrieval_unit=unit, top_k=2, truecase=False) == ours.search(qs[0], retrieval_unit=unit, top_k=2, truecase=False)
+    assert len(want["results"]) == 3 and all(len(x) <= 3 for x in want["results"])
+    assert as_json(b[0]) == want["results"]
+    assert as_json(strip_vectors(b[1])) == want["meta"]
+    assert as_json(ours.search(qs[0], retrieval_unit=unit, top_k=2, truecase=False)) == want["single"]
 
 
-def test_open_utils_and_single_utils_helpers_equal_unmodified_reference(tmp_path):
-    """`load_qa_pairs` (open_utils.py:103-163) and `backward_compat` (single_utils.py:36-56), the reference's code loaded by path
-    (its imports of squad_utils / embed_utils -- not on this path -- stubbed), against the facade's versions on awkward inputs."""
-    if not os.path.exists("/root/reference/densephrases/utils/open_utils.py"):
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib.util
-    import sys
-    import types
-    from densephrases.utils import open_utils as mine_open, single_utils as mine_single
-    stubs = {"densephrases.utils.squad_utils": ("get_question_dataloader", "TrueCaser"), "densephrases.utils.embed_utils": ("get_question_results",)}
-    for name, attrs in stubs.items():
-        m = types.ModuleType(name)
-        for a in attrs:
-            setattr(m, a, object)
-        sys.modules[name] = m
-    try:
-        mods = {}
-        for short in ("single_utils", "open_utils"):
-            spec = importlib.util.spec_from_file_location(f"ref_{short}", f"/root/reference/densephrases/utils/{short}.py")
-            mods[short] = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mods[short])
-    finally:
-        for name in stubs:
-            del sys.modules[name]
+QA_PAIR_CASES = [(False, None), (True, None), (False, 1), (False, 3)]
+BACKWARD_COMPAT_SD = {"bert_q_start.embeddings.w": 1, "bert_q_end.x": 2, "bert_start.y": 3, "cross_encoder.z": 4, "bert_qd.q": 5, "qa_outputs.w": 6,
+                      "query_start_encoder.k": 7, "linear.weight": 8}
+
+
+class QaArgs:
+    do_lower_case, draft, truecase, truecase_path = False, False, False, ""
+
+
+def write_qa_pairs_input(tmp):
     data = {"data": [{"id": "a1", "question": "Which river?", "answers": ["Seine"]},
                      {"id": "a2", "origin": "nq.dev.x", "question": "who signed it", "answers": ["Louis", "Anne"], "titles": ["T1", "T2"]},
                      {"id": "a3", "question": "skipped", "answers": []},
                      {"id": "a4", "question": "x" * 400 + " [START_ENT] Paris [END_ENT] " + "y" * 400 + "?", "answers": ["Paris"]},
                      {"id": "a5", "question": "ALL CAPS?", "answers": ["x"]}]}
-    p = tmp_path / "qa.json"
+    p = os.path.join(tmp, "qa.json")
     json.dump(data, open(p, "w"))
+    return p
 
-    class Args:
-        do_lower_case, draft, truecase, truecase_path = False, False, False, ""
 
-    for lower, q_idx in [(False, None), (True, None), (False, 1), (False, 3)]:
-        Args.do_lower_case = lower
-        want = mods["open_utils"].load_qa_pairs(str(p), Args, q_idx=q_idx)
-        got = mine_open.load_qa_pairs(str(p), Args, q_idx=q_idx)
-        assert [list(x) for x in got] == [list(x) for x in want]
-    sd = {"bert_q_start.embeddings.w": 1, "bert_q_end.x": 2, "bert_start.y": 3, "cross_encoder.z": 4, "bert_qd.q": 5, "qa_outputs.w": 6,
-          "query_start_encoder.k": 7, "linear.weight": 8}
-    assert mine_single.backward_compat(sd) == mods["single_utils"].backward_compat(sd)
+def test_open_utils_and_single_utils_helpers_equal_unmodified_reference(tmp_path):
+    """`load_qa_pairs` (open_utils.py:103-163) and `backward_compat` (single_utils.py:36-56): the facade's versions give what the
+    reference's code (loaded by path, its imports of squad_utils / embed_utils stubbed) gave on the same awkward inputs."""
+    from densephrases.utils import open_utils as mine_open, single_utils as mine_single
+    g = reference_golden()
+    p = write_qa_pairs_input(str(tmp_path))
+    for (lower, q_idx), want in zip(QA_PAIR_CASES, g["load_qa_pairs"]):
+        QaArgs.do_lower_case = lower
+        got = mine_open.load_qa_pairs(p, QaArgs, q_idx=q_idx)
+        assert as_json([list(x) for x in got]) == want
+    QaArgs.do_lower_case = False
+    assert as_json(mine_single.backward_compat(dict(BACKWARD_COMPAT_SD))) == g["backward_compat"]
+
+
+OPTIONS_ARGV = ["--cuda", "--top_k", "40", "--nprobe", "64", "--index_name", "start/1048576_flat_OPQ96", "--eval_batch_size", "32", "--agg_strat", "opt2"]
 
 
 def test_option_flags_and_defaults_equal_reference_parser():
     """Every flag of the four option groups eval_phrase_retrieval.py / model.py add (options.py: model, index, retrieval, data)
-    exists here with the same default; nothing is renamed."""
-    if not os.path.exists("/root/reference/densephrases/options.py"):
-        pytest.skip("reference tree not present (GPU box)")
-    import importlib.util
+    exists here with the same default as the reference parser; nothing is renamed."""
     from densephrases import Options
-    spec = importlib.util.spec_from_file_location("ref_options", "/root/reference/densephrases/options.py")
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    theirs, ours = mod.Options(), Options()
+    g = reference_golden()
+    ours = Options()
     for group in ("add_model_options", "add_index_options", "add_retrieval_options", "add_data_options"):
-        getattr(theirs, group)()
         getattr(ours, group)()
-    want, got = vars(theirs.parser.parse_args([])), vars(ours.parse([]))
-    assert not [k for k in want if k not in got]
+    want, got = g["options_defaults"], as_json(vars(ours.parse([])))
+    assert len(want) > 20 and not [k for k in want if k not in got]
     assert {k: got[k] for k in want} == want
-    argv = ["--cuda", "--top_k", "40", "--nprobe", "64", "--index_name", "start/1048576_flat_OPQ96", "--eval_batch_size", "32", "--agg_strat", "opt2"]
-    got2 = vars(ours.parse(argv))
-    assert {k: got2[k] for k in want} == vars(theirs.parser.parse_args(argv))
+    got2 = as_json(vars(ours.parse(OPTIONS_ARGV)))
+    assert {k: got2[k] for k in want} == g["options_argv"]
 
 
 def test_synthetic_dump_spec_objects(tmp_path):
@@ -401,41 +392,35 @@ def test_load_qa_pairs_truecases_lower_case_questions(tmp_path, monkeypatch, cap
     assert qs2[0] == "who is the president of france " and "truecase.dist" in capsys.readouterr().out
 
 
-def test_truecaser_differential_against_the_reference_class():
-    """In the build container the reference tree is present: run the UNMODIFIED `TrueCaser` source (cut out of squad_utils.py with
-    `ast`, like tests/golden/make_truecase_golden.py) next to ours on fresh random sentences -- every output string and every score
-    must be equal.  (On the GPU box the tree does not exist; the committed golden file covers that case.)"""
-    ref_file = "/root/reference/densephrases/utils/squad_utils.py"
-    if not os.path.exists(ref_file):
-        pytest.skip("reference tree not present (GPU box)")
-    import ast, math, pickle, random, string, tempfile
-    from collections import defaultdict
-    from densephrases_b200.truecase import TrueCaser
+def truecase_differential_inputs(tables):
+    """Seeded random sentences x OOV modes, and (prev, token, next) score queries, over the vocabulary of the statistics file."""
+    import random
+    rng = random.Random(12345)
+    vocab = list(tables["word_casing_lookup"]) + ["zzz", "o'brien", "42", "?", ",", "'s", "x-ray", "Ünïcode", "a.b"]
+    cases = []
+    for _ in range(400):
+        s = " ".join(rng.choice(vocab) for _ in range(rng.randint(0, 12)))
+        s = rng.choice([s, s.upper(), s.title(), "  " + s + " "])
+        cases += [(s, oov) for oov in ("title", "lower", "as-is")]
+    multi = [w for w, c in tables["word_casing_lookup"].items() if len(c) > 1]
+    scores = []
+    for _ in range(300):
+        tok = rng.choice(tables["word_casing_lookup"][rng.choice(multi)])
+        scores.append((rng.choice([None] + vocab), tok, rng.choice([None] + vocab)))
+    return cases, scores
 
-    def cut(path, name):
-        src = open(path).read()
-        node = next(n for n in ast.parse(src).body if getattr(n, "name", None) == name)
-        return ast.get_source_segment(src, node)
-    ns = {"os": os, "pickle": pickle, "math": math, "string": string}
-    exec(cut("/root/reference/densephrases/utils/data_utils.py", "whitespace_tokenize"), ns)
-    exec(cut(ref_file, "TrueCaser"), ns)
-    here = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "truecase.dist")
-    tables = pickle.load(open(here, "rb"))
-    with tempfile.NamedTemporaryFile(suffix=".dist", delete=False) as f:      # the reference indexes its count tables with []
-        pickle.dump({k: (defaultdict(int, v) if k != "word_casing_lookup" else v) for k, v in tables.items()}, f)
-    try:
-        ref, ours = ns["TrueCaser"](f.name), TrueCaser(here)
-        rng = random.Random(12345)
-        vocab = list(tables["word_casing_lookup"]) + ["zzz", "o'brien", "42", "?", ",", "'s", "x-ray", "Ünïcode", "a.b"]
-        for _ in range(400):
-            s = " ".join(rng.choice(vocab) for _ in range(rng.randint(0, 12)))
-            s = rng.choice([s, s.upper(), s.title(), "  " + s + " "])
-            for oov in ("title", "lower", "as-is"):
-                assert ours.get_true_case(s, oov) == ref.get_true_case(s, oov), (s, oov)
-        multi = [w for w, c in tables["word_casing_lookup"].items() if len(c) > 1]
-        for _ in range(300):
-            tok = rng.choice(tables["word_casing_lookup"][rng.choice(multi)])
-            prev, nxt = rng.choice([None] + vocab), rng.choice([None] + vocab)
-            assert ours.get_score(prev, tok, nxt) == ref.get_score(prev, tok, nxt)
-    finally:
-        os.unlink(f.name)
+
+def test_truecaser_differential_against_the_reference_class():
+    """The UNMODIFIED reference `TrueCaser` (cut out of squad_utils.py with `ast`, tests/golden/make_api_golden.py) was run on seeded
+    random sentences; every output string and every score of ours must be equal to what it gave."""
+    import pickle
+    from densephrases_b200.truecase import TrueCaser
+    want = reference_golden()["truecase"]
+    tables = pickle.load(open(TRUECASE_DIST, "rb"))
+    cases, scores = truecase_differential_inputs(tables)
+    assert len(want["cases"]) == len(cases) == 1200 and len(want["scores"]) == len(scores) == 300
+    ours = TrueCaser(TRUECASE_DIST)
+    for (s, oov), w in zip(cases, want["cases"]):
+        assert ours.get_true_case(s, oov) == w, (s, oov)
+    for x, w in zip(scores, want["scores"]):
+        assert ours.get_score(*x) == w, x

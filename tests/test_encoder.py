@@ -2,7 +2,7 @@
 tests/golden/make_encoder_golden.py) -> committed fixture tests/golden/encoder_query.npz -> (CPU test) the torch fp32
 restatement oracle/encoder_ref.py reproduces it -> (GPU tests) the CUDA encoder is compared with both.
 
-Tolerance (written here as the north star asks): the CUDA towers run their GEMMs on tcgen05 kind::tf32 (10-bit mantissa
+Tolerance (written here as the north star asks): the CUDA towers run their GEMMs on wgmma tf32 (10-bit mantissa
 operands, fp32 accumulate; everything else fp32).  Against the fp32 reference the [CLS] vectors (|x| ~ 0.8) differ by
 ~1e-3; we assert max |diff| < 5e-2 (observed 1-2e-2 over 98k outputs with std-0.04 random weights) and cosine > 0.9995 per vector."""
 import os
@@ -118,7 +118,7 @@ def test_cuda_encoder_bf16x3_meets_the_north_star_tolerance(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("B,S", [(5, 64), (3, 24), (2, 8), (7, 37)])
 def test_tensor_core_attention_matches_simt_attention(B, S):
-    """attention_tc.cu (tcgen05 TF32 QK^T and PV, S <= 64, padded / ragged masks) against the fp32 SIMT attention kernels inside the
+    """attention_tc.cu (wgmma TF32 QK^T and PV, S <= 64, padded / ragged masks) against the fp32 SIMT attention kernels inside the
     same encoder: the only difference is TF32 rounding of Q, K, P, V operands -> [CLS] vectors within 2e-2, cosine > 0.9999."""
     from densephrases_b200.encoder import BertGeometry, Encoder, random_state_dict, synthetic_query_batch
     geo = BertGeometry(vocab_size=2000)
@@ -135,7 +135,7 @@ def test_tensor_core_attention_matches_simt_attention(B, S):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("tensor_core,tol", [(0, 2e-5), (1, 1e-2), (2, 1e-4)])      # SIMT fp32 | tcgen05 TF32 | tcgen05 bf16 (hi, lo) planes
+@pytest.mark.parametrize("tensor_core,tol", [(0, 2e-5), (1, 1e-2), (2, 1e-4)])      # SIMT fp32 | wgmma TF32 | wgmma bf16 (hi, lo) planes
 @pytest.mark.parametrize("B,S", [(3, 64), (4, 20)])
 def test_attention_kernels_against_torch(B, S, tensor_core, tol):
     """One BERT self-attention (12 heads x 64) through the C ABI against torch fp32: softmax(QK^T/8 + (1-mask)*-1e4) V."""

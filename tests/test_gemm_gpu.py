@@ -1,4 +1,4 @@
-"""tcgen05 TF32 GEMM (densephrases_b200/csrc/gemm_tf32.cu) vs a plain PyTorch fp32 reference of the same op.
+"""wgmma TF32 GEMM (densephrases_b200/csrc/gemm_tf32.cu) vs a plain PyTorch fp32 reference of the same op.
 Tolerance: TF32 keeps 10 mantissa bits of each operand (rel. 2^-11 per product), accumulation is fp32; for K <= 3072 and
 unit-scale operands |err| <= 2e-3 * sqrt(K) * scale is comfortably loose; we assert a relative Frobenius error < 1e-3."""
 import ctypes as C
@@ -66,7 +66,7 @@ def test_gemm_tf32_matches_torch_fp32(M, N, K, variant):
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("M,N,K", [(4096, 768, 768), (333, 2304, 768), (64, 3072, 768), (1000, 256, 3072), (20000, 768, 96)])
 def test_gemm_schedules_are_bit_identical(M, N, K, mode):
-    """mode 1 (2-CTA clusters sharing the A tile by TMA multicast) and mode 2 (persistent 128x256 tiles, double-buffered TMEM)
+    """mode 1 (2-CTA clusters sharing the A tile by TMA multicast) and mode 2 (persistent 128x256 tiles, one CTA per SM)
     issue the same MMAs per output element in the same order as mode 0 (one 128x128 tile per CTA)."""
     import torch
     from densephrases_b200 import _lib as L
@@ -90,7 +90,7 @@ def test_gemm_schedules_are_bit_identical(M, N, K, mode):
                                    (333, 768, 768)])
 @pytest.mark.parametrize("variant", ["plain", "bias_gelu", "bias_resid"])
 def test_gemm_bf16x3_matches_fp64(M, N, K, variant):
-    """gemm_bf16x3.cu: fp32 operands carried as (hi, lo) bf16 planes, a_hi.b_lo + a_lo.b_hi + a_hi.b_hi in an fp32 TMEM accumulator.
+    """gemm_bf16x3.cu: fp32 operands carried as (hi, lo) bf16 planes, a_hi.b_lo + a_lo.b_hi + a_hi.b_hi in an fp32 register accumulator.
     Representation error 2^-18 per operand + the dropped lo.lo term 2^-18 -> relative Frobenius error well below 2e-5 (1xTF32: ~3e-4,
     torch fp32: ~1e-7); operands that are exact in two bf16 planes (16 mantissa bits) must reproduce the fp32 product to rounding."""
     import torch

@@ -282,7 +282,7 @@ def test_long_rows_chunked_select_both_coarse_paths(oracle, nprobe):
 
 @pytest.mark.parametrize("nprobe", [8, 256])
 def test_tensor_core_coarse_is_bit_identical(oracle, nprobe):
-    """Coarse quantizer on tcgen05 (3xTF32 candidates + exact re-rank + proof) == SIMT sequential-k path == oracle (probes AND scores)."""
+    """Coarse quantizer on the tensor cores (3xTF32 candidates + exact re-rank + proof) == SIMT sequential-k path == oracle (probes AND scores)."""
     nlist = 1024
     lens = np.full(nlist, 40, dtype=np.int64)
     ref, gpu = make_pair(oracle, nlist, lens)

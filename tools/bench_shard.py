@@ -1,4 +1,4 @@
-"""One rank of BASELINE.json configs[3] (C4): 1B phrases, IVF65536,PQ96, 8 list-range shards, batch 1024 -- measured on ONE B200
+"""One rank of BASELINE.json configs[3] (C4): 1B phrases, IVF65536,PQ96, 8 list-range shards, batch 1024 -- measured on ONE GPU
 by building shard 0 only (125M phrases, 12 GB) and timing the rank-local work of a sharded search with the protocol the product
 picks for the shape (densephrases_b200.sharded.use_query_split):
     query-split (C4):  coarse_split (this rank's 128 queries over all 65536 centroids)  +  search_assigned (LUT, plan, scan, merge)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Convert a DensePhrases release (index.faiss + idx2id.hdf5 + meta_compressed.pkl) into the containers densephrases_b200.MIPS reads
 (index.dph.npz + idx2id.npz + meta_dph.pkl).  Run this ONCE on a machine that still has the reference's dependencies
-(faiss, h5py, blosc -- requirements.txt of princeton-nlp/DensePhrases); the B200 serving path itself needs none of them.
+(faiss, h5py, blosc -- requirements.txt of princeton-nlp/DensePhrases); the GPU serving path itself needs none of them.
 
     python tools/convert_reference_artifacts.py $SAVE_DIR/densephrases-multi_wiki-20181220/dump start/1048576_flat_OPQ96 [--verify]
 

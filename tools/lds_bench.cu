@@ -1,5 +1,6 @@
-// tools/lds_bench.cu -- microbenchmark: what shared-memory gather rate can one SM sustain on B200?
-// (design input for scan.cu; run on the GPU box:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/lds_bench tools/lds_bench.cu && /tmp/lds_bench)
+// tools/lds_bench.cu -- microbenchmark: what shared-memory gather rate can one SM sustain on H100?
+// (design input for scan.cu:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o lds_bench tools/lds_bench.cu && ./lds_bench)
+#define NSM 132            // SMs of an H100 SXM: one CTA per SM
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -102,16 +103,16 @@ __global__ void __launch_bounds__(512, 1) k_stream(float* out, int iters, long l
 }
 template <class K> void run_stream(const char* name, K kern, int nthreads, int iters, const uint4* gbuf, long long nblk) {
     const int smem = 200 * 1024;
-    float* out; long long* cyc; cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 148 * 8);
+    float* out; long long* cyc; cudaMalloc(&out, NSM * 1024 * 4); cudaMalloc(&cyc, NSM * 8);
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    kern<<<148, nthreads, smem>>>(out, 10, cyc, gbuf, nblk);
+    kern<<<NSM, nthreads, smem>>>(out, 10, cyc, gbuf, nblk);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0); kern<<<148, nthreads, smem>>>(out, iters, cyc, gbuf, nblk); cudaEventRecord(e1); cudaDeviceSynchronize();
+    cudaEventRecord(e0); kern<<<NSM, nthreads, smem>>>(out, iters, cyc, gbuf, nblk); cudaEventRecord(e1); cudaDeviceSynchronize();
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    long long h[148]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
-    double avg = 0; for (int i = 0; i < 148; i++) avg += h[i]; avg /= 148;
+    long long h[NSM]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
+    double avg = 0; for (int i = 0; i < NSM; i++) avg += h[i]; avg /= NSM;
     double lookups = 96.0 * iters * nthreads;
-    double gbs = 148.0 * iters * (nthreads / 32) * 3072.0 / (ms * 1e-3) / 1e9;
+    double gbs = (double)NSM * iters * (nthreads / 32) * 3072.0 / (ms * 1e-3) / 1e9;
     printf("%-34s threads=%4d  warp-gathers/clk/SM=%.3f  %.0f GB/s (cycles %.0f, %.3f ms, err=%s)\n", name, nthreads, lookups / 32.0 / avg, gbs, avg, ms, cudaGetErrorString(cudaGetLastError()));
     cudaFree(out); cudaFree(cyc);
 }
@@ -133,14 +134,14 @@ __global__ void __launch_bounds__(1024, 1) k_pure(float* out, int iters, long lo
     if (threadIdx.x == 0) cyc[blockIdx.x] = t1 - t0;
 }
 template <class K> void run(const char* name, K kern, int nthreads, int iters, double per_iter_lookups_per_thread, int smem) {
-    float* out; long long* cyc; cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 148 * 8);
+    float* out; long long* cyc; cudaMalloc(&out, NSM * 1024 * 4); cudaMalloc(&cyc, NSM * 8);
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    kern<<<148, nthreads, smem>>>(out, 10, cyc);
+    kern<<<NSM, nthreads, smem>>>(out, 10, cyc);
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    cudaEventRecord(e0); kern<<<148, nthreads, smem>>>(out, iters, cyc); cudaEventRecord(e1); cudaDeviceSynchronize();
+    cudaEventRecord(e0); kern<<<NSM, nthreads, smem>>>(out, iters, cyc); cudaEventRecord(e1); cudaDeviceSynchronize();
     float ms; cudaEventElapsedTime(&ms, e0, e1);
-    long long h[148]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
-    double avg = 0; for (int i = 0; i < 148; i++) avg += h[i]; avg /= 148;
+    long long h[NSM]; cudaMemcpy(h, cyc, sizeof(h), cudaMemcpyDeviceToHost);
+    double avg = 0; for (int i = 0; i < NSM; i++) avg += h[i]; avg /= NSM;
     double lookups = per_iter_lookups_per_thread * iters * nthreads;
     printf("%-28s threads=%4d  warp-gathers/clk/SM=%.3f  (cycles %.0f, %.3f ms, err=%s)\n", name, nthreads, lookups / 32.0 / avg, avg, ms, cudaGetErrorString(cudaGetLastError()));
     cudaFree(out); cudaFree(cyc);
