@@ -73,6 +73,11 @@ _SIGS = {
     "dph_encoder_set_attention": (_i32, [_vp, _i32]),
     "dph_attention_bert": (_i32, [_vp, _vp, _i32, _i32, _vp, _i32, _vp]),
     "dph_index_window_scores": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _i32]),
+    "dph_index_encode": (_i32, [_vp, _vp, _i64, _vp, _vp, _i32]),
+    "dph_index_add_with_ids": (_i32, [_vp, _vp, _i64, _vp, _i32]),
+    "dph_index_copy_lists": (_i32, [_vp, _vp, _vp]),
+    "dph_index_get_list_len": (_i32, [_vp, _vp]),
+    "dph_index_last_add_ms": (_i32, [_vp, _vp]),
 }
 EXPORTS = tuple(_SIGS)
 

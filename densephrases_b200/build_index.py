@@ -8,7 +8,17 @@ Procrustes update of the rotation), k-means coarse quantizer with inner-product 
 each vector to the centroid of MAXIMUM inner product), PQ trained on RESIDUALS (by_residual=True) and encoded by nearest codeword
 in L2 per 8-dim sub-vector.  Plain PyTorch (CPU or CUDA) -- this is an offline tool; its outputs are exactly the arrays
 IvfPqIndex.from_arrays consumes.  Randomness is seeded; faiss' own random initialisations are not reproduced (trained indexes are
-equivalent in kind, not bit-identical to a faiss-trained one)."""
+equivalent in kind, not bit-identical to a faiss-trained one).
+
+Filling an index on the GPU (the add_with_ids of build_phrase_index.py:145-150,156-279, with the exact fp32 encoding of DESIGN.md 3.1):
+    A, centroids, pq = train_index(x_train, nlist)
+    ix = IvfPqIndex.from_arrays(A, centroids, pq, np.zeros(nlist, np.int64), np.zeros((0, 96), np.uint8))   # trained, empty
+    for x, ids in chunks:                        # numpy or CUDA tensors; ids None -> ntotal + arange(n)
+        ix.add_with_ids(x, ids)
+    list_len, codes, ids = ix.lists()            # list-major, what set_lists takes
+    artifacts.write_faiss_index(path, A, centroids, pq, list_len, codes, ids)
+add_to_index below is the PyTorch encoder that runs without a GPU; its argmax / argmin have no fixed floating-point order, so on
+ties and near-ties it may pick other lists or codewords than IvfPqIndex.encode."""
 import numpy as np
 import torch
 

@@ -58,6 +58,7 @@ struct dph_index {
     int64_t* dm_ids = nullptr;
     int64_t* dm_rows = nullptr;
     int64_t dm_n = 0;
+    int64_t dm_cap = -1;                // entries allocated for dm_ids / dm_rows (-1: as set_lists sized them, ntotal_local)
     std::vector<int64_t> h_list_len;    // host copies
     std::vector<int64_t> h_list_start;
     int64_t bytes = 0;
@@ -67,7 +68,8 @@ struct dph_index {
         work, Dp, Ip, Gp, Dh, Ih, eps, nseg,
         lutmin, lutmaxv, lutq, qparams, gdense, pl_cnt, pl_fill, pl_off, pl_blockpre, pl_entries, pl_unitpre, pl_units, pl_udesc, pairwork,
         csplit, xsplit, candkeys, cflags, selkeys, recbuf,
-        rb_ids, rb_out, rb_found, ws_q, ws_id, ws_out, ws_xq;        // reconstruct_batch / window_scores staging (host-buffer calls)
+        rb_ids, rb_out, rb_found, ws_q, ws_id, ws_out, ws_xq,        // reconstruct_batch / window_scores staging (host-buffer calls)
+        enc_key, enc_cd, enc_list, enc_codes;                        // encode / add: top-1 coarse result, host-call output staging
     int64_t csplit_lo = -1, csplit_nl = -1;
     int coarse_tc = 1;                 // tensor-core coarse quantizer with exact re-rank (0: always the SIMT sequential-k GEMM)
     int64_t last_n = 0;
@@ -76,6 +78,8 @@ struct dph_index {
     bool profile = false;              // CUDA events around the scan kernel of the last search chunk
     cudaEvent_t ev0[DPH_PROF_RING] = {}, ev1[DPH_PROF_RING] = {};
     int64_t prof_n = 0;
+    cudaEvent_t aev[6] = {};           // profiled adds: stage boundaries (encode.cu, index.cu)
+    float add_ms[4] = {};              // last add: rotation, coarse, PQ encode, re-layout + scatter (ms)
 };
 
 // process-wide variant selection (dph_set_tuning, measurement hook): [0] quad-scan IMAD level, [1] SGEMM tile
@@ -98,3 +102,6 @@ int dph_launch_scan(dph_index* ix, int64_t n, int k, int keep, int mode, int gri
 int dph_launch_merge(dph_index* ix, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,
                      uint32_t* G, cudaStream_t st);
 int dph_scan_setup_attrs();
+// ---- encode.cu ----
+int64_t dph_encode_chunk(const dph_index* ix);
+int dph_encode_rows(dph_index* ix, const float* x_dev, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad);

@@ -74,6 +74,75 @@ class IvfPqIndex:
         list_len = np.ascontiguousarray(list_len, dtype=np.int64)
         L.check(L.lib().dph_index_set_lists_synthetic(self._h, _np_ptr(list_len), seed))
 
+    # ---- growing the index (faiss add_with_ids, build_phrase_index.py:145-150) --------------------
+    def _rows(self, x):
+        if len(x.shape) != 2 or x.shape[1] != self.d:
+            raise RuntimeError(f"expected vectors of shape [n, {self.d}], got {tuple(x.shape)}")
+        return int(x.shape[0])
+
+    def encode(self, x):
+        """Assign + encode without changing the index: numpy [n,d] -> (list_no [n] i64, codes [n,96] u8) numpy | torch cuda -> torch
+        cuda.  Bit-identical to the oracle's ref_encode (DESIGN.md 3, "Growing the index")."""
+        if isinstance(x, np.ndarray):
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            n = self._rows(x)
+            list_no = np.empty(n, dtype=np.int64)
+            codes = np.empty((n, 96), dtype=np.uint8)
+            L.check(L.lib().dph_index_encode(self._h, _np_ptr(x), n, _np_ptr(list_no), _np_ptr(codes), L.MEM_HOST))
+            return list_no, codes
+        import torch
+        assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+        n = self._rows(x)
+        list_no = torch.empty(n, dtype=torch.int64, device=x.device)
+        codes = torch.empty((n, 96), dtype=torch.uint8, device=x.device)
+        self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
+        L.check(L.lib().dph_index_encode(self._h, x.data_ptr(), n, list_no.data_ptr(), codes.data_ptr(), L.MEM_DEVICE))
+        return list_no, codes
+
+    def add_with_ids(self, x, ids):
+        """== faiss index.add_with_ids(x, ids): append x [n,d] (numpy or torch cuda) with labels ids [n] (None: ntotal + arange(n))
+        to their lists, in input order.  Raises RuntimeError, leaving the index unchanged, on a negative label, a non-finite value,
+        a shape mismatch or too little device memory for the re-layout."""
+        if isinstance(x, np.ndarray):
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            n = self._rows(x)
+            if ids is not None:
+                ids = np.ascontiguousarray(np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids), dtype=np.int64)
+                if ids.shape != (n,):
+                    raise RuntimeError(f"ids has shape {ids.shape}, expected ({n},)")
+            L.check(L.lib().dph_index_add_with_ids(self._h, _np_ptr(x), n, None if ids is None else _np_ptr(ids), L.MEM_HOST))
+            return
+        import torch
+        assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+        n = self._rows(x)
+        if ids is not None:
+            ids = torch.as_tensor(ids, dtype=torch.int64).to(x.device).contiguous()
+            if tuple(ids.shape) != (n,):
+                raise RuntimeError(f"ids has shape {tuple(ids.shape)}, expected ({n},)")
+        self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
+        L.check(L.lib().dph_index_add_with_ids(self._h, x.data_ptr(), n, None if ids is None else ids.data_ptr(), L.MEM_DEVICE))
+
+    def add(self, x):
+        """== faiss index.add(x): labels ntotal + arange(n)."""
+        self.add_with_ids(x, None)
+
+    def lists(self):
+        """-> (list_len [nlist] i64 of ALL lists, codes [ntotal_local,96] u8, ids [ntotal_local] i64): this shard's lists, list-major
+        (the arrays set_lists / from_arrays / artifacts.write_faiss_index take)."""
+        list_len = np.empty(self.nlist, dtype=np.int64)
+        L.check(L.lib().dph_index_get_list_len(self._h, _np_ptr(list_len)))
+        n = self.ntotal_local
+        codes = np.empty((n, 96), dtype=np.uint8)
+        ids = np.empty(n, dtype=np.int64)
+        L.check(L.lib().dph_index_copy_lists(self._h, _np_ptr(codes), _np_ptr(ids)))
+        return list_len, codes, ids
+
+    def last_add_ms(self):
+        """With set_profile(True): stage times of the last add in ms (rotation, coarse, PQ encode, re-layout + scatter)."""
+        out = np.zeros(4, dtype=np.float32)
+        L.check(L.lib().dph_index_last_add_ms(self._h, _np_ptr(out)))
+        return out
+
     # ---- attributes ---------------------------------------------------------------------------
     @property
     def ntotal(self):

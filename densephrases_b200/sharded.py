@@ -142,6 +142,12 @@ class ShardedIvfPq:
         ix.set_lists(list_len, codes[off[lo]:off[hi]], None if ids is None else ids[off[lo]:off[hi]])
         return self
 
+    def add_with_ids(self, x, ids=None):
+        """== faiss index.add_with_ids (build_phrase_index.py:145-150); a collective by convention like search: every rank passes the
+        same batch.  No exchange is needed: assignment is deterministic and the coarse quantizer is replicated, so every rank derives
+        the same global list lengths and labels (ids None -> ntotal + arange(n)) and stores the rows of its own lists."""
+        self.local.add_with_ids(x, ids)
+
     # ---- the slice of the faiss index API that MIPS uses (index.py:30-33,200,286,296) ----
     @property
     def ntotal(self):

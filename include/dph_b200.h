@@ -11,6 +11,9 @@
  *   dph_index_set_nprobe        <- index_ivf.nprobe = 256                    densephrases/index.py:53,62
  *   dph_index_create/set_*      <- faiss.read_index(...) / IndexPreTransform(OPQMatrix, IndexIVFPQ(...))
  *                                  densephrases/index.py:30 ; build_phrase_index.py:113-116,149-150
+ *   dph_index_add_with_ids      <- index.add_with_ids(vectors, ids)          build_phrase_index.py:145-150,156-279
+ *   dph_index_encode            <- the assignment + PQ encoding inside add_with_ids (IndexIVFPQ::encode_vectors)
+ *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
  *
  * Conventions: every function returns 0 on success, non-zero on error (dph_last_error() gives the
  * message; the Python layer raises RuntimeError like faiss' SWIG layer does).  `mem` arguments say
@@ -60,6 +63,28 @@ int dph_index_set_shard(dph_index* ix, int64_t list_lo, int64_t list_hi);
 int dph_index_set_lists(dph_index* ix, const int64_t* list_len, const uint8_t* codes, const int64_t* ids);
 /* Same but codes are generated on device from `seed` (bit-identical to oracle ref_gen_codes); ids sequential. */
 int dph_index_set_lists_synthetic(dph_index* ix, const int64_t* list_len, uint64_t seed);
+
+/* ---- growing the index (replaces index.add_with_ids, build_phrase_index.py:145-150,156-279; DESIGN.md 3 "Growing the index") ----
+ * Encoding is IndexPreTransform(OPQ) -> IndexIVFPQ (by_residual) with a fixed fp32 order, bit-identical to the oracle's ref_encode:
+ * rotation, top-1 coarse list (smallest list id on a tie), fp32 residual, per sub-quantizer squared-L2 as one fmaf chain, lowest
+ * codeword on a tie.  Needs the OPQ matrix, centroids and PQ codebooks.  Uses the search workspace: dph_index_last_xr is not kept. */
+/* x [n,d] -> list_no_out [n] int64, codes_out [n,96] uint8 (m ascending); the index is not modified. */
+int dph_index_encode(dph_index* ix, const float* x, int64_t n, int64_t* list_no_out, uint8_t* codes_out, int mem);
+/* Append x [n,d] with labels ids [n] (NULL -> ntotal + i, like IndexIVF::add) to their lists, in input order; needs set_lists first
+ * (all-zero list lengths give an empty, trained index).  The device state afterwards is byte-identical to set_lists of the
+ * concatenated list-major arrays.  On a shard, rows of lists outside [list_lo, list_hi) only count into the list lengths: every rank
+ * that adds the same batch reaches the same global state.  An index with sequential labels turns them into explicit ones.  A label
+ * added twice is found at every row that carries it; reconstruct returns the most recent row (faiss' hashtable direct map), except
+ * for a label repeated across shards, which reconstruct leaves undefined.  Rejected, with the index unchanged: a negative label, a
+ * non-finite input value, too little device memory for the old and the new code buffers at once.  Synchronises the stream. */
+int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem);
+/* This shard's lists as list-major host arrays: codes_out [ntotal_local,96], ids_out [ntotal_local] (may be NULL); the inverse of
+ * set_lists, for writing a grown index back to a faiss file (artifacts.write_faiss_index). */
+int dph_index_copy_lists(dph_index* ix, uint8_t* codes_out, int64_t* ids_out);
+/* list_len_out [nlist] (host): the length of every list, all shards. */
+int dph_index_get_list_len(const dph_index* ix, int64_t* list_len_out);
+/* Measurement hook: with profiling on, the stage times of the last add in ms: rotation, coarse, PQ encode, re-layout + scatter. */
+int dph_index_last_add_ms(const dph_index* ix, float* ms_out /* [4] */);
 
 /* ---- getters ---- */
 int64_t dph_index_ntotal(const dph_index* ix);       /* all shards */

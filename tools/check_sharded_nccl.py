@@ -1,4 +1,5 @@
-"""Both sharded-search protocols on real NCCL ranks against the unsharded search of the same index (bit-identical D and I):
+"""Both sharded-search protocols on real NCCL ranks against the unsharded search of the same index (bit-identical D and I), before
+and after every rank adds the same batch (ShardedIvfPq.add_with_ids):
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29517 tools/check_sharded_nccl.py
 The index is synthetic (seeded, generated on the GPUs); rank 0 also builds the WHOLE index on its GPU as the reference."""
 import os, sys
@@ -37,6 +38,27 @@ for n, nprobe in ((1024, 64), (515, 32), (64, 256), (96, 16)):          # 515: r
         print(f"n={n} nprobe={nprobe} world={world}: query-split == list-split: {same}; == unsharded index: {ref_ok}", flush=True)
         ok = ok and same and ref_ok
     dist.barrier()
+# growing the sharded index: every rank adds the same batch (no exchange), then both protocols == the unsharded index after the same add
+xa = 0.5 * torch.randn((50_000, 768), generator=g, device="cuda")
+dist.broadcast(xa, 0)
+sh.add_with_ids(xa)
+x = 0.5 * torch.randn((1024, 768), generator=g, device="cuda")
+dist.broadcast(x, 0)
+sh.nprobe = 64
+res = {}
+for qs in (False, True):
+    sh.query_split = qs
+    res[qs] = tuple(t.clone() for t in sh.search_device(x, K))
+if rank == 0:
+    full = IvfPqIndex(NLIST, device=local)
+    full.set_opq(bench.opq_matrix(7)); full.gen_centroids(7); full.gen_pq(7); full.set_lists_synthetic(lens, 7)
+    full.add(xa)
+    full.nprobe = 64
+    Df, If = full.search(x, K)
+    add_ok = all(torch.equal(Df, res[qs][0]) and torch.equal(If, res[qs][1]) for qs in (False, True)) and full.ntotal == sh.ntotal
+    print(f"after add of {xa.shape[0]} vectors, world={world}: both protocols == unsharded grown index: {add_ok}", flush=True)
+    ok = ok and add_ok
+dist.barrier()
 if rank == 0:
     print("SHARDED NCCL CHECK", "PASSED" if ok else "FAILED", flush=True)
 dist.destroy_process_group()
