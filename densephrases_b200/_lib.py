@@ -78,6 +78,10 @@ _SIGS = {
     "dph_index_copy_lists": (_i32, [_vp, _vp, _vp]),
     "dph_index_get_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_add_ms": (_i32, [_vp, _vp]),
+    "dph_index_remove_ids": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
+    "dph_index_sync_list_len": (_i32, [_vp, _vp]),
+    "dph_index_last_remove_ms": (_i32, [_vp, _vp]),
+    "dph_index_last_remove_tmp_bytes": (_i64, [_vp]),
 }
 EXPORTS = tuple(_SIGS)
 

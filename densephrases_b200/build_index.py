@@ -17,6 +17,10 @@ Filling an index on the GPU (the add_with_ids of build_phrase_index.py:145-150,1
         ix.add_with_ids(x, ids)
     list_len, codes, ids = ix.lists()            # list-major, what set_lists takes
     artifacts.write_faiss_index(path, A, centroids, pq, list_len, codes, ids)
+Updating a document (DESIGN.md 3.2): its phrases carry consecutive labels [first, first + n) (build_phrase_index.py:149), so
+    ix.remove_ids(range(first, first + n))       # faiss remove_ids(IDSelectorRange); a label array drops a set of documents
+    ix.add_with_ids(x_new, ids_new)              # the document's new phrase vectors
+Keeping idx2id and the phrase metadata in step with re-added documents is the caller's job.
 add_to_index below is the PyTorch encoder that runs without a GPU; its argmax / argmin have no fixed floating-point order, so on
 ties and near-ties it may pick other lists or codewords than IvfPqIndex.encode."""
 import numpy as np

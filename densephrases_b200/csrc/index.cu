@@ -13,7 +13,7 @@
 static thread_local std::string g_err;
 void dph_set_error(const std::string& msg) { g_err = msg; }
 DPH_API const char* dph_last_error(void) { return g_err.c_str(); }
-DPH_API int dph_version(void) { return 101; }
+DPH_API int dph_version(void) { return 102; }
 int g_dph_tune[8] = {1, 0, 0, 0, 0, 0, 0, 0};      // [0] quad-scan IMAD level, [1] SGEMM tile (0 auto), [2] PQ-table kernel shape (0 auto)
 DPH_API int dph_set_tuning(int knob, int value) {
     DPH_CHECK(knob >= 0 && knob < 8, "dph_set_tuning: unknown knob");
@@ -50,10 +50,10 @@ __global__ void gen_normal_kernel(float* out, long long rows, int cols, uint64_t
     out[i] = dph_approx_normal(dph_rnd64(seed, stream, (uint64_t)r, (uint64_t)t), sc);
 }
 
-// Block -> list lookup inside the shard: last l in [lo,hi) with blk_off[l] <= blk.
-__device__ __forceinline__ long long list_of_block(const long long* blk_off, long long lo, long long hi, long long blk) {
-    while (hi - lo > 1) { long long mid = (lo + hi) >> 1; if (blk_off[mid] <= blk) lo = mid; else hi = mid; }
-    return lo;
+int64_t dph_chunk_rows() {
+    int64_t chunk_rows = (256ll << 20) / DPH_CODE;
+    if (const char* ev = getenv("DPH_UPLOAD_CHUNK_ROWS")) chunk_rows = std::max<int64_t>(1, atoll(ev));      // tests: force many chunks
+    return chunk_rows;
 }
 
 // One thread per (block, lane, 16-byte chunk): writes the interleaved/rotated layout (common.cuh).
@@ -196,7 +196,7 @@ static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_
         blk_off[l] = nb; local_row_start[l - lo] = rows;
         nb += (list_len[l] + 31) / 32; rows += list_len[l];
     }
-    ix->nblocks_local = nb; ix->ntotal_local = rows;
+    ix->nblocks_local = nb; ix->ntotal_local = rows; ix->blk_cap = -1;
     DPH_TRY(dev_alloc(&ix->list_len, (size_t)nlist, ix));
     DPH_TRY(dev_alloc(&ix->list_start, (size_t)nlist + 1, ix));
     DPH_TRY(dev_alloc(&ix->blk_off, (size_t)nlist, ix));
@@ -220,8 +220,7 @@ static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_
         // Upload in chunks of whole lists through a bounded staging buffer (<= ~256 MB of rows): the raw list-major copy never
         // sits on the device next to the blocked one.  Labels go the same way; the direct map (faiss DirectMap::Hashtable,
         // build_phrase_index.py:139-141) is filled by the same kernel and sorted ON THE DEVICE.
-        int64_t chunk_rows = (256ll << 20) / DPH_CODE;
-        if (const char* ev = getenv("DPH_UPLOAD_CHUNK_ROWS")) chunk_rows = std::max<int64_t>(1, atoll(ev));      // tests: force many chunks
+        const int64_t chunk_rows = dph_chunk_rows();
         auto chunk_end = [&](int64_t l0, int64_t& acc) {       // lists [l0, l1) of one upload: whole lists, <= chunk_rows rows (one list may exceed it)
             int64_t l1 = l0;
             acc = 0;
@@ -285,23 +284,6 @@ DPH_API int dph_index_set_lists_synthetic(dph_index* ix, const int64_t* list_len
 // -------------------------------------------------------------------------------------------------
 static int check_ready(dph_index* ix, int k);
 
-struct DevTmp {            // the device allocations of one call, freed on every exit path unless released
-    std::vector<void*> ps;
-    ~DevTmp() { for (void* p : ps) if (p) cudaFree(p); }
-    template <class T> int alloc(T** out, size_t count, const char* what) {
-        cudaError_t e = cudaMalloc((void**)out, std::max<size_t>(count, 1) * sizeof(T));
-        if (e != cudaSuccess) {
-            cudaGetLastError();                     // an allocation failure is not sticky: keep it out of later error checks
-            *out = nullptr;
-            dph_set_error(std::string(what) + ": " + cudaGetErrorString(e));
-            return 1;
-        }
-        ps.push_back(*out);
-        return 0;
-    }
-    void release(void* p) { for (void*& q : ps) if (q == p) q = nullptr; }
-};
-
 __global__ void iota_kernel(long long* out, long long n, long long base) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = base + i;
@@ -317,23 +299,23 @@ __global__ void add_validate_kernel(const long long* list_no, const long long* i
 }
 
 // one CTA per block of the new layout: old blocks move whole (same rows, same lanes), blocks past a list's old end start as zeros
-__global__ void __launch_bounds__(192) relayout_codes_kernel(uint8_t* codes_new, const long long* boff_new, const long long* boff_old,
+__global__ void __launch_bounds__(192) relayout_codes_kernel(uint8_t* dst, long long blk0, const long long* boff_new, const long long* boff_old,
                                                              const int* len_old, long long lo, long long hi, const uint8_t* codes_old) {
-    const long long blk = blockIdx.x;
+    const long long blk = blk0 + blockIdx.x;
     __shared__ long long s_l;
     if (threadIdx.x == 0) s_l = list_of_block(boff_new, lo, hi, blk);
     __syncthreads();
     const long long l = s_l, b = blk - boff_new[l];
     uint4 v = make_uint4(0, 0, 0, 0);
     if (b < ((long long)len_old[l] + 31) / 32) v = reinterpret_cast<const uint4*>(codes_old + (boff_old[l] + b) * DPH_BLK_BYTES)[threadIdx.x];
-    reinterpret_cast<uint4*>(codes_new + blk * DPH_BLK_BYTES)[threadIdx.x] = v;
+    reinterpret_cast<uint4*>(dst + (long long)blockIdx.x * DPH_BLK_BYTES)[threadIdx.x] = v;
 }
 // labels of the new layout's old rows (-1 elsewhere; the new rows are written by add_scatter_kernel).  Implicit labels (ids_old null)
 // become explicit: list_start_old[l] + j, with their direct-map pairs at the row's old local position (already in label order).
-__global__ void relayout_ids_kernel(long long* ids_new, const long long* boff_new, const long long* boff_old, const int* len_old, long long lo,
-                                    long long hi, const long long* ids_old, const long long* list_start_old, const long long* lrs_old,
-                                    long long* dm_ids, long long* dm_rows) {
-    const long long blk = blockIdx.x;
+__global__ void relayout_ids_kernel(long long* dst, long long blk0, const long long* boff_new, const long long* boff_old, const int* len_old,
+                                    long long lo, long long hi, const long long* ids_old, const long long* list_start_old,
+                                    const long long* lrs_old, long long* dm_ids, long long* dm_rows) {
+    const long long blk = blk0 + blockIdx.x;
     const long long l = list_of_block(boff_new, lo, hi, blk), b = blk - boff_new[l];
     const long long j = b * 32 + threadIdx.x;
     long long id = -1;
@@ -345,7 +327,7 @@ __global__ void relayout_ids_kernel(long long* ids_new, const long long* boff_ne
             dm_rows[lrs_old[l - lo] + j] = blk * 32 + threadIdx.x;
         }
     }
-    ids_new[blk * 32 + threadIdx.x] = id;
+    dst[(long long)blockIdx.x * 32 + threadIdx.x] = id;
 }
 // existing direct-map pairs (explicit labels): old padded row -> the same (list, j) in the new layout
 __global__ void remap_dm_kernel(const long long* dm_ids_old, const long long* dm_rows_old, long long cnt, const long long* boff_old,
@@ -373,17 +355,7 @@ __global__ void add_scatter_kernel(long long n, const long long* sorted_list, co
     uint4 row4[6];
 #pragma unroll
     for (int c = 0; c < 6; c++) row4[c] = reinterpret_cast<const uint4*>(codes_all + r * DPH_CODE)[c];
-    const unsigned char* row = reinterpret_cast<const unsigned char*>(row4);
-#pragma unroll
-    for (int c = 0; c < 6; c++) {          // the lane-rotated layout of fill_blocks_kernel / common.cuh:dph_blk_addr
-        unsigned char bytes[16];
-        const int seg = c >> 1;
-#pragma unroll
-        for (int b = 0; b < 16; b++) { const int t = c * 16 + b; bytes[b] = row[seg * 32 + ((lane + (t & 31)) & 31)]; }
-        uint4 v;
-        memcpy(&v, bytes, 16);
-        *reinterpret_cast<uint4*>(codes_new + blk * DPH_BLK_BYTES + c * 512 + lane * 16) = v;
-    }
+    dph_store_row(codes_new, blk, lane, reinterpret_cast<const unsigned char*>(row4));
     const long long id = ids_all[r];
     ids_new[blk * 32 + lane] = id;
     dm_ids[dm0 + r] = id;
@@ -465,8 +437,8 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[4], st));
     const long long *bo_new = (const long long*)d_boff_new, *bo_old = (const long long*)ix->blk_off;
     if (nb > 0) {
-        relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
-        relayout_ids_kernel<<<(unsigned)nb, 32, 0, st>>>((long long*)ids_new, bo_new, bo_old, ix->list_len, lo, hi, (const long long*)ix->ids,
+        relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, 0, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
+        relayout_ids_kernel<<<(unsigned)nb, 32, 0, st>>>((long long*)ids_new, 0, bo_new, bo_old, ix->list_len, lo, hi, (const long long*)ix->ids,
                                                        (const long long*)ix->list_start, (const long long*)d_lrs, (long long*)dm_ids_new,
                                                        (long long*)dm_rows_new);
     }
@@ -496,7 +468,7 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     DPH_CUDA(cudaMemcpy(ix->blk_off, d_boff_new, nlist * 8, cudaMemcpyDeviceToDevice));
     DPH_CUDA(cudaMemcpy(ix->list_len, len32.data(), nlist * 4, cudaMemcpyHostToDevice));
     DPH_CUDA(cudaMemcpy(ix->list_start, start_new.data(), (nlist + 1) * 8, cudaMemcpyHostToDevice));
-    const int64_t nb_old = ix->nblocks_local;
+    const int64_t nb_old = ix->blk_cap < 0 ? ix->nblocks_local : ix->blk_cap;       // a remove leaves the allocation as it was
     int64_t old_bytes = std::max<int64_t>(nb_old * DPH_BLK_BYTES, 1);
     if (ix->ids) old_bytes += std::max<int64_t>(nb_old * 32, 1) * 8;
     if (ix->dm_ids) old_bytes += 2 * std::max<int64_t>(ix->dm_cap < 0 ? ix->ntotal_local : ix->dm_cap, 1) * 8;
@@ -508,7 +480,7 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     ix->bytes += new_bytes - old_bytes;
     ix->dm_n = dm_old + in_shard; ix->dm_cap = dm_cap;
     ix->h_list_len = len_new; ix->h_list_start = start_new;
-    ix->ntotal = start_new[nlist]; ix->ntotal_local = rows; ix->nblocks_local = nb;
+    ix->ntotal = start_new[nlist]; ix->ntotal_local = rows; ix->nblocks_local = nb; ix->blk_cap = -1;
     if (prof) DPH_CUDA(cudaEventElapsedTime(&ix->add_ms[3], ix->aev[4], ix->aev[5]));
     return 0;
 }
@@ -545,8 +517,7 @@ DPH_API int dph_index_copy_lists(dph_index* ix, uint8_t* codes_out, int64_t* ids
     if (ix->ntotal_local == 0) return 0;
     std::vector<int64_t> boff(hi - lo), lrs(hi - lo);
     for (int64_t l = lo, nb = 0, rows = 0; l < hi; l++) { boff[l - lo] = nb; lrs[l - lo] = rows; nb += (len[l] + 31) / 32; rows += len[l]; }
-    int64_t chunk_rows = (256ll << 20) / DPH_CODE;
-    if (const char* ev = getenv("DPH_UPLOAD_CHUNK_ROWS")) chunk_rows = std::max<int64_t>(1, atoll(ev));
+    const int64_t chunk_rows = dph_chunk_rows();
     auto chunk_end = [&](int64_t l0, int64_t& acc) {           // lists [l0, l1): whole lists, <= chunk_rows rows (one list may exceed it)
         int64_t l1 = l0;
         acc = 0;

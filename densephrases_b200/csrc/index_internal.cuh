@@ -2,6 +2,8 @@
 #pragma once
 #include "common.cuh"
 #include "../../include/dph_b200.h"
+#include <algorithm>
+#include <string.h>
 #include <vector>
 
 #define DPH_SCAN_THREADS 512
@@ -78,9 +80,73 @@ struct dph_index {
     bool profile = false;              // CUDA events around the scan kernel of the last search chunk
     cudaEvent_t ev0[DPH_PROF_RING] = {}, ev1[DPH_PROF_RING] = {};
     int64_t prof_n = 0;
-    cudaEvent_t aev[6] = {};           // profiled adds: stage boundaries (encode.cu, index.cu)
+    cudaEvent_t aev[6] = {};           // profiled adds and removes: stage boundaries (encode.cu, index.cu, remove.cu)
     float add_ms[4] = {};              // last add: rotation, coarse, PQ encode, re-layout + scatter (ms)
+    float remove_ms[3] = {};           // last remove: mark + plan, row moves + block shift, direct map (ms)
+    int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
+    int64_t blk_cap = -1;              // blocks allocated for codes / ids (-1: nblocks_local; a remove does not shrink them)
 };
+
+// Block -> list lookup inside the shard: last l in [lo,hi) with blk_off[l] <= blk.
+__device__ __forceinline__ long long list_of_block(const long long* blk_off, long long lo, long long hi, long long blk) {
+    while (hi - lo > 1) { long long mid = (lo + hi) >> 1; if (blk_off[mid] <= blk) lo = mid; else hi = mid; }
+    return lo;
+}
+// One 96-byte code row -> the lane-rotated layout of fill_blocks_kernel / common.cuh:dph_blk_addr (six 16-byte stores of one lane).
+__device__ __forceinline__ void dph_store_row(uint8_t* codes, long long blk, int lane, const unsigned char* row) {
+#pragma unroll
+    for (int c = 0; c < 6; c++) {
+        unsigned char bytes[16];
+        const int seg = c >> 1;
+#pragma unroll
+        for (int b = 0; b < 16; b++) { const int t = c * 16 + b; bytes[b] = row[seg * 32 + ((lane + (t & 31)) & 31)]; }
+        uint4 v;
+        memcpy(&v, bytes, 16);
+        *reinterpret_cast<uint4*>(codes + blk * DPH_BLK_BYTES + c * 512 + lane * 16) = v;
+    }
+}
+// The inverse: the row of `lane` in block `blk`, m ascending.
+__device__ __forceinline__ void dph_load_row(const uint8_t* codes, long long blk, int lane, unsigned char* row) {
+#pragma unroll
+    for (int c = 0; c < 6; c++) {
+        const uint4 v = *reinterpret_cast<const uint4*>(codes + blk * DPH_BLK_BYTES + c * 512 + lane * 16);
+        unsigned char bytes[16];
+        memcpy(bytes, &v, 16);
+        const int seg = c >> 1;
+#pragma unroll
+        for (int b = 0; b < 16; b++) { const int t = c * 16 + b; row[seg * 32 + ((lane + (t & 31)) & 31)] = bytes[b]; }
+    }
+}
+
+struct DevTmp {            // the device allocations of one call, freed on every exit path unless released
+    std::vector<void*> ps;
+    int64_t live = 0, peak = 0;             // bytes allocated through this object (released ones included), and the largest total
+    ~DevTmp() { for (void* p : ps) if (p) cudaFree(p); }
+    template <class T> int alloc(T** out, size_t count, const char* what) {
+        const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
+        cudaError_t e = cudaMalloc((void**)out, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();                     // an allocation failure is not sticky: keep it out of later error checks
+            *out = nullptr;
+            dph_set_error(std::string(what) + ": " + cudaGetErrorString(e));
+            return 1;
+        }
+        ps.push_back(*out);
+        live += (int64_t)bytes; peak = std::max(peak, live);
+        return 0;
+    }
+    void release(void* p) { for (void*& q : ps) if (q == p) q = nullptr; }
+};
+
+// Rows per staging chunk of set_lists / copy_lists / remove (about 256 MB of code rows; DPH_UPLOAD_CHUNK_ROWS overrides it for tests).
+int64_t dph_chunk_rows();
+// Block re-layout of the add (index.cu), also the remove's block shift: blocks [blk0, blk0 + gridDim.x) of the layout boff_new are
+// written to dst[0 ..) from the same list's block in boff_old (whole, same rows and lanes; zeros / -1 past the list's old end).
+__global__ void relayout_codes_kernel(uint8_t* dst, long long blk0, const long long* boff_new, const long long* boff_old, const int* len_old,
+                                      long long lo, long long hi, const uint8_t* codes_old);
+__global__ void relayout_ids_kernel(long long* dst, long long blk0, const long long* boff_new, const long long* boff_old, const int* len_old,
+                                    long long lo, long long hi, const long long* ids_old, const long long* list_start_old,
+                                    const long long* lrs_old, long long* dm_ids, long long* dm_rows);
 
 // process-wide variant selection (dph_set_tuning, measurement hook): [0] quad-scan IMAD level, [1] SGEMM tile
 extern int g_dph_tune[8];

@@ -143,6 +143,65 @@ class IvfPqIndex:
         L.check(L.lib().dph_index_last_add_ms(self._h, _np_ptr(out)))
         return out
 
+    # ---- removing vectors (faiss index.remove_ids with IDSelectorBatch / IDSelectorRange) ----------
+    def remove_ids_per_list(self, sel):
+        """Remove every row whose label is selected -> rows removed per list [nlist] i64 (this shard's lists only).  sel: a numpy or
+        torch int64 array of labels (any order, duplicates allowed, absent or negative labels match nothing) or a step-1 range of
+        labels.  Survivor order and the rejected cases: DESIGN.md 3.2 / dph_index_remove_ids."""
+        per = np.zeros(self.nlist, dtype=np.int64)
+        n = C.c_int64(0)
+        if isinstance(sel, range):
+            if sel.step != 1:
+                raise ValueError("remove_ids: a range selector must have step 1")
+            # ctypes would wrap bounds past the int64 range: clamp them (a stop past it then reaches every label up to 2^63 - 2)
+            lo, hi = (min(max(v, -2**63), 2**63 - 1) for v in (sel.start, sel.stop))
+            L.check(L.lib().dph_index_remove_ids(self._h, None, 0, lo, hi, L.MEM_HOST, C.byref(n), _np_ptr(per)))
+            return per
+        if isinstance(sel, np.ndarray):
+            if sel.dtype != np.int64:
+                raise TypeError(f"remove_ids: labels must be int64, got {sel.dtype}")
+            ids = np.ascontiguousarray(sel).ravel()
+            L.check(L.lib().dph_index_remove_ids(self._h, _np_ptr(ids), len(ids), 0, 0, L.MEM_HOST, C.byref(n), _np_ptr(per)))
+            return per
+        import torch
+        if not isinstance(sel, torch.Tensor) or sel.dtype != torch.int64:
+            raise TypeError("remove_ids: expected an int64 numpy array, an int64 torch tensor or a step-1 range, got %r" % type(sel))
+        ids = sel.contiguous().view(-1)
+        if ids.is_cuda:
+            self.set_stream(torch.cuda.current_stream(ids.device).cuda_stream)
+            L.check(L.lib().dph_index_remove_ids(self._h, ids.data_ptr(), ids.numel(), 0, 0, L.MEM_DEVICE, C.byref(n), _np_ptr(per)))
+        else:
+            ids = ids.numpy()
+            L.check(L.lib().dph_index_remove_ids(self._h, _np_ptr(ids), len(ids), 0, 0, L.MEM_HOST, C.byref(n), _np_ptr(per)))
+        return per
+
+    def remove_ids(self, sel):
+        """== faiss index.remove_ids(IDSelectorBatch(sel)) for a label array, index.remove_ids(IDSelectorRange(lo, hi)) for
+        range(lo, hi) -> the number of rows removed (on a shard: from this shard)."""
+        return int(self.remove_ids_per_list(sel).sum())
+
+    def list_len(self):
+        """-> [nlist] i64: the length of every list (all shards)."""
+        out = np.empty(self.nlist, dtype=np.int64)
+        L.check(L.lib().dph_index_get_list_len(self._h, _np_ptr(out)))
+        return out
+
+    def sync_list_len(self, list_len):
+        """Sharded remove: set the lengths of the other shards' lists (this shard's entries must equal its own)."""
+        list_len = np.ascontiguousarray(list_len, dtype=np.int64)
+        assert list_len.shape == (self.nlist,)
+        L.check(L.lib().dph_index_sync_list_len(self._h, _np_ptr(list_len)))
+
+    def last_remove_ms(self):
+        """With set_profile(True): stage times of the last remove in ms (mark + plan, row moves + block shift, direct map)."""
+        out = np.zeros(3, dtype=np.float32)
+        L.check(L.lib().dph_index_last_remove_ms(self._h, _np_ptr(out)))
+        return out
+
+    def last_remove_tmp_bytes(self):
+        """The largest total of the last remove's temporary device allocations, in bytes."""
+        return int(L.lib().dph_index_last_remove_tmp_bytes(self._h))
+
     # ---- attributes ---------------------------------------------------------------------------
     @property
     def ntotal(self):

@@ -148,6 +148,17 @@ class ShardedIvfPq:
         the same global list lengths and labels (ids None -> ntotal + arange(n)) and stores the rows of its own lists."""
         self.local.add_with_ids(x, ids)
 
+    def remove_ids(self, sel):
+        """== faiss index.remove_ids (IvfPqIndex.remove_ids selectors); a collective: every rank passes the same selector.  Each rank
+        removes the rows of its own lists; the per-list counts are all-reduced so that every rank sets the same global list lengths
+        (and list starts, which order ties in the merge).  Returns the number of rows removed from the whole index."""
+        if self.world == 1:
+            return self.local.remove_ids(sel)
+        before = self.local.list_len()
+        removed = self._sum_over_shards(self.local.remove_ids_per_list(sel))
+        self.local.sync_list_len(before - removed)
+        return int(removed.sum())
+
     # ---- the slice of the faiss index API that MIPS uses (index.py:30-33,200,286,296) ----
     @property
     def ntotal(self):

@@ -14,6 +14,8 @@
  *   dph_index_add_with_ids      <- index.add_with_ids(vectors, ids)          build_phrase_index.py:145-150,156-279
  *   dph_index_encode            <- the assignment + PQ encoding inside add_with_ids (IndexIVFPQ::encode_vectors)
  *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
+ *   dph_index_remove_ids        <- index.remove_ids(IDSelectorBatch(ids) | IDSelectorRange(lo, hi)) (faiss 1.6.x IndexIVF)
+ *   dph_index_sync_list_len     <- (sharded remove) the list lengths faiss keeps in one process, exchanged between shards
  *
  * Conventions: every function returns 0 on success, non-zero on error (dph_last_error() gives the
  * message; the Python layer raises RuntimeError like faiss' SWIG layer does).  `mem` arguments say
@@ -85,6 +87,31 @@ int dph_index_copy_lists(dph_index* ix, uint8_t* codes_out, int64_t* ids_out);
 int dph_index_get_list_len(const dph_index* ix, int64_t* list_len_out);
 /* Measurement hook: with profiling on, the stage times of the last add in ms: rotation, coarse, PQ encode, re-layout + scatter. */
 int dph_index_last_add_ms(const dph_index* ix, float* ms_out /* [4] */);
+
+/* ---- removing vectors (replaces index.remove_ids(faiss.IDSelectorBatch(ids)) / remove_ids(faiss.IDSelectorRange(lo, hi)) of faiss
+ * 1.6.x IndexIVF; DESIGN.md 3.2 "Removing vectors") ----
+ * Selector: the label set ids [n_ids] (mem says where it lives; any order, duplicates allowed, absent or negative labels match nothing)
+ * when ids is non-NULL, with range_lo = range_hi = 0; else the label range [range_lo, range_hi), with n_ids = 0.  Every row of this
+ * shard whose label is selected is removed.  Each list keeps the survivors in the order of faiss' IndexIVF::remove_ids loop without a
+ * direct map (the last row fills each hole); the device state afterwards is byte-identical to set_lists of the resulting list-major
+ * arrays.  An empty selector (n_ids == 0, or range_lo >= range_hi) changes nothing; any other turns sequential labels into explicit
+ * ones, as the first add does.  The shard compacts in place: extra device memory is one staging buffer of <= ~256 MB plus
+ * O(nlist + n_ids + rows removed), and 24 B per row for an index that gains labels; the code allocation is not shrunk.  Rejected,
+ * with the index unchanged: n_ids < 0, both or neither selector forms, too little device memory for those buffers.
+ * n_removed_out: rows removed from this shard; removed_per_list_out [nlist] (host, may be NULL): per list, zero outside the shard.
+ * On a shard, the lengths of other shards' lists are left as they were: see dph_index_sync_list_len.  Synchronises the stream. */
+int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_ids, int64_t range_lo, int64_t range_hi, int mem,
+                         int64_t* n_removed_out, int64_t* removed_per_list_out);
+/* Sharded remove (sharded.py): after every shard removed the same selector, list_len [nlist] (host) = the old lengths minus the
+ * all-reduced per-list counts.  Sets the lengths (and list starts, which order ties in the sharded merge) of the lists outside
+ * [list_lo, list_hi); refuses, with the index unchanged, when an entry of this shard differs from its own length, or when other lists
+ * change on a shard whose labels are still sequential (they would move). */
+int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len);
+/* Measurement hooks: with profiling on, the stage times of the last remove in ms: mark + plan, row moves + block shift, direct map;
+ * and the largest total of its temporary device allocations in bytes (the device sorts' own scratch not included).  A call with an
+ * empty selector resets both to zero. */
+int dph_index_last_remove_ms(const dph_index* ix, float* ms_out /* [3] */);
+int64_t dph_index_last_remove_tmp_bytes(const dph_index* ix);
 
 /* ---- getters ---- */
 int64_t dph_index_ntotal(const dph_index* ix);       /* all shards */
