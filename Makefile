@@ -19,14 +19,16 @@ $(LIB): $(OBJS)
 	@mkdir -p densephrases_b200/lib
 	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -lcudart
 
-oracle: oracle/libivfpq_ref.so oracle/libencode_ref.so oracle/libremove_ref.so
+oracle: oracle/libivfpq_ref.so oracle/libencode_ref.so oracle/libremove_ref.so oracle/libtrain_ref.so
 oracle/libivfpq_ref.so: oracle/ivfpq_ref.c
 	gcc -O3 -march=x86-64-v3 -ffp-contract=off -fno-fast-math -fopenmp -fPIC -shared -fvisibility=hidden -o $@ $< -lm
 oracle/libencode_ref.so: oracle/encode_ref.c oracle/ivfpq_ref.c
 	gcc -O3 -march=x86-64-v3 -ffp-contract=off -fno-fast-math -fopenmp -fPIC -shared -fvisibility=hidden -o $@ $< -lm
 oracle/libremove_ref.so: oracle/remove_ref.c
 	gcc -O3 -fPIC -shared -fvisibility=hidden -o $@ $<
+oracle/libtrain_ref.so: oracle/train_ref.c oracle/ivfpq_ref.c
+	gcc -O3 -march=x86-64-v3 -ffp-contract=off -fno-fast-math -fopenmp -fPIC -shared -fvisibility=hidden -o $@ $< -lm
 
 clean:
-	rm -rf build $(LIB) oracle/libivfpq_ref.so oracle/libencode_ref.so oracle/libremove_ref.so
+	rm -rf build $(LIB) oracle/libivfpq_ref.so oracle/libencode_ref.so oracle/libremove_ref.so oracle/libtrain_ref.so
 .PHONY: all oracle clean

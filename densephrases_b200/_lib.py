@@ -82,6 +82,12 @@ _SIGS = {
     "dph_index_sync_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_remove_ms": (_i32, [_vp, _vp]),
     "dph_index_last_remove_tmp_bytes": (_i64, [_vp]),
+    "dph_index_train_coarse": (_i32, [_vp, _vp, _i64, _i32, _u64, _i64, _i32, _i32, _vp, _vp]),
+    "dph_index_train_pq": (_i32, [_vp, _vp, _i64, _i32, _u64, _i64, _i32, _i32, _i32]),
+    "dph_index_encode_pq": (_i32, [_vp, _vp, _i64, _vp, _i32]),
+    "dph_index_get_centroids": (_i32, [_vp, _vp, _i32]),
+    "dph_index_get_pq": (_i32, [_vp, _vp, _i32]),
+    "dph_index_last_train_ms": (_i32, [_vp, _vp]),
 }
 EXPORTS = tuple(_SIGS)
 

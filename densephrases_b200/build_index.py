@@ -10,6 +10,12 @@ in L2 per 8-dim sub-vector.  Plain PyTorch (CPU or CUDA) -- this is an offline t
 IvfPqIndex.from_arrays consumes.  Randomness is seeded; faiss' own random initialisations are not reproduced (trained indexes are
 equivalent in kind, not bit-identical to a faiss-trained one).
 
+Training on the GPU (index.train of build_phrase_index.py:96-142, with the fixed fp32 order of DESIGN.md 3.3; train_index_gpu below):
+    ix = IvfPqIndex(nlist)
+    ix.train(x_train)                            # OPQ, spherical k-means coarse quantizer, PQ on residuals -> trained, empty
+    ix.add_with_ids(x, ids)                      # as below
+    list_len, codes, ids = ix.lists()
+    artifacts.write_faiss_index(path, ix.opq_matrix(), ix.centroids(), ix.pq_codebooks(), list_len, codes, ids)
 Filling an index on the GPU (the add_with_ids of build_phrase_index.py:145-150,156-279, with the exact fp32 encoding of DESIGN.md 3.1):
     A, centroids, pq = train_index(x_train, nlist)
     ix = IvfPqIndex.from_arrays(A, centroids, pq, np.zeros(nlist, np.int64), np.zeros((0, 96), np.uint8))   # trained, empty
@@ -90,6 +96,16 @@ def train_index(x, nlist, niter_opq=10, niter_km=10, niter_pq=8, seed=123, devic
     assign = (xr @ centroids.T).argmax(1)
     pq = _train_pq(xr - centroids[assign], niter_pq, seed + 13)
     return A.cpu().numpy(), centroids.cpu().numpy(), pq.cpu().numpy()
+
+
+def train_index_gpu(x, nlist, niter_opq=10, niter_km=10, niter_pq=25, seed=123, max_points_per_centroid=256, device=0):
+    """train_index on the GPU (IvfPqIndex.train): x [ns, 768] numpy or CUDA float32 -> (A, centroids, pq) like train_index.  Unlike
+    train_index it subsamples to max_points_per_centroid per centroid, so it trains the IVF65536 and larger shapes, and its coarse
+    k-means is spherical, as faiss' is for an inner-product IVF index."""
+    from .ivfpq import IvfPqIndex
+    ix = IvfPqIndex(nlist, device=device)
+    ix.train(x, niter=niter_km, niter_pq=niter_pq, opq_niter=niter_opq, seed=seed, max_points_per_centroid=max_points_per_centroid)
+    return ix.opq_matrix(), ix.centroids(), ix.pq_codebooks()
 
 
 def add_to_index(A, centroids, pq, x, ids=None, offset=0, running_total=0, device=None, chunk=65536):

@@ -128,8 +128,11 @@ __global__ void cnorm_max_kernel(const float* C, long long nl, float* out) {
 }
 
 // Coarse top-nprobe over lists [lo, lo+nl) of the index.  Writes keys64 (sharded path) or key/cd.  Returns 1 if the tensor-core
-// path does not apply to this shape (caller uses the SIMT path).
-int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, unsigned long long* keys64, int32_t* key, float* cd, cudaStream_t st) {
+// path does not apply to this shape (caller uses the SIMT path).  xr / C: the rotated rows [n, d] and the centroids [nlist, d]
+// (nullptr: the index's xr workspace and centroids).  The (hi, lo) centroid split is cached by list range: a caller that passes other
+// centroids, or changes them, sets ix->csplit_lo = -1 first.
+int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, unsigned long long* keys64, int32_t* key, float* cd, cudaStream_t st,
+                  const float* xr, const float* C) {
     const int margin = nprobe / 4 > 32 ? nprobe / 4 : 32;
     const int ncand = (int)std::min<int64_t>(nprobe + margin, nl);
     // pays for small probe counts; at nprobe 256 the exact re-rank of 320 candidates costs about what the tensor cores save, so the
@@ -140,7 +143,8 @@ int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, 
     if (ncand > DPH_MAX_NPROBE || n < 32 || !(few_candidates || many_lists)) return 1;
     const int64_t nlp = (nl + 127) / 128 * 128;          // GEMM N must be a multiple of the 128-wide tile: zero-padded centroid rows
     if ((size_t)n * nlp * 4 > ix->S.cap) return 1;
-    const float* Cl = ix->C + lo * DPH_D;
+    const float* Cl = (C ? C : ix->C) + lo * DPH_D;
+    const float* X = xr ? xr : ix->xr.as<float>();
     if (!ix->csplit.p || ix->csplit_lo != lo || ix->csplit_nl != nl) {          // (hi, lo) TF32 split of the shard's centroids + max norm, once
         DPH_TRY(ix->csplit.ensure((size_t)nlp * DPH_D * 8 + 16));
         float* hi = ix->csplit.as<float>();
@@ -157,12 +161,12 @@ int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, 
     DPH_TRY(ix->candkeys.ensure((size_t)n * ncand * 8));
     DPH_TRY(ix->cflags.ensure((size_t)n * 4));
     float* xhi = ix->xsplit.as<float>(); float* xlo = xhi + n * DPH_D;
-    DPH_TRY(dph_launch_split_tf32(ix->xr.as<float>(), xhi, xlo, n * DPH_D, st));
+    DPH_TRY(dph_launch_split_tf32(X, xhi, xlo, n * DPH_D, st));
     const float* A1[1] = {xhi}; const float* W1[1] = {chi}; const float* A2[1] = {xlo}; const float* W2[1] = {clo}; float* O1[1] = {ix->S.as<float>()};
     DPH_TRY(dph_launch_gemm_tf32(1, A1, W1, nullptr, nullptr, O1, (int)n, (int)nlp, DPH_D, 0, st, A2, W2));
     DPH_TRY(dph_launch_coarse_select(ix->S.as<float>(), n, nl, ncand, nullptr, nullptr, st, ix->candkeys.as<unsigned long long>(), 0u, nullptr, nlp, &ix->selkeys));
     CoarseTcArgs a;
-    a.xr = ix->xr.as<float>(); a.C = Cl; a.Sapprox = ix->S.as<float>(); a.nl = nl; a.ncand = ncand; a.nprobe = nprobe; a.list_base = (unsigned)lo;
+    a.xr = X; a.C = Cl; a.Sapprox = ix->S.as<float>(); a.nl = nl; a.ncand = ncand; a.nprobe = nprobe; a.list_base = (unsigned)lo;
     a.cand_keys = ix->candkeys.as<unsigned long long>(); a.cnorm_max = cnorm; a.keys64 = keys64; a.key = key; a.cd = cd;
     a.flags = ix->cflags.as<int>(); a.S_exact = ix->S.as<float>();       // repaired rows are rewritten with stride nl (the approximate scores are dead by then)
     coarse_tc_finish_kernel<<<(unsigned)n, 256, 0, st>>>(a);

@@ -88,6 +88,26 @@ int64_t dph_encode_chunk(const dph_index* ix) {
     return std::max<int64_t>(c, 1);
 }
 
+int dph_coarse_top1(dph_index* ix, const float* xr, const float* C, int64_t n, int32_t* key, float* cd, cudaStream_t st) {
+    const int rc = ix->coarse_tc ? dph_coarse_tc(ix, n, 0, ix->nlist, 1, nullptr, key, cd, st, xr, C) : 1;
+    if (rc > 1) return rc;
+    if (rc == 1) {
+        DPH_TRY(dph_launch_sgemm_nt_seq(xr, n, C, ix->nlist, ix->d, ix->S.as<float>(), st));
+        DPH_TRY(dph_launch_coarse_select(ix->S.as<float>(), n, ix->nlist, 1, key, cd, st, nullptr, 0u, nullptr, 0, &ix->selkeys));
+    }
+    return 0;
+}
+
+int dph_pq_assign(dph_index* ix, const float* xr, const float* C, const int32_t* key, const float* pq, int64_t n, int64_t* list_out,
+                  uint8_t* codes_out, cudaStream_t st) {
+    const int64_t tiles = (n + ENC_TILE - 1) / ENC_TILE;
+    int msplit = 1;                                                       // enough CTAs for two waves; msplit divides 96
+    while (msplit < 32 && tiles * msplit < 2 * ix->num_sms) msplit *= 2;
+    pq_encode_kernel<<<dim3((unsigned)tiles, (unsigned)msplit), ENC_TILE, 0, st>>>(xr, C, pq, key, n, msplit, (long long*)list_out, codes_out);
+    DPH_CUDA(cudaGetLastError());
+    return 0;
+}
+
 static int encode_rows_chunk(dph_index* ix, const float* x, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad) {
     cudaStream_t st = ix->stream;
     const bool prof = ix->profile && ix->aev[0];
@@ -99,18 +119,9 @@ static int encode_rows_chunk(dph_index* ix, const float* x, int64_t n, int64_t* 
     DPH_TRY(dph_launch_sgemm_nt_seq(x, n, ix->A, ix->d, ix->d, ix->xr.as<float>(), st));                      // OPQ rotation
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[1], st));
     int32_t* key = ix->enc_key.as<int32_t>(); float* cd = ix->enc_cd.as<float>();
-    const int rc = ix->coarse_tc ? dph_coarse_tc(ix, n, 0, ix->nlist, 1, nullptr, key, cd, st) : 1;
-    if (rc > 1) return rc;
-    if (rc == 1) {
-        DPH_TRY(dph_launch_sgemm_nt_seq(ix->xr.as<float>(), n, ix->C, ix->nlist, ix->d, ix->S.as<float>(), st));
-        DPH_TRY(dph_launch_coarse_select(ix->S.as<float>(), n, ix->nlist, 1, key, cd, st, nullptr, 0u, nullptr, 0, &ix->selkeys));
-    }
+    DPH_TRY(dph_coarse_top1(ix, ix->xr.as<float>(), ix->C, n, key, cd, st));
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[2], st));
-    const int64_t tiles = (n + ENC_TILE - 1) / ENC_TILE;
-    int msplit = 1;                                                       // enough CTAs for two waves; msplit divides 96
-    while (msplit < 32 && tiles * msplit < 2 * ix->num_sms) msplit *= 2;
-    pq_encode_kernel<<<dim3((unsigned)tiles, (unsigned)msplit), ENC_TILE, 0, st>>>(ix->xr.as<float>(), ix->C, ix->pq, key, n, msplit,
-                                                                                  (long long*)list_out, codes_out);
+    DPH_TRY(dph_pq_assign(ix, ix->xr.as<float>(), ix->C, key, ix->pq, n, list_out, codes_out, st));
     DPH_CUDA(cudaGetLastError());
     if (prof) {
         DPH_CUDA(cudaEventRecord(ix->aev[3], st));

@@ -82,7 +82,8 @@ struct dph_index {
     int64_t prof_n = 0;
     cudaEvent_t aev[6] = {};           // profiled adds and removes: stage boundaries (encode.cu, index.cu, remove.cu)
     float add_ms[4] = {};              // last add: rotation, coarse, PQ encode, re-layout + scatter (ms)
-    float remove_ms[3] = {};           // last remove: mark + plan, row moves + block shift, direct map (ms)
+    float remove_ms[3] = {};
+    float train_ms[3] = {};            // last train_coarse / train_pq: assign, sort + update, split + renorm (ms, summed over iterations)           // last remove: mark + plan, row moves + block shift, direct map (ms)
     int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
     int64_t blk_cap = -1;              // blocks allocated for codes / ids (-1: nblocks_local; a remove does not shrink them)
 };
@@ -155,7 +156,8 @@ int dph_launch_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m
 int dph_launch_coarse_select(const float* S, int64_t n, int64_t nlist, int nprobe, int32_t* key, float* cd, cudaStream_t st,
                              unsigned long long* keys64 = nullptr, unsigned list_base = 0, const int* only_rows = nullptr, int64_t ld = 0,
                              DevBuf* tmp = nullptr);      // tmp: scratch for the chunked selection of long rows (nullptr: one CTA per row)
-int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, unsigned long long* keys64, int32_t* key, float* cd, cudaStream_t st);
+int dph_coarse_tc(dph_index* ix, int64_t n, int64_t lo, int64_t nl, int nprobe, unsigned long long* keys64, int32_t* key, float* cd, cudaStream_t st,
+                  const float* xr = nullptr, const float* C = nullptr);
 int dph_launch_coarse_merge(const unsigned long long* keys, int W, int64_t n, int nprobe, int32_t* key, float* cd, cudaStream_t st,
                             unsigned long long* keys64 = nullptr);
 int dph_launch_lut(const float* xr, int64_t n, const float* pq, float* lut_canon, float* lutmax, float* lutmin, float* lutmaxv,
@@ -171,3 +173,11 @@ int dph_scan_setup_attrs();
 // ---- encode.cu ----
 int64_t dph_encode_chunk(const dph_index* ix);
 int dph_encode_rows(dph_index* ix, const float* x_dev, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad);
+// Top-1 coarse list of n <= dph_encode_chunk rows xr [n, d] against centroids C [nlist, d]: the encoding's assignment (tensor-core
+// candidates + exact re-rank where the shape allows, else the SIMT sequential-k GEMM; smallest list id on a tie).  ix->S must hold
+// the n x nlist (padded to 128) scores.  key [n] int32, cd [n] the top-1 score.
+int dph_coarse_top1(dph_index* ix, const float* xr, const float* C, int64_t n, int32_t* key, float* cd, cudaStream_t st);
+// PQ codes [n, 96] of the residuals xr - C[key] under the codebooks pq (pq_encode_kernel); list_out [n] int64 receives key.
+int dph_pq_assign(dph_index* ix, const float* xr, const float* C, const int32_t* key, const float* pq, int64_t n, int64_t* list_out,
+                  uint8_t* codes_out, cudaStream_t st);
+__global__ void nonfinite_kernel(const float* __restrict__ x, long long count, int* __restrict__ bad);

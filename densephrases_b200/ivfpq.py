@@ -202,6 +202,112 @@ class IvfPqIndex:
         """The largest total of the last remove's temporary device allocations, in bytes."""
         return int(L.lib().dph_index_last_remove_tmp_bytes(self._h))
 
+    # ---- training (faiss index.train, build_phrase_index.py:96-142; DESIGN.md 3.3) -------------------------
+    def _train_input(self, x):
+        """-> (pointer, n, mem, keepalive) for numpy or a CUDA float32 tensor [n, d]."""
+        if isinstance(x, np.ndarray):
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            return _np_ptr(x), self._rows(x), L.MEM_HOST, x
+        import torch
+        if not (x.is_cuda and x.dtype == torch.float32):
+            raise TypeError("train: expected a numpy array or a float32 CUDA tensor")
+        x = x.contiguous()
+        self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
+        return x.data_ptr(), self._rows(x), L.MEM_DEVICE, x
+
+    def train_coarse(self, x, niter=10, seed=1234, max_points_per_centroid=256, hot_start=False):
+        """Spherical k-means of the coarse quantizer on x A^T (the handle's OPQ matrix) -> (obj [niter] f64, nsplit [niter] i64):
+        the summed inner products of the assignment before each update and the empty clusters re-seeded by splits.  hot_start keeps
+        the current centroids instead of drawing new ones."""
+        p, n, mem, keep = self._train_input(x)
+        if n < 39 * self.nlist:
+            import warnings
+            warnings.warn(f"train_coarse: {n} training points for {self.nlist} centroids; faiss wants at least {39 * self.nlist}")
+        obj = np.zeros(max(niter, 1), dtype=np.float64)
+        nsplit = np.zeros(max(niter, 1), dtype=np.int64)
+        L.check(L.lib().dph_index_train_coarse(self._h, p, n, int(niter), C.c_uint64(seed), int(max_points_per_centroid), int(bool(hot_start)),
+                                                mem, _np_ptr(obj), _np_ptr(nsplit)))
+        del keep
+        return obj[:niter], nsplit[:niter]
+
+    def train_pq(self, x, niter=25, seed=1234, max_points_per_centroid=256, hot_start=False, residual=True):
+        """96 L2 k-means of the PQ codebooks on the residuals x A^T - C[top-1 list] (residual=False: on x A^T, OPQ's case)."""
+        p, n, mem, keep = self._train_input(x)
+        L.check(L.lib().dph_index_train_pq(self._h, p, n, int(niter), C.c_uint64(seed), int(max_points_per_centroid), int(bool(hot_start)),
+                                            int(bool(residual)), mem))
+        del keep
+
+    def encode_pq(self, x):
+        """PQ codes of x A^T without a coarse residual: numpy [n,d] -> [n,96] u8 numpy | torch cuda -> torch cuda."""
+        if isinstance(x, np.ndarray):
+            x = np.ascontiguousarray(x, dtype=np.float32)
+            codes = np.empty((self._rows(x), 96), dtype=np.uint8)
+            L.check(L.lib().dph_index_encode_pq(self._h, _np_ptr(x), len(x), _np_ptr(codes), L.MEM_HOST))
+            return codes
+        import torch
+        assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+        codes = torch.empty((self._rows(x), 96), dtype=torch.uint8, device=x.device)
+        self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
+        L.check(L.lib().dph_index_encode_pq(self._h, x.data_ptr(), x.shape[0], codes.data_ptr(), L.MEM_DEVICE))
+        return codes
+
+    def train_opq(self, x, niter=10, seed=1234, niter_pq=40, niter_pq_hot=4, max_train_points=65536):
+        """faiss OPQMatrix::train: from a seeded random rotation, alternate PQ training on x R^T (niter_pq passes the first time, then
+        niter_pq_hot with hot start) and the orthogonal Procrustes update R = (U V^T)^T of svd(x^T y), y = decode(encode(x R^T)).  The
+        PQ passes run on the GPU; the 768 x 768 cross-covariance and its SVD are fp64 torch.  Sets and returns the OPQ matrix."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        n = int(x.shape[0])
+        rows = np.arange(n) if n <= max_train_points else np.sort(np.random.default_rng(seed).choice(n, max_train_points, replace=False))
+        xs = torch.as_tensor(x[rows] if isinstance(x, np.ndarray) else x[torch.as_tensor(rows, device=x.device)]).to(dev, torch.float32).contiguous()
+        g = torch.Generator().manual_seed(seed)
+        R = torch.linalg.qr(torch.randn((self.d, self.d), generator=g, dtype=torch.float64))[0].to(dev)
+        xd = xs.double()
+        for it in range(niter):
+            self.set_opq(R.float().cpu().numpy())
+            self.train_pq(xs, niter=niter_pq if it == 0 else niter_pq_hot, seed=seed, max_points_per_centroid=max_train_points,
+                          hot_start=it > 0, residual=False)
+            torch.cuda.current_stream(dev).synchronize()
+            codes = self.encode_pq(xs).long()
+            pq = torch.from_numpy(self.pq_codebooks()).to(dev)
+            y = pq[torch.arange(96, device=dev)[None, :], codes].reshape(len(xs), self.d)
+            u, _, vt = torch.linalg.svd(xd.T @ y.double())
+            R = (u @ vt).T.contiguous()
+        A = R.float().cpu().numpy()
+        self.set_opq(A)
+        return A
+
+    def train(self, x, niter=10, niter_pq=25, opq_niter=10, seed=1234, max_points_per_centroid=256):
+        """== faiss index.train(x) of IndexPreTransform(OPQMatrix, IndexIVFPQ(IndexFlatIP)): OPQ (skipped with opq_niter=0, which
+        keeps the current matrix), then the coarse quantizer, then the PQ on residuals, as IndexPreTransform::train does.  x: numpy or a
+        CUDA float32 tensor [n, 768].  Leaves a trained, empty index -> dict(obj, nsplit) of the coarse iterations."""
+        if self.ntotal:
+            raise RuntimeError("train: the index holds vectors")
+        if opq_niter > 0:
+            self.train_opq(x, niter=opq_niter, seed=seed)
+        obj, nsplit = self.train_coarse(x, niter=niter, seed=seed, max_points_per_centroid=max_points_per_centroid)
+        self.train_pq(x, niter=niter_pq, seed=seed, max_points_per_centroid=max_points_per_centroid, residual=True)
+        self.set_lists(np.zeros(self.nlist, np.int64), np.zeros((0, 96), np.uint8))
+        return dict(obj=obj, nsplit=nsplit)
+
+    def centroids(self):
+        """-> [nlist, d] f32: the coarse centroids (rotated space)."""
+        out = np.empty((self.nlist, self.d), dtype=np.float32)
+        L.check(L.lib().dph_index_get_centroids(self._h, _np_ptr(out), L.MEM_HOST))
+        return out
+
+    def pq_codebooks(self):
+        """-> [96, 256, 8] f32: the PQ codebooks."""
+        out = np.empty((96, 256, 8), dtype=np.float32)
+        L.check(L.lib().dph_index_get_pq(self._h, _np_ptr(out), L.MEM_HOST))
+        return out
+
+    def last_train_ms(self):
+        """With set_profile(True): stage times of the last train_coarse / train_pq in ms (assign, sort + update, split + renorm)."""
+        out = np.zeros(3, dtype=np.float32)
+        L.check(L.lib().dph_index_last_train_ms(self._h, _np_ptr(out)))
+        return out
+
     # ---- attributes ---------------------------------------------------------------------------
     @property
     def ntotal(self):

@@ -16,6 +16,10 @@
  *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
  *   dph_index_remove_ids        <- index.remove_ids(IDSelectorBatch(ids) | IDSelectorRange(lo, hi)) (faiss 1.6.x IndexIVF)
  *   dph_index_sync_list_len     <- (sharded remove) the list lengths faiss keeps in one process, exchanged between shards
+ *   dph_index_train_coarse      <- the coarse quantizer's k-means inside index.train(x)   build_phrase_index.py:96-142
+ *   dph_index_train_pq          <- ProductQuantizer::train inside index.train(x) (and OPQMatrix::train's PQ)
+ *   dph_index_encode_pq         <- OPQMatrix::train's pq_regular.compute_codes (PQ codes without a coarse residual)
+ *   dph_index_get_centroids/pq  <- the trained tables faiss.write_index stores
  *
  * Conventions: every function returns 0 on success, non-zero on error (dph_last_error() gives the
  * message; the Python layer raises RuntimeError like faiss' SWIG layer does).  `mem` arguments say
@@ -112,6 +116,32 @@ int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len);
  * empty selector resets both to zero. */
 int dph_index_last_remove_ms(const dph_index* ix, float* ms_out /* [3] */);
 int64_t dph_index_last_remove_tmp_bytes(const dph_index* ix);
+
+/* ---- training (replaces index.train(x) of build_phrase_index.py:96-142: faiss Clustering with cp.spherical over IndexFlatIP and
+ * ProductQuantizer::train on residuals; DESIGN.md 3.3 "Training the index") ----
+ * The trained tables are bit-identical to the oracle's ref_train_coarse / ref_train_pq: a sample of at most max_points_per_centroid
+ * x k rows drawn from rnd64(seed, ...), rotated by the handle's OPQ matrix; init from sample rows ranked by rnd64 (unless hot_start,
+ * which starts from the handle's current table); per iteration the encoding's own assignment, per-cluster sums in ascending row order,
+ * faiss' split of empty clusters with the repo's draws, and (coarse) renormalisation to unit norm.  x [n, d] fp32 (mem: host or
+ * device).  Only the rotated sample stays on the device.  Rejected, with the index unchanged: a handle that holds vectors, no OPQ
+ * matrix, n < k (nlist, or 256 for the PQ), a non-finite value in a sampled row, too little device memory for the sample and the
+ * workspace; hot start without the table, train_pq with residual = 1 without centroids.  Synchronise the stream. */
+/* Coarse centroids [nlist, d]: niter iterations of spherical k-means (faiss' IVF default 10).  obj_out [niter] (may be NULL): the sum
+ * of the assigned inner products in fp64 before each update; nsplit_out [niter] (may be NULL): empty clusters re-seeded by a split. */
+int dph_index_train_coarse(dph_index* ix, const float* x, int64_t n, int niter, uint64_t seed, int64_t max_points_per_centroid,
+                           int hot_start, int mem, double* obj_out, int64_t* nsplit_out);
+/* PQ codebooks [96, 256, 8]: 96 independent L2 k-means of niter iterations (faiss default 25), assignment = the encoding's argmin.
+ * residual = 1: on xr - C[top-1 list] (IndexIVFPQ by_residual); 0: on xr itself (OPQ's PQ). */
+int dph_index_train_pq(dph_index* ix, const float* x, int64_t n, int niter, uint64_t seed, int64_t max_points_per_centroid,
+                       int hot_start, int residual, int mem);
+/* codes_out [n, 96] = PQ codes of x A^T without a coarse residual (the encoding's argmin, lowest codeword on a tie). */
+int dph_index_encode_pq(dph_index* ix, const float* x, int64_t n, uint8_t* codes_out, int mem);
+/* Read the tables back (for artifacts.write_faiss_index / save_container): C_out [nlist, d], pq_out [96, 256, 8]. */
+int dph_index_get_centroids(const dph_index* ix, float* C_out, int mem);
+int dph_index_get_pq(const dph_index* ix, float* pq_out, int mem);
+/* Measurement hook: with profiling on, the stage times of the last train_coarse / train_pq in ms, summed over its iterations:
+ * assignment, sort + update, split + renorm. */
+int dph_index_last_train_ms(const dph_index* ix, float* ms_out /* [3] */);
 
 /* ---- getters ---- */
 int64_t dph_index_ntotal(const dph_index* ix);       /* all shards */
