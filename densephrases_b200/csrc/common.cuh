@@ -129,18 +129,19 @@ struct DphPairWork {   // pair mode: the work queue of (list, block segment, ite
     int total_units;
     int next_unit;                  // queue head, advanced with atomicAdd by the scan CTAs; reset by the plan
 };
-// Quad mode: one fully resolved work item (list segment x group of <= 4 probing queries), written by the plan so that a scan CTA
-// starts an item from ONE 96-byte read (prefetched during the previous item) instead of a chain of dependent look-ups.
+// Quad mode: one fully resolved work item (list segment x group of <= 8 probing queries), written by the plan so that a scan CTA
+// starts an item from ONE 160-byte read (prefetched during the previous item) instead of a chain of dependent look-ups.
+#define DPH_QUAD_ITEM_Q 8           // queries per quad-mode work item: two packed tables of four
 struct __align__(16) DphUnit {
     long long blk;                  // first code block of the list in this shard's code array
     int len;                        // list length (vectors)
     unsigned bi0, bend;             // block range of this segment inside the list
-    int nq;                         // queries in the group (1..4); the unused slots repeat slot 0
+    int nq;                         // queries in the group (1..8); the unused slots repeat slot 0
     int list, pad;
-    unsigned q[4];                  // query numbers
-    unsigned gs[4];                 // canonical scan position of the list's first vector, per query
-    float base[4];                  // <xr, centroid> + the query's quantisation offset
-    float step[4];                  // the query's quantisation step
+    unsigned q[DPH_QUAD_ITEM_Q];    // query numbers
+    unsigned gs[DPH_QUAD_ITEM_Q];   // canonical scan position of the list's first vector, per query
+    float base[DPH_QUAD_ITEM_Q];    // <xr, centroid> + the query's quantisation offset
+    float step[DPH_QUAD_ITEM_Q];    // the query's quantisation step
 };
 #define DPH_PAIR_SEG_MIN 128        // shortest segment worth rebuilding the packed 192 KB LUT for
 #define DPH_PAIR_UNITS_PER_CTA 16   // lists are cut only when the batch has fewer than this many whole-list units per CTA

@@ -673,7 +673,10 @@ static int search_chunk(dph_index* ix, const float* x_dev, int64_t n, int k, flo
     if (group == 2 && keep_pair > 1536 - DPH_SCAN_THREADS) group = 1;
     const bool pair = group > 1;
     const int keep_fast = group == 4 ? keep_quad : (group == 2 ? keep_pair : keep_single);
-    DPH_TRY(ix->cand.ensure(((size_t)(2 * grid + 2 * n + 2) + (pair ? (size_t)(n * nprobe + 2 * DPH_PAIR_UNITS_PER_CTA * grid + 2 * n + 16) : 0)) * keep_max * 8));
+    // group modes: query q's region holds nseg_q + blocks_q / per + 1 units of keep (plan_scan_kernel); summed over the batch,
+    // sum_q blocks_q <= (queries per item) * sum over items of blocks <= (queries per item) * per * UNITS_PER_CTA * grid
+    const size_t item_q = group == 4 ? DPH_QUAD_ITEM_Q : 2;
+    DPH_TRY(ix->cand.ensure(((size_t)(2 * grid + 2 * n + 2) + (pair ? (size_t)(n * nprobe + item_q * DPH_PAIR_UNITS_PER_CTA * grid + 2 * n + 16) : 0)) * keep_max * 8));
     DPH_TRY(ix->cand_off.ensure((size_t)(n + 1) * 8));
     DPH_TRY(ix->cand_cnt.ensure((size_t)n * 4));
     DPH_TRY(ix->gthr.ensure((size_t)n * 4));

@@ -10,7 +10,7 @@
 #define DPH_SCAN_WARPS (DPH_SCAN_THREADS / 32)
 #define DPH_CAND_CAP 3072          // shared-memory candidate buffer (u64 keys) per scan CTA
 #define DPH_PAIR_CAP 1280          // pair mode: one buffer per query of the pair
-#define DPH_QUAD_KEEP_MAX 256       // quad mode: QCAP (768) - scan threads (512), see scan.cu
+#define DPH_QUAD_KEEP_MAX 256       // quad mode: QCAP (512) - quad scan threads (256), see scan.cu
 
 #define DPH_KEEP_SLACK 32          // fast mode keeps k + slack candidates per CTA
 #define DPH_MAX_K 1024
@@ -25,7 +25,7 @@
 // pair / quad tables, the exact kernel and the exact re-scoring in the merge.
 #define DPH_LUTC_IDX(m, code) ((((m) >> 5) << 13) + ((code) << 5) + ((m) & 31))
 #define DPH_SEG_SMEM 256            // segment descriptors of one query kept in shared memory by the scan kernel
-#define DPH_L2_PREFETCH_ROUNDS 4    // scan kernel: bulk L2 prefetch distance, in rounds (one 3 KB block per warp per round)
+#define DPH_L2_PREFETCH_ROUNDS 2    // scan kernels: bulk L2 prefetch distance, in rounds (one 3 KB block per warp per round; tools/scan_floor.cu)
 
 struct DevBuf {            // grow-only device buffer
     void* p = nullptr;

@@ -832,7 +832,7 @@ struct PairPlanArgs {
     const int* key; long long nq_probes; int nprobe; const int* list_len; long long list_lo, list_hi, nlist; int grid;
     int* cnt; int* fill; int* off; long long* blockpre; unsigned* entries; DphPairWork* work;
     int* unitpre; unsigned long long* units;
-    int gsz;                       // queries per work item: 2 (pair-packed scan) or 4 (quad-packed scan)
+    int gsz;                       // queries per work item: 2 (pair-packed scan) or DPH_QUAD_ITEM_Q (quad-packed scan)
     DphUnit* udesc;                // quad mode (nullable): resolved unit descriptors, parallel to `units`
     const long long* blk_off; const float* cd; const unsigned* gdense; const float2* qparams;
 };
@@ -934,10 +934,10 @@ __global__ void pair_units_kernel(PairPlanArgs a) {
         DphUnit d;
         if (a.udesc) {
             d.blk = a.blk_off[l]; d.len = a.list_len[l]; d.list = (int)l; d.pad = 0;
-            d.nq = min(4, cnt - 4 * it);
-            const int e0 = a.off[l] + 4 * it;
+            d.nq = min(a.gsz, cnt - a.gsz * it);
+            const int e0 = a.off[l] + a.gsz * it;
 #pragma unroll
-            for (int i = 0; i < 4; i++) {
+            for (int i = 0; i < DPH_QUAD_ITEM_Q; i++) {
                 const unsigned e = a.entries[e0 + (i < d.nq ? i : 0)];
                 const long long q = e >> 10; const int r = (int)(e & 1023u);
                 const float2 pp = a.qparams[q];
@@ -983,7 +983,7 @@ int dph_launch_plan(dph_index* ix, int64_t n, int k, int keep, int grid, const i
         p.list_hi = ix->list_hi; p.nlist = ix->nlist; p.grid = grid; p.cnt = ix->pl_cnt.as<int>(); p.fill = ix->pl_fill.as<int>();
         p.off = ix->pl_off.as<int>(); p.blockpre = ix->pl_blockpre.as<long long>(); p.entries = ix->pl_entries.as<unsigned>();
         p.work = ix->pairwork.as<DphPairWork>(); p.unitpre = ix->pl_unitpre.as<int>(); p.units = ix->pl_units.as<unsigned long long>();
-        p.gsz = group;
+        p.gsz = group == 4 ? DPH_QUAD_ITEM_Q : group;         // quad mode: an item runs one code read through two packed tables
         p.udesc = group == 4 ? ix->pl_udesc.as<DphUnit>() : nullptr;
         p.blk_off = (const long long*)ix->blk_off; p.cd = ix->cd.as<float>(); p.gdense = ix->gdense.as<unsigned>(); p.qparams = ix->qparams.as<float2>();
         DPH_CUDA(cudaMemsetAsync(p.cnt, 0, (size_t)ix->nlist * 4, st));

@@ -341,15 +341,15 @@ template <int C> __device__ __forceinline__ void pair_chunk(const uint4& v, unsi
     pair_word<C * 16 + 8>(v.z, y, a0, a1, a2, a3);
     pair_word<C * 16 + 12>(v.w, y, a0, a1, a2, a3);
 }
-template <int CAP>
+template <int CAP, int NTH>     // NTH: the block's thread count
 __device__ __forceinline__ void compact_buffer(unsigned long long* cb, int* cnt, unsigned* thr, int keep, unsigned* gthr_q, SelectScratch* sc) {
     const int tid = threadIdx.x;
     const int n = *cnt;
     unsigned long long pivot = block_radix_select([&](int i) { return cb[i]; }, n, keep, sc);
-    constexpr int PER = (CAP + NT - 1) / NT;
+    constexpr int PER = (CAP + NTH - 1) / NTH;
     unsigned long long mine[PER];
 #pragma unroll
-    for (int e = 0; e < PER; e++) { int i = tid + e * NT; mine[e] = (i < n) ? cb[i] : 0ull; }
+    for (int e = 0; e < PER; e++) { int i = tid + e * NTH; mine[e] = (i < n) ? cb[i] : 0ull; }
     __syncthreads();
     if (tid == 0) *cnt = 0;
     __syncthreads();
@@ -475,8 +475,8 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(PairScanArgs a) {
             }
             if (!more && !counted) { counted = true; if (lane == 0) atomicAdd(&sh->ndone, 1); }
             __syncthreads();
-            if (sh->cnt[0] > a.keep) compact_buffer<PCAP>(sh->cbuf[0], &sh->cnt[0], &sh->thr[0], a.keep, a.gthr + qa, &sh->sc);
-            if (sh->cnt[1] > a.keep) compact_buffer<PCAP>(sh->cbuf[1], &sh->cnt[1], &sh->thr[1], a.keep, a.gthr + qb, &sh->sc);
+            if (sh->cnt[0] > a.keep) compact_buffer<PCAP, NT>(sh->cbuf[0], &sh->cnt[0], &sh->thr[0], a.keep, a.gthr + qa, &sh->sc);
+            if (sh->cnt[1] > a.keep) compact_buffer<PCAP, NT>(sh->cbuf[1], &sh->cnt[1], &sh->thr[1], a.keep, a.gthr + qb, &sh->sc);
             if (tid == 0) {
                 unsigned ga = *((volatile unsigned*)(a.gthr + qa));
                 if (ga > sh->thr[0]) sh->thr[0] = ga;
@@ -511,36 +511,53 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(PairScanArgs a) {
 //     accb  = sum of PRMT(word -> [b1, 0, b3, 0]) = S1 + 2^16 S3     (exact: both lanes stay below 2^16)
 // and decoded once per vector:  sraw - (accb << 8) = S0 + 2^16 S2 (exact, < 2^32).
 // The integer sums are exact; the only error is the quantisation (<= 0.5 step per entry), which the plan folds into eps, so the
-// same proof + exact canonical re-scoring applies (merge_kernel).  Work items are (list segment, group of <= 4 probing queries).
+// same proof + exact canonical re-scoring applies (merge_kernel).
+//
+// Work items are (list segment, group of <= 8 probing queries): every code block is read from HBM once into registers and run
+// through one packed table (queries 0-3) or two (queries 4-7 as well), so a list probed by up to 8 queries of the batch is read
+// once, by one CTA.  Two tables fit in shared memory because the table is WRAP-FREE: a row holds only the 32 real words, and the
+// lane rotation lives in the address instead -- at step t lane l reads word (l + t) & 31, whose byte offset comes from per-lane
+// registers (11 registers of three offsets and a zero byte; the dynamic window's top address byte is 0, checked at setup).  One
+// PRMT still builds the address (rotated offset | code << 8) and serves both tables; the table, segment and half-row go in the
+// LDS immediate.  Rows stay 256 bytes: three 64 KB regions, region r row c = two 128-byte halves:
+//     region 0: [table 0 segment 0 | table 0 segment 1]   region 1: [table 1 segment 0 | table 1 segment 1]
+//     region 2: [table 0 segment 2 | table 1 segment 2]
+// A lane's bank is still (l + t) mod 32, so the gathers stay conflict-free.
 // =================================================================================================
-#define QCAP 768
+#define QNT 256                    // quad kernel threads: eight candidate buffers must fit next to the two 96 KB tables
+#define QNW (QNT / 32)
+#define QCAP 512                   // QCAP - QNT = DPH_QUAD_KEEP_MAX (each warp adds <= 32 per buffer after the latch is polled)
+#define SMEM_QUAD_TABLES (3 * 65536)
+static_assert(QCAP - QNT == DPH_QUAD_KEEP_MAX, "quad latch margin");
 struct QuadShared {
-    unsigned long long cbuf[4][QCAP];
+    unsigned long long cbuf[DPH_QUAD_ITEM_Q][QCAP];
     SelectScratch sc;
     DphUnit desc[2];                 // current item / next item (fetched with cp.async while the current one is scanned)
-    int cnt[4]; unsigned thr[4]; int base[4]; int ndone; int ndone_snap; int unit; int full;
-    long long qs[4];                 // the group's queries (shared copy: indexed by thread id in the publish step)
+    int cnt[DPH_QUAD_ITEM_Q]; unsigned thr[DPH_QUAD_ITEM_Q]; int base[DPH_QUAD_ITEM_Q]; int ndone; int ndone_snap; int unit; int full;
+    long long qs[DPH_QUAD_ITEM_Q];   // the group's queries (shared copy: indexed by thread id in the publish step)
 };
 // 32-bit add on the FMA pipe: d = a * one + c with `one` a kernel parameter holding 1 (opaque to ptxas, so the multiply-add is not
-// folded back into an IADD3).  The quad scan is bound by the ALU pipe (PRMT + IADD3, one warp instruction per two cycles per
-// sub-partition, B300_MICROARCH "fma vs alu split"); IMAD issues on the otherwise idle FMA pipe at the same rate.
+// folded back into an IADD3).  The quad scan's gathers are bound by the ALU pipe (PRMT + IADD3, one warp instruction per two cycles
+// per sub-partition); IMAD issues on the otherwise idle FMA pipe at the same rate.
 __device__ __forceinline__ unsigned imad_add(unsigned x, unsigned one, unsigned c) {
     unsigned d;
     asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(d) : "r"(x), "r"(one), "r"(c));
     return d;
 }
+// Four gathers of one table (code bytes T0..T0+3 of a segment, addresses built by quad_word) into that table's sums.
 // IMADL: how many of the running-sum additions go to the FMA pipe: 0 = none (all IADD3), 1 = the raw sums, 2 = the raw sums and
 // half of the odd-byte sums, 3 = all of them.
-template <int T0, int IMADL> __device__ __forceinline__ void quad_word(unsigned wv, unsigned y, unsigned one, unsigned (&sr)[4], unsigned (&ab)[4]) {
-    constexpr int TB = DPH_DYN_SMEM_BASE + (T0 >> 5) * 65536 + (T0 & 31) * 4;
+template <int T0, int TAB, int IMADL> __device__ __forceinline__ void quad_gather(const unsigned (&ad)[4], unsigned one, unsigned (&sr)[4], unsigned (&ab)[4]) {
+    constexpr int S = T0 >> 5;
+    constexpr int TB = DPH_DYN_SMEM_BASE + (S < 2 ? TAB : 2) * 65536 + (S < 2 ? S : TAB) * 128;
     constexpr int A = (T0 >> 2) & 1;                  // two accumulator sets, alternating per code word
-    const unsigned w0 = lds_imm_u32<TB + 0>(__byte_perm(wv, y, 0x7504));
-    const unsigned w1 = lds_imm_u32<TB + 4>(__byte_perm(wv, y, 0x7514));
-    const unsigned w2 = lds_imm_u32<TB + 8>(__byte_perm(wv, y, 0x7524));
-    const unsigned w3 = lds_imm_u32<TB + 12>(__byte_perm(wv, y, 0x7534));
+    const unsigned w0 = lds_imm_u32<TB>(ad[0]);
+    const unsigned w1 = lds_imm_u32<TB>(ad[1]);
+    const unsigned w2 = lds_imm_u32<TB>(ad[2]);
+    const unsigned w3 = lds_imm_u32<TB>(ad[3]);
     // 8-bit entries: the odd bytes are widened per gather (a lane-wise add of two words could carry).  A 7-bit variant that widens
-    // once per TWO gathers is 11 % faster (ncu r2d) but doubles eps, and then the exactness proof fails for ~10 % of the queries at
-    // C2 (measured); the exact fallback costs far more than it saves.
+    // once per TWO gathers is faster but doubles eps, and then the exactness proof fails for ~10 % of the queries at C2 (measured
+    // on B200); the exact fallback costs far more than it saves.
     if (IMADL >= 1) {
         sr[2 * A] = imad_add(w1, one, imad_add(w0, one, sr[2 * A]));
         sr[2 * A + 1] = imad_add(w3, one, imad_add(w2, one, sr[2 * A + 1]));
@@ -558,11 +575,24 @@ template <int T0, int IMADL> __device__ __forceinline__ void quad_word(unsigned 
         ab[2 * A + 1] += e2 + e3;
     }
 }
-template <int C, int IMADL> __device__ __forceinline__ void quad_chunk(const uint4& v, unsigned y, unsigned one, unsigned (&sr)[4], unsigned (&ab)[4]) {
-    quad_word<C * 16 + 0, IMADL>(v.x, y, one, sr, ab);
-    quad_word<C * 16 + 4, IMADL>(v.y, y, one, sr, ab);
-    quad_word<C * 16 + 8, IMADL>(v.z, y, one, sr, ab);
-    quad_word<C * 16 + 12, IMADL>(v.w, y, one, sr, ab);
+// Byte b of rot[r] = ((lane + 3r + b) & 31) * 4, the rotated word offset of step t = 3r + b of a segment; byte 3 is zero.
+// Selector of code byte i at step t: [rotated offset of t, code byte i, 0, 0].
+template <int T> struct RotSel { static constexpr int reg = (T & 31) / 3, sel = 0x7700 | (4 + (T & 31) % 3); };
+template <int T0, int NTAB, int IMADL> __device__ __forceinline__ void quad_word(unsigned wv, const unsigned (&rot)[11], unsigned one,
+                                                                                  unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
+    const unsigned ad[4] = {__byte_perm(wv, rot[RotSel<T0>::reg], RotSel<T0>::sel | 0x00),
+                            __byte_perm(wv, rot[RotSel<T0 + 1>::reg], RotSel<T0 + 1>::sel | 0x10),
+                            __byte_perm(wv, rot[RotSel<T0 + 2>::reg], RotSel<T0 + 2>::sel | 0x20),
+                            __byte_perm(wv, rot[RotSel<T0 + 3>::reg], RotSel<T0 + 3>::sel | 0x30)};
+    quad_gather<T0, 0, IMADL>(ad, one, sr[0], ab[0]);
+    if (NTAB == 2) quad_gather<T0, 1, IMADL>(ad, one, sr[1], ab[1]);
+}
+template <int C, int NTAB, int IMADL> __device__ __forceinline__ void quad_chunk(const uint4& v, const unsigned (&rot)[11], unsigned one,
+                                                                                   unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
+    quad_word<C * 16 + 0, NTAB, IMADL>(v.x, rot, one, sr, ab);
+    quad_word<C * 16 + 4, NTAB, IMADL>(v.y, rot, one, sr, ab);
+    quad_word<C * 16 + 8, NTAB, IMADL>(v.z, rot, one, sr, ab);
+    quad_word<C * 16 + 12, NTAB, IMADL>(v.w, rot, one, sr, ab);
 }
 // append with an overflow latch: the round loop polls ONE flag instead of every buffer's counter
 __device__ __forceinline__ void warp_append_latch(bool pass, unsigned long long key, unsigned long long* cb, int* cnt, int* full, int lane) {
@@ -570,7 +600,7 @@ __device__ __forceinline__ void warp_append_latch(bool pass, unsigned long long 
     if (pm) {
         int basep = 0;
         const int np = __popc(pm);
-        if (lane == 0) { basep = atomicAdd(cnt, np); if (basep + np > QCAP - NT) *((volatile int*)full) = 1; }
+        if (lane == 0) { basep = atomicAdd(cnt, np); if (basep + np > QCAP - QNT) *((volatile int*)full) = 1; }
         basep = __shfl_sync(0xffffffffu, basep, 0);
         if (pass) { int p = basep + __popc(pm & ((1u << lane) - 1u)); if (p < QCAP) cb[p] = key; }
     }
@@ -578,96 +608,202 @@ __device__ __forceinline__ void warp_append_latch(bool pass, unsigned long long 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" :: "r"((unsigned)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
+// float image of a threshold (0xFFFFFFFF = "never passes" for the empty slots of a short group -> +inf)
+__device__ __forceinline__ float quad_thr_f(unsigned t) {
+    return t == 0xFFFFFFFFu ? __int_as_float(0x7f800000) : (t == 0u ? -__int_as_float(0x7f800000) : dph_fkey_inv(t));
+}
 
-// Item start-up is kept off the critical path (at C2 / C4 list lengths an item is only 30-50 rounds long): the plan resolves every
-// unit into one DphUnit record; the record of the NEXT unit is fetched into shared memory with cp.async while the current one is
-// scanned (its queue index was requested at the start of the current item); the first code blocks of an item are requested BEFORE the
-// packed LUT is built, so the HBM latency overlaps the build; the build reads only the 32 real bytes of every 64-byte table row and
-// writes the wrap copy itself (half the L2 traffic).
+#ifdef DPH_SCAN_PHASES
+// Per-CTA %globaltimer phase totals of thread 0 (build -DDPH_SCAN_PHASES): packed-table build, scan rounds (to the epoch barrier),
+// compaction barriers, candidate publish; summed over the CTAs of a launch and printed by the last CTA to finish.
+__device__ unsigned long long g_quad_phase_ns[4];
+__device__ unsigned g_quad_phase_ctas;
+__device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
+#define QPH_MARK(i) do { if (threadIdx.x == 0) { const unsigned long long t_ = globaltimer_ns(); ph[i] += t_ - ph_t; ph_t = t_; } } while (0)
+#else
+#define QPH_MARK(i) do { } while (0)
+#endif
+
+// The scan of one item over its block range with NTAB packed tables: rounds until a candidate buffer may overflow or the warp is out
+// of blocks, then a barrier, the compaction of the buffers over keep and the refresh of the thresholds; until every warp is done.
+template <int NTAB, int IMADL>
+__device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
+                                                 unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, unsigned long long* ph,
+                                                 unsigned long long& ph_t) {
+    (void)ph; (void)ph_t;
+    const int lane = threadIdx.x & 31;
+    const int len = dsc->len, nq = dsc->nq;
+    const unsigned bend = dsc->bend;
+    constexpr int NS = 4 * NTAB;
+    unsigned gsv[NS]; float stepv[NS], basev[NS], tf[NS]; unsigned thr[NS];
+#pragma unroll
+    for (int i = 0; i < NS; i++) { gsv[i] = dsc->gs[i]; basev[i] = dsc->base[i]; stepv[i] = dsc->step[i]; thr[i] = sh->thr[i]; tf[i] = quad_thr_f(thr[i]); }
+    bool more = b < bend, counted = false;
+    while (true) {
+        while (more) {
+            if (*((volatile int*)&sh->full)) break;
+            uint4 cur6[6];
+#pragma unroll
+            for (int c6 = 0; c6 < 6; c6++) cur6[c6] = nxt[c6];
+            const unsigned bcur = b;
+            if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16)); bp += QNW; }
+            b += QNW;
+            more = b < bend;
+            if (more) {
+                const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+#pragma unroll
+                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+            }
+            unsigned sr[2][4] = {}, ab[2][4] = {};
+            quad_chunk<0, NTAB, IMADL>(cur6[0], rot, one, sr, ab);
+            quad_chunk<1, NTAB, IMADL>(cur6[1], rot, one, sr, ab);
+            quad_chunk<2, NTAB, IMADL>(cur6[2], rot, one, sr, ab);
+            quad_chunk<3, NTAB, IMADL>(cur6[3], rot, one, sr, ab);
+            quad_chunk<4, NTAB, IMADL>(cur6[4], rot, one, sr, ab);
+            quad_chunk<5, NTAB, IMADL>(cur6[5], rot, one, sr, ab);
+            const unsigned j = bcur * 32u + lane;
+            const bool valid = (int)j < len;
+            // thresholds are compared in the float domain (one FSETP per query); the order-preserving integer key is built only for
+            // the rare vector that passes.  (float)(unsigned short) converts a 16-bit half of the register without a mask / shift.
+            float f[NS]; bool p[NS]; bool any = false;
+#pragma unroll
+            for (int tb = 0; tb < NTAB; tb++) {
+                const unsigned SR = (sr[tb][0] + sr[tb][1]) + (sr[tb][2] + sr[tb][3]);
+                const unsigned AB = (ab[tb][0] + ab[tb][1]) + (ab[tb][2] + ab[tb][3]);      // S1 | S3 << 16
+                const unsigned AE = SR - (AB << 8);                                         // S0 | S2 << 16
+                f[4 * tb + 0] = fmaf(stepv[4 * tb + 0], (float)(unsigned short)(AE), basev[4 * tb + 0]);
+                f[4 * tb + 1] = fmaf(stepv[4 * tb + 1], (float)(unsigned short)(AB), basev[4 * tb + 1]);
+                f[4 * tb + 2] = fmaf(stepv[4 * tb + 2], (float)(unsigned short)(AE >> 16), basev[4 * tb + 2]);
+                f[4 * tb + 3] = fmaf(stepv[4 * tb + 3], (float)(unsigned short)(AB >> 16), basev[4 * tb + 3]);
+            }
+#pragma unroll
+            for (int i = 0; i < NS; i++) { p[i] = valid && f[i] >= tf[i]; any = any || p[i]; }
+            if (__any_sync(0xffffffffu, any)) {
+#pragma unroll
+                for (int i = 0; i < NS; i++) {
+                    const unsigned k = dph_fkey(f[i]);
+                    warp_append_latch(p[i] && k >= thr[i], ((unsigned long long)k << 32) | (unsigned long long)(0xFFFFFFFFu - (gsv[i] + j)),
+                                      sh->cbuf[i], &sh->cnt[i], &sh->full, lane);
+                }
+            }
+        }
+        if (!more && !counted) { counted = true; if (lane == 0) atomicAdd(&sh->ndone, 1); }
+        __syncthreads();
+        QPH_MARK(1);
+#pragma unroll 1
+        for (int i = 0; i < nq; i++)
+            if (sh->cnt[i] > a.keep) compact_buffer<QCAP, QNT>(sh->cbuf[i], &sh->cnt[i], &sh->thr[i], a.keep, a.gthr + sh->qs[i], &sh->sc);
+        if (threadIdx.x == 0) {
+            for (int i = 0; i < nq; i++) { unsigned g = *((volatile unsigned*)(a.gthr + sh->qs[i])); if (g > sh->thr[i]) sh->thr[i] = g; }
+            sh->ndone_snap = sh->ndone;
+            sh->full = 0;
+        }
+        __syncthreads();
+        QPH_MARK(2);
+#pragma unroll
+        for (int i = 0; i < NS; i++) { thr[i] = sh->thr[i]; tf[i] = quad_thr_f(thr[i]); }
+        if (sh->ndone_snap == QNW) break;
+    }
+}
+
+// Item start-up is kept off the critical path: the plan resolves every unit into one DphUnit record; the record of the NEXT unit is
+// fetched into shared memory with cp.async while the current one is scanned (its queue index is requested at the start of the current
+// item, so that the fetch can be issued right after the table build); the first code blocks of an item are requested BEFORE the
+// packed tables are built, so the HBM latency overlaps the build; the build reads only the 32 real bytes of every 64-byte row of the
+// quantised tables.
 template <int IMADL>
-__global__ void __launch_bounds__(NT, 1) scan_quad_kernel(PairScanArgs a) {
+__global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
     unsigned char* const smem = dph_smem;
-    QuadShared* sh = reinterpret_cast<QuadShared*>(smem + SMEM_LUT_FAST);
+    QuadShared* sh = reinterpret_cast<QuadShared*>(smem + SMEM_QUAD_TABLES);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int total_units = a.work->total_units;
-    const unsigned ywin = (((unsigned)__cvta_generic_to_shared(dph_smem)) & 0xFF000000u) | ((unsigned)lane * 4u);
     const unsigned char* lut8 = reinterpret_cast<const unsigned char*>(a.lutq);
     const unsigned one = a.one;
+    unsigned rot[11];
+#pragma unroll
+    for (int r = 0; r < 11; r++) {
+        unsigned v = 0;
+#pragma unroll
+        for (int bb = 0; bb < 3; bb++)
+            if (3 * r + bb < 32) v |= (unsigned)(((lane + 3 * r + bb) & 31) * 4) << (8 * bb);
+        rot[r] = v;
+    }
+    unsigned long long ph[4] = {0ull, 0ull, 0ull, 0ull}, ph_t = 0ull;
+#ifdef DPH_SCAN_PHASES
+    if (tid == 0) ph_t = globaltimer_ns();
+#endif
 
     if (tid == 0) sh->unit = atomicAdd(a.next_unit, 1);
     __syncthreads();
-    {
-        const int u = sh->unit;
-        if (u >= total_units) return;
-        if (tid < (int)(sizeof(DphUnit) / 16)) reinterpret_cast<uint4*>(&sh->desc[0])[tid] = __ldg(reinterpret_cast<const uint4*>(a.udesc + u) + tid);
-    }
-    __syncthreads();
     int cur = 0;
-    while (true) {
+    bool any_unit = sh->unit < total_units;
+    if (any_unit && tid < (int)(sizeof(DphUnit) / 16))
+        reinterpret_cast<uint4*>(&sh->desc[0])[tid] = __ldg(reinterpret_cast<const uint4*>(a.udesc + sh->unit) + tid);
+    __syncthreads();
+    while (any_unit) {
         int next_u = 0;
-        if (tid == 0) next_u = atomicAdd(a.next_unit, 1);          // consumed after the LUT build (fetch of the next record)
+        if (tid == 0) next_u = atomicAdd(a.next_unit, 1);          // consumed after the table build (fetch of the next record)
         const DphUnit* dsc = &sh->desc[cur];
-        const int len = dsc->len, nq = dsc->nq;
+        const int nq = dsc->nq;
+        const int ntab = nq > 4 ? 2 : 1;
         const unsigned bi0 = dsc->bi0, bend = dsc->bend;
         const uint4* lbase = reinterpret_cast<const uint4*>(a.codes + dsc->blk * DPH_BLK_BYTES);
-        unsigned qv[4], gsv[4]; float stepv[4], basev[4];
-#pragma unroll
-        for (int i = 0; i < 4; i++) { qv[i] = dsc->q[i]; gsv[i] = dsc->gs[i]; basev[i] = dsc->base[i]; stepv[i] = dsc->step[i]; }
 
-        // ---- first code blocks: L2 prefetch + this warp's first block into registers, in flight during the LUT build ----
+        // ---- first code blocks: L2 prefetch + this warp's first block into registers, in flight during the table build ----
         unsigned b = bi0 + warp, bp = bi0 + warp;
         uint4 nxt[6];
 #pragma unroll 1
-        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += NW)
+        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += QNW)
             if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16));
-        bool more = b < bend;
-        if (more) {
+        if (b < bend) {
             const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
             for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
         }
-        unsigned g4[4] = {0u, 0u, 0u, 0u};
-        if (tid == 0) {
+        unsigned gq = 0xFFFFFFFFu;
+        if (tid < DPH_QUAD_ITEM_Q && tid < nq) gq = *((volatile unsigned*)(a.gthr + dsc->q[tid]));
+        {   // ---- packed tables: byte j of a word of table t = query 4t + j's 8-bit entry, wrap-free layout (see above) ----
+            const unsigned* src[DPH_QUAD_ITEM_Q];
 #pragma unroll
-            for (int i = 0; i < 4; i++) g4[i] = i < nq ? *((volatile unsigned*)(a.gthr + qv[i])) : 0xFFFFFFFFu;
-        }
-        {   // ---- packed LUT: byte i of every word = query i's 8-bit entry, [3][256][64] scan layout (words 32..62 = words 0..30) ----
-            const unsigned* T0p = reinterpret_cast<const unsigned*>(lut8 + (size_t)qv[0] * DPH_LUT_SCAN_FLOATS);
-            const unsigned* T1p = reinterpret_cast<const unsigned*>(lut8 + (size_t)qv[1] * DPH_LUT_SCAN_FLOATS);
-            const unsigned* T2p = reinterpret_cast<const unsigned*>(lut8 + (size_t)qv[2] * DPH_LUT_SCAN_FLOATS);
-            const unsigned* T3p = reinterpret_cast<const unsigned*>(lut8 + (size_t)qv[3] * DPH_LUT_SCAN_FLOATS);
+            for (int i = 0; i < DPH_QUAD_ITEM_Q; i++) src[i] = reinterpret_cast<const unsigned*>(lut8 + (size_t)dsc->q[i] * DPH_LUT_SCAN_FLOATS);
             uint4* dst = reinterpret_cast<uint4*>(smem);
-            // (row, group of four real words): a quarter-warp moves one row.  The empty slots of a short group repeat query 0 (their
-            // byte lanes are summed like the others and never pass: threshold +inf), so all four loads are unconditional and a
-            // thread keeps 24 of them in flight.
-            constexpr int LB = 6;
+            // (table, row, group of four real words): a quarter-warp moves one 128-byte half-row.  The empty slots of a short group
+            // repeat query 0 (their byte lanes are summed like the others and never pass: threshold +inf), so all four loads are
+            // unconditional and a thread keeps 24 of them in flight.
+            constexpr int LB = 6, PER_TAB = 768 * 8;
+            static_assert(PER_TAB % (QNT * LB) == 0, "a batch of the build stays inside one table");
 #pragma unroll 1
-            for (int i0 = tid; i0 < 768 * 8; i0 += NT * LB) {
+            for (int i0 = tid; i0 < ntab * PER_TAB; i0 += QNT * LB) {
+                const int tb = i0 >= PER_TAB;
+                const unsigned* T0p = tb ? src[4] : src[0];
+                const unsigned* T1p = tb ? src[5] : src[1];
+                const unsigned* T2p = tb ? src[6] : src[2];
+                const unsigned* T3p = tb ? src[7] : src[3];
+                const int ib = i0 - tb * PER_TAB;
                 unsigned va[LB], vb[LB], vc[LB], vd[LB];
 #pragma unroll
                 for (int e = 0; e < LB; e++) {
-                    const int i = i0 + e * NT, src = (i >> 3) * 16 + (i & 7);
-                    va[e] = __ldg(T0p + src); vb[e] = __ldg(T1p + src); vc[e] = __ldg(T2p + src); vd[e] = __ldg(T3p + src);
+                    const int i = ib + e * QNT, s = (i >> 3) * 16 + (i & 7);
+                    va[e] = __ldg(T0p + s); vb[e] = __ldg(T1p + s); vc[e] = __ldg(T2p + s); vd[e] = __ldg(T3p + s);
                 }
 #pragma unroll
                 for (int e = 0; e < LB; e++) {
-                    const int i = i0 + e * NT, row = i >> 3, cg = i & 7;
+                    const int i = ib + e * QNT, row = i >> 3, cg = i & 7;
+                    const int seg = row >> 8, code = row & 255;
+                    const int region = seg < 2 ? tb : 2, half = seg < 2 ? seg : tb;
                     const unsigned t0 = __byte_perm(va[e], vb[e], 0x5140), t1 = __byte_perm(va[e], vb[e], 0x7362);     // [a0 b0 a1 b1], [a2 b2 a3 b3]
                     const unsigned u0 = __byte_perm(vc[e], vd[e], 0x5140), u1 = __byte_perm(vc[e], vd[e], 0x7362);
                     uint4 o;
                     o.x = __byte_perm(t0, u0, 0x5410); o.y = __byte_perm(t0, u0, 0x7632);
                     o.z = __byte_perm(t1, u1, 0x5410); o.w = __byte_perm(t1, u1, 0x7632);
-                    dst[row * 16 + cg] = o;
-                    dst[row * 16 + 8 + cg] = o;                        // wrap copy (word 63 = word 31: never read)
+                    dst[region * 4096 + code * 16 + half * 8 + cg] = o;
                 }
             }
         }
-        if (tid == 0) {
-            sh->ndone = 0; sh->ndone_snap = 0; sh->full = 0;
-#pragma unroll
-            for (int i = 0; i < 4; i++) { sh->cnt[i] = 0; sh->qs[i] = (long long)qv[i]; sh->thr[i] = g4[i]; }
-        }
+        if (tid < DPH_QUAD_ITEM_Q) { sh->cnt[tid] = 0; sh->qs[tid] = (long long)dsc->q[tid]; sh->thr[tid] = gq; }
+        if (tid == 0) { sh->ndone = 0; sh->ndone_snap = 0; sh->full = 0; }
         __syncthreads();
+        QPH_MARK(0);
         if (warp == 0) {          // the next unit's record -> the other descriptor slot (waited for at the end of this item)
             const int nu = __shfl_sync(0xffffffffu, next_u, 0);
             if (lane == 0) sh->unit = nu;
@@ -675,70 +811,9 @@ __global__ void __launch_bounds__(NT, 1) scan_quad_kernel(PairScanArgs a) {
                 cp_async16(reinterpret_cast<unsigned char*>(&sh->desc[cur ^ 1]) + lane * 16, reinterpret_cast<const unsigned char*>(a.udesc + nu) + lane * 16);
             asm volatile("cp.async.commit_group;" ::: "memory");
         }
-        unsigned thr0 = sh->thr[0], thr1 = sh->thr[1], thr2 = sh->thr[2], thr3 = sh->thr[3];     // refreshed after every barrier
-        // float images of the thresholds (0xFFFFFFFF = "never passes" for the empty slots of a short group -> +inf)
-        auto thr_f = [](unsigned t) { return t == 0xFFFFFFFFu ? __int_as_float(0x7f800000) : (t == 0u ? -__int_as_float(0x7f800000) : dph_fkey_inv(t)); };
-        float tf0 = thr_f(thr0), tf1 = thr_f(thr1), tf2 = thr_f(thr2), tf3 = thr_f(thr3);
-
-        bool counted = false;
-        while (true) {
-            while (more) {
-                if (*((volatile int*)&sh->full)) break;
-                uint4 cur6[6];
-#pragma unroll
-                for (int c6 = 0; c6 < 6; c6++) cur6[c6] = nxt[c6];
-                const unsigned bcur = b;
-                if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16)); bp += NW; }
-                b += NW;
-                more = b < bend;
-                if (more) {
-                    const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
-#pragma unroll
-                    for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
-                }
-                unsigned sr[4] = {0u, 0u, 0u, 0u}, ab[4] = {0u, 0u, 0u, 0u};
-                quad_chunk<0, IMADL>(cur6[0], ywin, one, sr, ab);
-                quad_chunk<1, IMADL>(cur6[1], ywin, one, sr, ab);
-                quad_chunk<2, IMADL>(cur6[2], ywin, one, sr, ab);
-                quad_chunk<3, IMADL>(cur6[3], ywin, one, sr, ab);
-                quad_chunk<4, IMADL>(cur6[4], ywin, one, sr, ab);
-                quad_chunk<5, IMADL>(cur6[5], ywin, one, sr, ab);
-                const unsigned SR = (sr[0] + sr[1]) + (sr[2] + sr[3]);
-                const unsigned AB = (ab[0] + ab[1]) + (ab[2] + ab[3]);          // S1 | S3 << 16
-                const unsigned AE = SR - (AB << 8);                             // S0 | S2 << 16
-                const unsigned j = bcur * 32u + lane;
-                const bool valid = (int)j < len;
-                // thresholds are compared in the float domain (one FSETP per query); the order-preserving integer key is built only for
-                // the rare vector that passes.  (float)(unsigned short) converts a 16-bit half of the register without a mask / shift.
-                const float f0 = fmaf(stepv[0], (float)(unsigned short)(AE), basev[0]);
-                const float f1 = fmaf(stepv[1], (float)(unsigned short)(AB), basev[1]);
-                const float f2 = fmaf(stepv[2], (float)(unsigned short)(AE >> 16), basev[2]);
-                const float f3 = fmaf(stepv[3], (float)(unsigned short)(AB >> 16), basev[3]);
-                const bool p0 = valid && f0 >= tf0, p1 = valid && f1 >= tf1, p2 = valid && f2 >= tf2, p3 = valid && f3 >= tf3;
-                if (__any_sync(0xffffffffu, p0 || p1 || p2 || p3)) {
-                    const unsigned k0 = dph_fkey(f0), k1 = dph_fkey(f1), k2 = dph_fkey(f2), k3 = dph_fkey(f3);
-                    warp_append_latch(p0 && k0 >= thr0, ((unsigned long long)k0 << 32) | (unsigned long long)(0xFFFFFFFFu - (gsv[0] + j)), sh->cbuf[0], &sh->cnt[0], &sh->full, lane);
-                    warp_append_latch(p1 && k1 >= thr1, ((unsigned long long)k1 << 32) | (unsigned long long)(0xFFFFFFFFu - (gsv[1] + j)), sh->cbuf[1], &sh->cnt[1], &sh->full, lane);
-                    warp_append_latch(p2 && k2 >= thr2, ((unsigned long long)k2 << 32) | (unsigned long long)(0xFFFFFFFFu - (gsv[2] + j)), sh->cbuf[2], &sh->cnt[2], &sh->full, lane);
-                    warp_append_latch(p3 && k3 >= thr3, ((unsigned long long)k3 << 32) | (unsigned long long)(0xFFFFFFFFu - (gsv[3] + j)), sh->cbuf[3], &sh->cnt[3], &sh->full, lane);
-                }
-            }
-            if (!more && !counted) { counted = true; if (lane == 0) atomicAdd(&sh->ndone, 1); }
-            __syncthreads();
-#pragma unroll 1
-            for (int i = 0; i < nq; i++)
-                if (sh->cnt[i] > a.keep) compact_buffer<QCAP>(sh->cbuf[i], &sh->cnt[i], &sh->thr[i], a.keep, a.gthr + sh->qs[i], &sh->sc);
-            if (tid == 0) {
-                for (int i = 0; i < nq; i++) { unsigned g = *((volatile unsigned*)(a.gthr + sh->qs[i])); if (g > sh->thr[i]) sh->thr[i] = g; }
-                sh->ndone_snap = sh->ndone;
-                sh->full = 0;
-            }
-            __syncthreads();
-            thr0 = sh->thr[0]; thr1 = sh->thr[1]; thr2 = sh->thr[2]; thr3 = sh->thr[3];
-            tf0 = thr_f(thr0); tf1 = thr_f(thr1); tf2 = thr_f(thr2); tf3 = thr_f(thr3);
-            if (sh->ndone_snap == NW) break;
-        }
-        // ---- publish the candidate sets: the (up to) four region reservations go out together, one barrier ----
+        if (ntab == 2) quad_item_rounds<2, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, ph, ph_t);
+        else quad_item_rounds<1, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, ph, ph_t);
+        // ---- publish the candidate sets: the (up to) eight region reservations go out together, one barrier ----
         if (tid < nq) sh->base[tid] = atomicAdd(a.cand_cnt + sh->qs[tid], sh->cnt[tid]);
         if (warp == 0) asm volatile("cp.async.wait_all;" ::: "memory");
         __syncthreads();
@@ -748,17 +823,32 @@ __global__ void __launch_bounds__(NT, 1) scan_quad_kernel(PairScanArgs a) {
             const int cnt = sh->cnt[i];
             const long long off = a.cand_off[q], cap = a.cand_off[q + 1] - off;
             const int basep = sh->base[i];
-            for (int c = tid; c < cnt; c += NT)
+            for (int c = tid; c < cnt; c += QNT)
                 if (basep + c < cap) a.cand[off + basep + c] = sh->cbuf[i][c];
         }
-        const int un = sh->unit;
+        any_unit = sh->unit < total_units;
         __syncthreads();             // buffers, counters, sh->unit and the descriptor slots are reused by the next item
-        if (un >= total_units) break;
+        QPH_MARK(3);
         cur ^= 1;
     }
+#ifdef DPH_SCAN_PHASES
+    if (tid == 0) {
+        for (int i = 0; i < 4; i++) atomicAdd(&g_quad_phase_ns[i], ph[i]);
+        __threadfence();
+        if (atomicAdd(&g_quad_phase_ctas, 1u) == gridDim.x - 1) {
+            __threadfence();
+            unsigned long long v[4];
+            for (int i = 0; i < 4; i++) { v[i] = atomicExch(&g_quad_phase_ns[i], 0ull); }
+            printf("scan_quad_kernel phases (ms, summed over %u CTAs): table build %.3f, scan rounds %.3f, compaction barriers %.3f, publish %.3f\n",
+                   gridDim.x, v[0] * 1e-6, v[1] * 1e-6, v[2] * 1e-6, v[3] * 1e-6);
+            g_quad_phase_ctas = 0;
+        }
+    }
+#endif
 }
+#undef QPH_MARK
 
-__global__ void smem_base_probe_kernel(unsigned* out) { *out = (unsigned)__cvta_generic_to_shared(dph_smem) & 0x00FFFFFFu; }
+__global__ void smem_base_probe_kernel(unsigned* out) { *out = (unsigned)__cvta_generic_to_shared(dph_smem); }
 
 int dph_scan_setup_attrs() {
     static DphPerDeviceOnce once;
@@ -769,15 +859,16 @@ int dph_scan_setup_attrs() {
         smem_base_probe_kernel<<<1, 32, 1024>>>(d);
         DPH_CUDA(cudaMemcpy(&h, d, 4, cudaMemcpyDeviceToHost));
         cudaFree(d);
+        // the quad scan also needs the window's top address byte to be 0 (its gather addresses are built without it)
         DPH_CHECK(h == DPH_DYN_SMEM_BASE, "dynamic shared memory window does not start at 0x400 on this driver; rebuild with the probed value");
     }
     DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(ScanShared)));
     DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
     DPH_CUDA(cudaFuncSetAttribute(scan_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(QuadShared)));
+    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
     return 0;
 }
 
@@ -810,12 +901,12 @@ int dph_launch_scan_pair(dph_index* ix, int64_t n, int keep, int grid, cudaStrea
     a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.keep = keep;
     a.udesc = ix->pl_udesc.as<DphUnit>(); a.one = 1u;
     if (group == 4) {
-        const size_t sm = SMEM_LUT_FAST + sizeof(QuadShared);
+        const size_t sm = SMEM_QUAD_TABLES + sizeof(QuadShared);
         switch (g_dph_tune[0]) {
-            case 0: scan_quad_kernel<0><<<grid, NT, sm, st>>>(a); break;
-            case 2: scan_quad_kernel<2><<<grid, NT, sm, st>>>(a); break;
-            case 3: scan_quad_kernel<3><<<grid, NT, sm, st>>>(a); break;
-            default: scan_quad_kernel<1><<<grid, NT, sm, st>>>(a); break;
+            case 0: scan_quad_kernel<0><<<grid, QNT, sm, st>>>(a); break;
+            case 2: scan_quad_kernel<2><<<grid, QNT, sm, st>>>(a); break;
+            case 3: scan_quad_kernel<3><<<grid, QNT, sm, st>>>(a); break;
+            default: scan_quad_kernel<1><<<grid, QNT, sm, st>>>(a); break;
         }
     }
     else scan_pair_kernel<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
