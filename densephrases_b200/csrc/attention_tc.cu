@@ -346,25 +346,27 @@ __global__ void __launch_bounds__(256, 2) attention_tc_bx_kernel(const __grid_co
     }
 }
 
-// qkv[t]: [T, 2304] fp32 (Q | K | V, heads contiguous inside each), ctx[t]: [T, 768]; mask int64 [B, S]; S <= 64, 12 heads.
-int dph_launch_attention_tc(const float* const qkv[2], float* const ctx[2], const long long* mask, int B, int S, long long T, cudaStream_t st, int split,
-                            unsigned short* const* ctx_hi, unsigned short* const* ctx_lo) {
-    DPH_CHECK(S >= 1 && S <= 64 && B >= 1 && T >= (long long)B * S, "attention_tc: S must be 1..64");
+// towers (1 or 2) independent problems on the same mask; qkv[t]: [T, 2304] fp32 (Q | K | V, heads contiguous inside each),
+// ctx[t]: [T, 768]; mask int64 [B, S]; S <= 64, 12 heads.
+int dph_launch_attention_tc(int towers, const float* const* qkv, float* const* ctx, const long long* mask, int B, int S, long long T, cudaStream_t st,
+                            int split, unsigned short* const* ctx_hi, unsigned short* const* ctx_lo) {
+    DPH_CHECK(towers >= 1 && towers <= 2, "attention_tc: one or two towers");
+    DPH_CHECK(S >= 1 && S <= 64 && B >= 1 && B <= 65535 && T >= (long long)B * S && T <= INT32_MAX, "attention_tc: S must be 1..64");
     static DphPerDeviceOnce once;
     if (once.first()) {
         DPH_CUDA(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AT_SMEM_BYTES));
         DPH_CUDA(cudaFuncSetAttribute(attention_tc_bx_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ATB_SMEM_BYTES));
     }
-    AttnTcMaps maps;
-    AttnTcArgs a;
-    for (int t = 0; t < 2; t++) {
+    AttnTcMaps maps{};
+    AttnTcArgs a{};
+    for (int t = 0; t < towers; t++) {
         DPH_TRY(dph_make_map_f32(&maps.qkv[t], qkv[t], T, 3 * AT_H, 3 * AT_H, 64));
         a.qkv[t] = qkv[t]; a.ctx[t] = ctx[t];
         a.ctx_hi[t] = ctx_hi ? ctx_hi[t] : nullptr; a.ctx_lo[t] = ctx_lo ? ctx_lo[t] : nullptr;
     }
     a.mask = mask; a.S = S;
-    if (split) attention_tc_bx_kernel<<<dim3(6, (unsigned)B, 2), 256, ATB_SMEM_BYTES, st>>>(maps, a);
-    else attention_tc_kernel<<<dim3(6, (unsigned)B, 2), 256, AT_SMEM_BYTES, st>>>(maps, a);
+    if (split) attention_tc_bx_kernel<<<dim3(6, (unsigned)B, (unsigned)towers), 256, ATB_SMEM_BYTES, st>>>(maps, a);
+    else attention_tc_kernel<<<dim3(6, (unsigned)B, (unsigned)towers), 256, AT_SMEM_BYTES, st>>>(maps, a);
     DPH_CUDA(cudaGetLastError());
     return 0;
 }

@@ -1,7 +1,10 @@
-// encoder.cu -- query-side encoder forward: two independent BERT-base towers on the same tokens, hidden state at
-// position 0 of each (Encoder.forward(return_query=True) -> embed_query, reference densephrases/encoder.py:146-152,
-// 101-118; HF BertModel semantics restated in SURVEY.md Appendix B).  Both towers run as one grouped problem:
-// every GEMM is one launch of the wgmma GEMM (gemm_tf32.cu / gemm_bf16x3.cu) over the tiles of both towers.
+// encoder.cu -- the DensePhrases encoder forward (HF BertModel semantics restated in SURVEY.md Appendix B):
+//   query path:  two independent BERT-base towers on the same tokens, hidden state at position 0 of each
+//                (Encoder.forward(return_query=True) -> embed_query, reference densephrases/encoder.py:146-152, 101-118);
+//   phrase path: the phrase tower over every token, plus the filter head's two logits per token
+//                (Encoder.forward(input_ids=..., return_phrase=True) -> embed_phrase + filter_linear, encoder.py:92-99, 130-144).
+// One forward runs a set of towers as one grouped problem: every GEMM is one launch of the wgmma GEMM (gemm_tf32.cu /
+// gemm_bf16x3.cu) over the tiles of all its towers.
 #include "common.cuh"
 #include "../../include/dph_b200.h"
 #include <cuda_bf16.h>
@@ -11,7 +14,9 @@
 #define ENC_DH 64
 #define ENC_LAYERS 12
 #define ENC_FF 3072
-#define ENC_MAX_S 384          // Makefile:357-375 uses max_query_length 384 for KILT; attention keeps K,V of one head in smem
+#define ENC_MAX_S 384          // Makefile:357-375 uses max_query_length 384 for KILT; the SIMT attention keeps K,V of one head in smem
+#define ENC_MAX_S_PHRASE 512   // phrase path: max_seq_length 384 (options.py:33) / 512 (the dump recipe), BERT's position table
+#define ENC_TOWERS 3           // 0 query_start_encoder, 1 query_end_encoder, 2 phrase_encoder
 
 int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W, const float* const* bias, const float* const* residual,
                          float* const* out, int M, int N, int K, int act, cudaStream_t st, const float* const* A_lo, const float* const* W_lo);
@@ -20,8 +25,10 @@ int dph_launch_split_bf16(const float* x, void* hi, void* lo, long long n, cudaS
 int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const* A_lo, const void* const* W_hi, const void* const* W_lo,
                            const float* const* bias, const float* const* residual, float* const* out, void* const* out_hi, void* const* out_lo,
                            int M, int N, int K, int act, cudaStream_t st);
-int dph_launch_attention_tc(const float* const qkv[2], float* const ctx[2], const long long* mask, int B, int S, long long T, cudaStream_t st, int split,
-                            unsigned short* const* ctx_hi, unsigned short* const* ctx_lo);   // attention_tc.cu
+int dph_launch_attention_tc(int towers, const float* const* qkv, float* const* ctx, const long long* mask, int B, int S, long long T, cudaStream_t st,
+                            int split, unsigned short* const* ctx_hi, unsigned short* const* ctx_lo);                                // attention_tc.cu
+int dph_launch_attention_flash(const float* qkv, float* ctx, const long long* mask, int B, int S, long long T, cudaStream_t st, int split,
+                               unsigned short* ctx_hi, unsigned short* ctx_lo);                                                      // attention_flash.cu
 
 struct LayerW { const float *Wqkv, *bqkv, *Wo, *bo, *ln1g, *ln1b, *Wi, *bi, *Wo2, *bo2, *ln2g, *ln2b; };
 struct TowerW { const float *word, *pos, *type, *embg, *embb; LayerW L[ENC_LAYERS]; };
@@ -29,17 +36,20 @@ struct TowerW { const float *word, *pos, *type, *embg, *embb; LayerW L[ENC_LAYER
 struct dph_encoder {
     int device = 0; int vocab = 0, max_pos = 512, type_vocab = 2;
     cudaStream_t stream = 0;
-    float* blob[2] = {nullptr, nullptr};
-    TowerW tw[2];
+    float* blob[ENC_TOWERS] = {};
+    TowerW tw[ENC_TOWERS];
+    float* filt = nullptr;                       // filter_linear: weight [2, 768] | bias [2]
     // 3xTF32 mode: (hi, lo) copies of the four GEMM weight matrices of every layer, made lazily on the first precise forward
     int precise = 0;                             // 0: 1xTF32, 1: 3xTF32 split (fp32 planes), 2: bf16x3 split (bf16 planes, gemm_bf16x3.cu)
-    unsigned short* wbf[2] = {nullptr, nullptr}; // bf16x3 mode: per tower, per layer [Wqkv_hi, Wqkv_lo, Wo_hi, Wo_lo, Wi_hi, Wi_lo, Wo2_hi, Wo2_lo]
-    int attention_tc = 1;                        // S <= 64 and not precise: attention on the tensor cores (attention_tc.cu); 0: SIMT fp32 kernels below
-    float* wsplit[2] = {nullptr, nullptr};       // per tower: for each layer [Wqkv_hi, Wqkv_lo, Wo_hi, Wo_lo, Wi_hi, Wi_lo, Wo2_hi, Wo2_lo]
+    unsigned short* wbf[ENC_TOWERS] = {};        // bf16x3 mode: per tower, per layer [Wqkv_hi, Wqkv_lo, Wo_hi, Wo_lo, Wi_hi, Wi_lo, Wo2_hi, Wo2_lo]
+    int attention_tc = 1;                        // 1: attention on the tensor cores where a kernel exists (attention_tc.cu: S <= 64; attention_flash.cu:
+                                                 // S > 64 on the phrase path); 0: SIMT fp32 kernels below
+    float* wsplit[ENC_TOWERS] = {};              // per tower: for each layer [Wqkv_hi, Wqkv_lo, Wo_hi, Wo_lo, Wi_hi, Wi_lo, Wo2_hi, Wo2_lo]
+    // workspace for T tokens, per slot: slot t holds the t-th tower of the running forward (query path: two, phrase path: one)
+    int64_t cap_tokens[2] = {};
     float *act_hi[2] = {}, *act_lo[2] = {};      // split copy of the current GEMM input activation (up to T x 3072)
-    // workspace for T tokens
-    int64_t cap_tokens = 0;
     float *x[2] = {}, *qkv[2] = {}, *ctx[2] = {}, *a[2] = {}, *ffn[2] = {};
+    int64_t cap_in = 0;
     long long *ids = nullptr, *mask = nullptr, *tt = nullptr;
     float *out_s = nullptr, *out_e = nullptr;
     int64_t cap_b = 0;
@@ -135,9 +145,12 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(EmbedArgs a) {
     }
 }
 struct LnArgs { const float* in[2]; const float* g[2]; const float* b[2]; float* out[2]; long long rows; long long in_stride, out_stride;
-                unsigned short* out_hi[2]; unsigned short* out_lo[2]; };          // nullable: dense [rows, 768] bf16 planes of the output
+                unsigned short* out_hi[2]; unsigned short* out_lo[2];             // nullable: dense [rows, 768] bf16 planes of the output
+                const float* filt; float* filt_out; };                            // FILTER: filter_linear weight [2,768] | bias [2] -> [rows, 2]
 // One warp per row, 24 elements per lane as six float4: no shared memory, no block barrier; two-pass mean / variance like
 // torch.nn.LayerNorm.  in/out row strides allow normalising only the [CLS] rows of the last layer.
+// FILTER (last layer of the phrase path): the filter head, 768 -> 2 in fp32, on the normalised row while it is in registers.
+template <bool FILTER>
 __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int tw = blockIdx.y, lane = threadIdx.x & 31;
@@ -162,6 +175,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
     const float4* g = reinterpret_cast<const float4*>(a.g[tw]);
     const float4* b = reinterpret_cast<const float4*>(a.b[tw]);
     float4* o = reinterpret_cast<float4*>(a.out[tw] + row * a.out_stride);
+    float f0 = 0.f, f1 = 0.f;
 #pragma unroll
     for (int i = 0; i < 6; i++) {
         const float4 gg = g[lane + 32 * i], bb = b[lane + 32 * i];
@@ -173,6 +187,16 @@ __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
             reinterpret_cast<uint2*>(a.out_hi[tw] + row * ENC_H)[lane + 32 * i] = h4;
             reinterpret_cast<uint2*>(a.out_lo[tw] + row * ENC_H)[lane + 32 * i] = l4;
         }
+        if constexpr (FILTER) {
+            const float4 w0 = reinterpret_cast<const float4*>(a.filt)[lane + 32 * i], w1 = reinterpret_cast<const float4*>(a.filt + ENC_H)[lane + 32 * i];
+            f0 = fmaf(r4.x, w0.x, fmaf(r4.y, w0.y, fmaf(r4.z, w0.z, fmaf(r4.w, w0.w, f0))));
+            f1 = fmaf(r4.x, w1.x, fmaf(r4.y, w1.y, fmaf(r4.z, w1.z, fmaf(r4.w, w1.w, f1))));
+        }
+    }
+    if constexpr (FILTER) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) { f0 += __shfl_xor_sync(0xffffffffu, f0, off); f1 += __shfl_xor_sync(0xffffffffu, f1, off); }
+        if (lane == 0) *reinterpret_cast<float2*>(a.filt_out + row * 2) = make_float2(f0 + a.filt[2 * ENC_H], f1 + a.filt[2 * ENC_H + 1]);
     }
 }
 // gather rows b*S of [B*S, 768] into a dense [B, 768] buffer (the [CLS] rows the last layer's output actually needs)
@@ -343,27 +367,28 @@ __global__ void __launch_bounds__(256) attention_tile_kernel(AttnArgs a) {
         if (r < S) *reinterpret_cast<float4*>(a.ctx[tw] + ((long long)b * S + r) * ENC_H + h * ENC_DH + tx * 4) = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
     }
 }
-template <int KT> static int launch_attention_tile(const AttnArgs& aa, int B, cudaStream_t st) {
+template <int KT> static int launch_attention_tile(const AttnArgs& aa, int towers, int B, cudaStream_t st) {
     constexpr int SP = 16 * KT;
     const size_t smem = (size_t)(64 * 68 + 64 * (SP + 4) + SP * 64 + SP * 68 + SP) * 4;
     static DphPerDeviceOnce once;
     if (once.first()) { DPH_CUDA(cudaFuncSetAttribute(attention_tile_kernel<KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); }
-    attention_tile_kernel<KT><<<dim3(ENC_HEADS * ((aa.S + 63) / 64), (unsigned)B, 2), 256, smem, st>>>(aa);
+    attention_tile_kernel<KT><<<dim3(ENC_HEADS * ((aa.S + 63) / 64), (unsigned)B, (unsigned)towers), 256, smem, st>>>(aa);
     DPH_CUDA(cudaGetLastError());
     return 0;
 }
-static int launch_attention(const AttnArgs& aa, int B, cudaStream_t st) {
+// SIMT attention of `towers` (1 or 2) towers: aa.qkv[t] / aa.ctx[t] for t < towers
+static int launch_attention(const AttnArgs& aa, int towers, int B, cudaStream_t st) {
     const int S = aa.S;
-    if (S <= 16) return launch_attention_tile<1>(aa, B, st);
-    if (S <= 32) return launch_attention_tile<2>(aa, B, st);
-    if (S <= 64) return launch_attention_tile<4>(aa, B, st);
-    if (S <= 96) return launch_attention_tile<6>(aa, B, st);
-    if (S <= 128) return launch_attention_tile<8>(aa, B, st);
+    if (S <= 16) return launch_attention_tile<1>(aa, towers, B, st);
+    if (S <= 32) return launch_attention_tile<2>(aa, towers, B, st);
+    if (S <= 64) return launch_attention_tile<4>(aa, towers, B, st);
+    if (S <= 96) return launch_attention_tile<6>(aa, towers, B, st);
+    if (S <= 128) return launch_attention_tile<8>(aa, towers, B, st);
     const int attn_warps = 8;      // long sequences (max_query_length 384 for KILT entity linking): K,V of the head in shared memory
     const size_t attn_smem = ((size_t)S * 65 + (size_t)S * 64 + S + attn_warps * 64 + (size_t)attn_warps * S) * 4;
     static DphPerDeviceOnce once;
     if (once.first()) { DPH_CUDA(cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); }
-    attention_kernel<<<dim3(ENC_HEADS, (unsigned)B, 2), attn_warps * 32, attn_smem, st>>>(aa);
+    attention_kernel<<<dim3(ENC_HEADS, (unsigned)B, (unsigned)towers), attn_warps * 32, attn_smem, st>>>(aa);
     DPH_CUDA(cudaGetLastError());
     return 0;
 }
@@ -383,12 +408,15 @@ DPH_API int dph_encoder_create(dph_encoder** out, int device, int vocab_size, in
 DPH_API void dph_encoder_free(dph_encoder* e) {
     if (!e) return;
     cudaSetDevice(e->device);
+    for (int t = 0; t < ENC_TOWERS; t++) {
+        float* w[] = {e->blob[t], e->wsplit[t], (float*)e->wbf[t]};
+        for (float* p : w) if (p) cudaFree(p);
+    }
     for (int t = 0; t < 2; t++) {
-        if (e->blob[t]) cudaFree(e->blob[t]);
-        float* ws[] = {e->x[t], e->qkv[t], e->ctx[t], e->a[t], e->ffn[t], e->wsplit[t], e->act_hi[t], e->act_lo[t], (float*)e->wbf[t]};
+        float* ws[] = {e->x[t], e->qkv[t], e->ctx[t], e->a[t], e->ffn[t], e->act_hi[t], e->act_lo[t]};
         for (float* p : ws) if (p) cudaFree(p);
     }
-    void* misc[] = {e->ids, e->mask, e->tt, e->out_s, e->out_e, e->bad_ids};
+    void* misc[] = {e->ids, e->mask, e->tt, e->out_s, e->out_e, e->bad_ids, e->filt};
     for (void* p : misc) if (p) cudaFree(p);
     delete e;
 }
@@ -402,29 +430,29 @@ DPH_API int dph_encoder_set_attention(dph_encoder* e, int tensor_core) { e->atte
 
 // C ABI (test / standalone use): one BERT self-attention over a [B*S, 2304] QKV activation (device pointers) -> ctx [B*S, 768].
 DPH_API int dph_attention_bert(const float* qkv, const int64_t* mask, int B, int S, float* ctx, int tensor_core, void* cuda_stream) {
-    DPH_CHECK(qkv && mask && ctx && B >= 1 && S >= 1 && S <= ENC_MAX_S, "attention: bad arguments");
-    DPH_CHECK(!tensor_core || S <= 64, "tensor-core attention handles S <= 64");
+    DPH_CHECK(qkv && mask && ctx && B >= 1 && B <= 65535 && S >= 1, "attention: bad arguments");
     DPH_CHECK(tensor_core >= 0 && tensor_core <= 2, "tensor_core: 0 SIMT fp32, 1 wgmma TF32, 2 wgmma bf16x3 planes (fp32-accurate)");
+    DPH_CHECK(tensor_core ? S <= ENC_MAX_S_PHRASE : S <= ENC_MAX_S, "attention: S <= 512 on the tensor cores, S <= 384 on the SIMT kernels");
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    float* scratch = nullptr;                            // the launchers run two towers: the second one repeats the first into scratch
-    DPH_CUDA(cudaMalloc((void**)&scratch, (size_t)B * S * ENC_H * 4));
+    const long long T = (long long)B * S;
     int rc;
-    if (tensor_core) {
-        const float* q2[2] = {qkv, qkv}; float* c2[2] = {ctx, scratch};
-        rc = dph_launch_attention_tc(q2, c2, (const long long*)mask, B, S, (long long)B * S, st, tensor_core == 2, nullptr, nullptr);
+    if (tensor_core && S <= 64) {
+        rc = dph_launch_attention_tc(1, &qkv, &ctx, (const long long*)mask, B, S, T, st, tensor_core == 2, nullptr, nullptr);
+    } else if (tensor_core) {
+        rc = dph_launch_attention_flash(qkv, ctx, (const long long*)mask, B, S, T, st, tensor_core == 2, nullptr, nullptr);
     } else {
-        AttnArgs aa; aa.qkv[0] = qkv; aa.qkv[1] = qkv; aa.ctx[0] = ctx; aa.ctx[1] = scratch; aa.mask = (const long long*)mask; aa.S = S;
-        rc = launch_attention(aa, B, st);
+        AttnArgs aa{}; aa.qkv[0] = qkv; aa.ctx[0] = ctx; aa.mask = (const long long*)mask; aa.S = S;
+        rc = launch_attention(aa, 1, B, st);
     }
-    cudaStreamSynchronize(st);
-    cudaFree(scratch);
+    if (!rc) DPH_CUDA(cudaStreamSynchronize(st));
     return rc;
 }
 
 static const int64_t kGemmW[4] = {(int64_t)3 * ENC_H * ENC_H, (int64_t)ENC_H * ENC_H, (int64_t)ENC_FF * ENC_H, (int64_t)ENC_H * ENC_FF};
 static int64_t split_layer_floats() { return 2 * (kGemmW[0] + kGemmW[1] + kGemmW[2] + kGemmW[3]); }
-static int ensure_split_weights(dph_encoder* e) {
-    for (int t = 0; t < 2; t++) {
+static int ensure_split_weights(dph_encoder* e, const int* tws, int nt) {
+    for (int i = 0; i < nt; i++) {
+        const int t = tws[i];
         if (e->wsplit[t]) continue;
         DPH_CUDA(cudaMalloc((void**)&e->wsplit[t], (size_t)split_layer_floats() * ENC_LAYERS * 4));
         for (int l = 0; l < ENC_LAYERS; l++) {
@@ -436,8 +464,9 @@ static int ensure_split_weights(dph_encoder* e) {
     }
     return 0;
 }
-static int ensure_bf16_weights(dph_encoder* e) {
-    for (int t = 0; t < 2; t++) {
+static int ensure_bf16_weights(dph_encoder* e, const int* tws, int nt) {
+    for (int i = 0; i < nt; i++) {
+        const int t = tws[i];
         if (e->wbf[t]) continue;
         DPH_CUDA(cudaMalloc((void**)&e->wbf[t], (size_t)split_layer_floats() * ENC_LAYERS * 2));
         for (int l = 0; l < ENC_LAYERS; l++) {
@@ -465,7 +494,7 @@ DPH_API int64_t dph_encoder_tower_floats(const dph_encoder* e) { return tower_fl
 //   per layer: [Wq;Wk;Wv] [2304,768] | [bq;bk;bv] | attention.output.dense W [768,768], b | attention.output.LayerNorm w, b |
 //              intermediate.dense W [3072,768], b | output.dense W [768,3072], b | output.LayerNorm w, b
 DPH_API int dph_encoder_load_tower(dph_encoder* e, int tower, const float* blob, int mem) {
-    DPH_CHECK(tower == 0 || tower == 1, "tower must be 0 (query_start_encoder) or 1 (query_end_encoder)");
+    DPH_CHECK(tower >= 0 && tower < ENC_TOWERS, "tower must be 0 (query_start_encoder), 1 (query_end_encoder) or 2 (phrase_encoder)");
     DPH_CUDA(cudaSetDevice(e->device));
     const size_t bytes = (size_t)tower_floats(e) * 4;
     if (!e->blob[tower]) DPH_CUDA(cudaMalloc((void**)&e->blob[tower], bytes));
@@ -475,30 +504,220 @@ DPH_API int dph_encoder_load_tower(dph_encoder* e, int tower, const float* blob,
     if (e->wbf[tower]) { cudaFree(e->wbf[tower]); e->wbf[tower] = nullptr; }
     return 0;
 }
+DPH_API int dph_encoder_load_filter(dph_encoder* e, const float* W, const float* b, int mem) {
+    DPH_CHECK(e && W && b, "filter_linear: weight [2,768] and bias [2] required");
+    DPH_CUDA(cudaSetDevice(e->device));
+    if (!e->filt) DPH_CUDA(cudaMalloc((void**)&e->filt, (2 * ENC_H + 2) * 4));
+    const cudaMemcpyKind kind = mem == DPH_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    DPH_CUDA(cudaMemcpy(e->filt, W, 2 * ENC_H * 4, kind));
+    DPH_CUDA(cudaMemcpy(e->filt + 2 * ENC_H, b, 2 * 4, kind));
+    return 0;
+}
 // free + null + allocate, so that a failed allocation never leaves a dangling pointer behind for dph_encoder_free
 static int regrow(void** p, size_t bytes) {
     if (*p) { cudaFree(*p); *p = nullptr; }
     DPH_CUDA(cudaMalloc(p, bytes));
     return 0;
 }
-static int ensure_ws(dph_encoder* e, int64_t T, int64_t B) {
-    if (T > e->cap_tokens) {
-        e->cap_tokens = 0;                                   // stays 0 if anything below fails: the next call starts over
-        for (int t = 0; t < 2; t++) {
-            float** ps[] = {&e->x[t], &e->qkv[t], &e->ctx[t], &e->a[t], &e->ffn[t], &e->act_hi[t], &e->act_lo[t]};
-            size_t sz[] = {(size_t)T * ENC_H, (size_t)T * 3 * ENC_H, (size_t)T * ENC_H, (size_t)T * ENC_H, (size_t)T * ENC_FF, (size_t)T * ENC_FF,
-                           (size_t)T * ENC_FF};
-            for (int i = 0; i < 7; i++) DPH_TRY(regrow((void**)ps[i], sz[i] * 4));
-        }
+// workspace of `slots` tower slots for T tokens, input staging for T tokens, [CLS] outputs for B rows
+static int ensure_ws(dph_encoder* e, int64_t T, int64_t B, int slots) {
+    for (int t = 0; t < slots; t++) {
+        if (T <= e->cap_tokens[t]) continue;
+        e->cap_tokens[t] = 0;                                // stays 0 if anything below fails: the next call starts over
+        float** ps[] = {&e->x[t], &e->qkv[t], &e->ctx[t], &e->a[t], &e->ffn[t], &e->act_hi[t], &e->act_lo[t]};
+        size_t sz[] = {(size_t)T * ENC_H, (size_t)T * 3 * ENC_H, (size_t)T * ENC_H, (size_t)T * ENC_H, (size_t)T * ENC_FF, (size_t)T * ENC_FF,
+                       (size_t)T * ENC_FF};
+        for (int i = 0; i < 7; i++) DPH_TRY(regrow((void**)ps[i], sz[i] * 4));
+        e->cap_tokens[t] = T;
+    }
+    if (T > e->cap_in) {
+        e->cap_in = 0;
         long long** ip[] = {&e->ids, &e->mask, &e->tt};
         for (auto p : ip) DPH_TRY(regrow((void**)p, (size_t)T * 8));
-        e->cap_tokens = T;
+        e->cap_in = T;
     }
     if (B > e->cap_b) {
         e->cap_b = 0;
         DPH_TRY(regrow((void**)&e->out_s, (size_t)B * ENC_H * 4));
         DPH_TRY(regrow((void**)&e->out_e, (size_t)B * ENC_H * 4));
         e->cap_b = B;
+    }
+    return 0;
+}
+
+// Common start of a forward: report the id flag of earlier asynchronous calls, size the workspace, stage host inputs.
+static int begin_forward(dph_encoder* e, const int64_t* ids, const int64_t* mask, const int64_t* tt, int64_t T, int64_t B, int slots, int mem,
+                         const long long** d_ids, const long long** d_mask, const long long** d_tt) {
+    cudaStream_t st = e->stream;
+    DPH_TRY(ensure_ws(e, T, B, slots));
+    if (!e->bad_ids) { DPH_CUDA(cudaMalloc((void**)&e->bad_ids, 4)); DPH_CUDA(cudaMemset(e->bad_ids, 0, 4)); }
+    if (e->bad_pending) {       // flag of the previous asynchronous forward(s): report it now instead of never
+        int h = 0;
+        DPH_CUDA(cudaMemcpyAsync(&h, e->bad_ids, 4, cudaMemcpyDeviceToHost, st));
+        DPH_CUDA(cudaStreamSynchronize(st));
+        e->bad_pending = false;
+        if (h) { DPH_CUDA(cudaMemsetAsync(e->bad_ids, 0, 4, st)); dph_set_error("encoder: an earlier forward received input_ids / token_type_ids outside the embedding tables"); return 1; }
+    }
+    *d_ids = (const long long*)ids; *d_mask = (const long long*)mask; *d_tt = (const long long*)tt;
+    if (mem == DPH_MEM_HOST) {
+        DPH_CUDA(cudaMemcpyAsync(e->ids, ids, T * 8, cudaMemcpyHostToDevice, st));
+        DPH_CUDA(cudaMemcpyAsync(e->mask, mask, T * 8, cudaMemcpyHostToDevice, st));
+        DPH_CUDA(cudaMemcpyAsync(e->tt, tt, T * 8, cudaMemcpyHostToDevice, st));
+        *d_ids = e->ids; *d_mask = e->mask; *d_tt = e->tt;
+    }
+    return 0;
+}
+// Common end: host buffers wait for the forward (and its output copies, queued before) and check the id flag now; device buffers
+// leave the flag to the next call.
+static int end_forward(dph_encoder* e, int mem) {
+    cudaStream_t st = e->stream;
+    if (mem == DPH_MEM_HOST) {
+        int h = 0;
+        DPH_CUDA(cudaMemcpyAsync(&h, e->bad_ids, 4, cudaMemcpyDeviceToHost, st));
+        DPH_CUDA(cudaStreamSynchronize(st));
+        if (h) { DPH_CUDA(cudaMemsetAsync(e->bad_ids, 0, 4, st)); dph_set_error("encoder: input_ids / token_type_ids outside the embedding tables (IndexError in torch)"); return 1; }
+    } else {
+        e->bad_pending = true;
+    }
+    return 0;
+}
+
+// The 12-layer forward of nt towers (tws[t] runs in workspace slot t) over the B x S tokens at d_ids / d_mask / d_tt.
+//   query path  (phrase = false, nt = 2): the last layer runs on the [CLS] rows only after its attention; its result is left in
+//     ctx[t] ([B,768]; x[t] when S == 1).  Attention: tensor cores for S <= 64, SIMT above.
+//   phrase path (phrase = true, nt = 1): every layer on every token; the last LayerNorm writes final_out [T,768] and, with
+//     filter_out, the filter head's logits [T,2].  Attention: tensor cores at every S (attention_flash.cu above 64).
+static int encoder_forward(dph_encoder* e, const int* tws, int nt, const long long* d_ids, const long long* d_mask, const long long* d_tt, int B, int S,
+                           bool phrase, float* final_out, float* filter_out) {
+    cudaStream_t st = e->stream;
+    const int64_t T = (int64_t)B * S;
+    // bf16x3 mode: (hi, lo) planes of the three T x 768 GEMM inputs (x, ctx, a) live in act_hi / act_lo; their producers (LayerNorm,
+    // attention) write them, so no separate split pass runs.  The T x 3072 FFN intermediate's planes live in ffn[] (see `linear`).
+    unsigned short *xh[2] = {}, *xl[2] = {}, *ch[2] = {}, *cl[2] = {}, *ah[2] = {}, *al[2] = {};
+    for (int t = 0; t < nt; t++) {
+        xh[t] = reinterpret_cast<unsigned short*>(e->act_hi[t]); xl[t] = reinterpret_cast<unsigned short*>(e->act_lo[t]);
+        ch[t] = xh[t] + T * ENC_H; cl[t] = xl[t] + T * ENC_H;
+        ah[t] = ch[t] + T * ENC_H; al[t] = cl[t] + T * ENC_H;
+    }
+    {
+        EmbedArgs a{};
+        a.ids = d_ids; a.tt = d_tt; a.S = S;
+        for (int t = 0; t < nt; t++) {
+            const TowerW& w = e->tw[tws[t]];
+            a.word[t] = w.word; a.pos[t] = w.pos; a.type[t] = w.type; a.g[t] = w.embg; a.b[t] = w.embb; a.out[t] = e->x[t];
+        }
+        a.vocab = e->vocab; a.type_vocab = e->type_vocab; a.bad = e->bad_ids;
+        for (int t = 0; t < nt; t++) { a.out_hi[t] = e->precise == 2 ? xh[t] : nullptr; a.out_lo[t] = e->precise == 2 ? xl[t] : nullptr; }
+        embed_ln_kernel<<<dim3((unsigned)T, (unsigned)nt), 256, 0, st>>>(a);
+        DPH_CUDA(cudaGetLastError());
+    }
+    if (e->precise == 1) DPH_TRY(ensure_split_weights(e, tws, nt));
+    if (e->precise == 2) DPH_TRY(ensure_bf16_weights(e, tws, nt));
+    // one grouped linear layer over the towers: out = act(in . W^T + b) + residual; m = which weight of the layer (0 qkv, 1 attn out, 2 ffn in, 3 ffn out)
+    unsigned short* const PH[3][2] = {{xh[0], xh[1]}, {ch[0], ch[1]}, {ah[0], ah[1]}};
+    unsigned short* const PL[3][2] = {{xl[0], xl[1]}, {cl[0], cl[1]}, {al[0], al[1]}};
+    // planes_ready (bf16x3 mode): the producer of `in` already wrote its (hi, lo) planes into PH[m] / PL[m]
+    auto linear = [&](int l, int m, float* const in[2], const float* const bias[2], float* const resid[2], float* const out[2], int N, int K, int act,
+                      long long rows, bool planes_ready) -> int {
+        const float* Wfull[2] = {};
+        for (int t = 0; t < nt; t++) {
+            const LayerW& Lt = e->tw[tws[t]].L[l];
+            Wfull[t] = m == 0 ? Lt.Wqkv : m == 1 ? Lt.Wo : m == 2 ? Lt.Wi : Lt.Wo2;
+        }
+        const float* R[2] = {resid ? resid[0] : nullptr, resid ? resid[1] : nullptr};
+        if (!e->precise) {
+            const float* A[2] = {in[0], in[1]};
+            return dph_launch_gemm_tf32(nt, A, Wfull, bias, resid ? R : nullptr, out, (int)rows, N, K, act, st, nullptr, nullptr);
+        }
+        if (e->precise == 2) {
+            // bf16x3: operands as (hi, lo) bf16 planes.  The FFN intermediate never exists in fp32: the GELU epilogue of GEMM m = 2
+            // writes its planes (into the memory of `out`), GEMM m = 3 reads them; the other inputs' planes come from their producers
+            // (LayerNorm / embedding / tensor-core attention) or, failing that, from one split pass.
+            const void *Whi[2] = {}, *Wlo[2] = {}, *Ahi[2] = {}, *Alo[2] = {};
+            void *Ohi[2] = {nullptr, nullptr}, *Olo[2] = {nullptr, nullptr};
+            for (int t = 0; t < nt; t++) {
+                bf16_ptrs(e, tws[t], l, m, &Whi[t], &Wlo[t]);
+                if (m == 3) {                                                     // planes left by GEMM m = 2 in `in`
+                    Ahi[t] = in[t]; Alo[t] = reinterpret_cast<const unsigned short*>(in[t]) + rows * (long long)K;
+                } else {
+                    if (!planes_ready) DPH_TRY(dph_launch_split_bf16(in[t], PH[m][t], PL[m][t], rows * K, st));
+                    Ahi[t] = PH[m][t]; Alo[t] = PL[m][t];
+                }
+                if (m == 2) { Ohi[t] = out[t]; Olo[t] = reinterpret_cast<unsigned short*>(out[t]) + rows * (long long)N; }
+            }
+            return dph_launch_gemm_bf16x3(nt, Ahi, Alo, Whi, Wlo, bias, resid ? R : nullptr, m == 2 ? nullptr : out, m == 2 ? Ohi : nullptr,
+                                          m == 2 ? Olo : nullptr, (int)rows, N, K, act, st);
+        }
+        const float *Whi[2] = {}, *Wlo[2] = {};
+        for (int t = 0; t < nt; t++) {
+            split_ptrs(e, tws[t], l, m, &Whi[t], &Wlo[t]);
+            DPH_TRY(dph_launch_split_tf32(in[t], e->act_hi[t], e->act_lo[t], rows * K, st));
+        }
+        const float* Ahi[2] = {e->act_hi[0], e->act_hi[1]}; const float* Alo[2] = {e->act_lo[0], e->act_lo[1]};
+        return dph_launch_gemm_tf32(nt, Ahi, Whi, bias, resid ? R : nullptr, out, (int)rows, N, K, act, st, Alo, Wlo);
+    };
+    for (int l = 0; l < ENC_LAYERS; l++) {
+        const LayerW* Lt[2] = {&e->tw[tws[0]].L[l], &e->tw[tws[nt - 1]].L[l]};
+        float* X[2] = {e->x[0], e->x[1]};
+        float* QKV[2] = {e->qkv[0], e->qkv[1]};
+        float* CTX[2] = {e->ctx[0], e->ctx[1]};
+        float* A2[2] = {e->a[0], e->a[1]};
+        float* FF[2] = {e->ffn[0], e->ffn[1]};
+        const float* bqkv[2] = {Lt[0]->bqkv, Lt[1]->bqkv}; const float* bo[2] = {Lt[0]->bo, Lt[1]->bo};
+        const float* bi[2] = {Lt[0]->bi, Lt[1]->bi}; const float* bo2[2] = {Lt[0]->bo2, Lt[1]->bo2};
+        const bool bx = e->precise == 2;
+        DPH_TRY(linear(l, 0, X, bqkv, nullptr, QKV, 3 * ENC_H, ENC_H, 0, T, bx));          // x planes: embedding LayerNorm / previous layer's LayerNorm
+        AttnArgs aa; aa.qkv[0] = e->qkv[0]; aa.qkv[1] = e->qkv[1]; aa.ctx[0] = e->ctx[0]; aa.ctx[1] = e->ctx[1]; aa.mask = d_mask; aa.S = S;
+        bool ctx_planes = false;
+        if (e->attention_tc && S <= 64) {      // tensor cores: TF32 in the 1xTF32 mode, the bf16 (hi, lo) plane kernel (fp32-accurate) in the precise modes
+            const float* q2[2] = {e->qkv[0], e->qkv[1]}; float* c2[2] = {e->ctx[0], e->ctx[1]};
+            DPH_TRY(dph_launch_attention_tc(nt, q2, c2, d_mask, B, S, T, st, e->precise ? 1 : 0, bx ? ch : nullptr, bx ? cl : nullptr));
+            ctx_planes = bx;
+        } else if (e->attention_tc && phrase) {   // context lengths: key blocks streamed with an online softmax
+            DPH_TRY(dph_launch_attention_flash(e->qkv[0], e->ctx[0], d_mask, B, S, T, st, e->precise ? 1 : 0, bx ? ch[0] : nullptr, bx ? cl[0] : nullptr));
+            ctx_planes = bx;
+        } else {
+            DPH_TRY(launch_attention(aa, nt, B, st));
+        }
+        // Query path: only position 0 of the LAST layer is returned (encoder.py:116-117): after its attention, everything (attention
+        // output projection, both LayerNorms, the FFN) runs on the B [CLS] rows instead of all B*S tokens.
+        const bool last = !phrase && (l == ENC_LAYERS - 1) && S >= 2;      // (S == 1: the scratch aliasing below needs T >= 2B rows)
+        long long rows = T;
+        if (last) {
+            rows = B;
+            const unsigned gb = (unsigned)((B * (ENC_H / 4) + 255) / 256);
+            gather_cls_kernel<<<dim3(gb, 2), 256, 0, st>>>(e->ctx[0], e->ctx[1], e->ffn[0], e->ffn[1], S, B);                         // ctx rows  -> ffn[:B]  (scratch)
+            gather_cls_kernel<<<dim3(gb, 2), 256, 0, st>>>(e->x[0], e->x[1], e->ffn[0] + (size_t)B * ENC_H, e->ffn[1] + (size_t)B * ENC_H, S, B);   // residual rows
+            DPH_CUDA(cudaGetLastError());
+            CTX[0] = e->ffn[0]; CTX[1] = e->ffn[1];
+            X[0] = e->ffn[0] + (size_t)B * ENC_H; X[1] = e->ffn[1] + (size_t)B * ENC_H;
+            FF[0] = e->qkv[0]; FF[1] = e->qkv[1];                                                                                     // qkv is dead after attention: [B, 3072] fits
+        }
+        DPH_TRY(linear(l, 1, CTX, bo, X, A2, ENC_H, ENC_H, 0, rows, ctx_planes && !last));           // dense + residual (last layer: gathered rows, split here)
+        LnArgs ln1{}; for (int t = 0; t < nt; t++) { ln1.in[t] = e->a[t]; ln1.out[t] = e->a[t]; ln1.out_hi[t] = bx ? ah[t] : nullptr; ln1.out_lo[t] = bx ? al[t] : nullptr; }
+        ln1.g[0] = Lt[0]->ln1g; ln1.g[1] = Lt[1]->ln1g; ln1.b[0] = Lt[0]->ln1b; ln1.b[1] = Lt[1]->ln1b;
+        ln1.rows = rows; ln1.in_stride = ENC_H; ln1.out_stride = ENC_H;
+        layernorm_kernel<false><<<dim3((unsigned)((rows + 7) / 8), (unsigned)nt), 256, 0, st>>>(ln1);
+        DPH_CUDA(cudaGetLastError());
+        DPH_TRY(linear(l, 2, A2, bi, nullptr, FF, ENC_FF, ENC_H, 1, rows, bx));                          // intermediate + erf-GELU
+        float* XO[2] = {last ? e->ctx[0] : e->x[0], last ? e->ctx[1] : e->x[1]};                         // last layer: dense [B,768] result in ctx
+        DPH_TRY(linear(l, 3, FF, bo2, A2, XO, ENC_H, ENC_FF, 0, rows, bx));                              // output dense + residual
+        const bool final_ln = phrase && l == ENC_LAYERS - 1;                                               // phrase path: -> final_out (+ filter head)
+        LnArgs ln2{};
+        for (int t = 0; t < nt; t++) {
+            ln2.in[t] = XO[t]; ln2.out[t] = final_ln ? final_out : XO[t];
+            ln2.out_hi[t] = (bx && !last && !final_ln) ? xh[t] : nullptr; ln2.out_lo[t] = (bx && !last && !final_ln) ? xl[t] : nullptr;
+        }
+        ln2.g[0] = Lt[0]->ln2g; ln2.g[1] = Lt[1]->ln2g; ln2.b[0] = Lt[0]->ln2b; ln2.b[1] = Lt[1]->ln2b;
+        ln2.rows = rows; ln2.in_stride = ENC_H; ln2.out_stride = ENC_H;
+        const dim3 lgrid((unsigned)((rows + 7) / 8), (unsigned)nt);
+        if (final_ln && filter_out) {
+            ln2.filt = e->filt; ln2.filt_out = filter_out;
+            layernorm_kernel<true><<<lgrid, 256, 0, st>>>(ln2);
+        } else {
+            layernorm_kernel<false><<<lgrid, 256, 0, st>>>(ln2);
+        }
+        DPH_CUDA(cudaGetLastError());
     }
     return 0;
 }
@@ -512,131 +731,10 @@ DPH_API int dph_encoder_embed_query(dph_encoder* e, const int64_t* ids, const in
     DPH_CUDA(cudaSetDevice(e->device));
     cudaStream_t st = e->stream;
     const int64_t T = (int64_t)B * S;
-    DPH_TRY(ensure_ws(e, T, B));
-    if (!e->bad_ids) { DPH_CUDA(cudaMalloc((void**)&e->bad_ids, 4)); DPH_CUDA(cudaMemset(e->bad_ids, 0, 4)); }
-    if (e->bad_pending) {       // flag of the previous asynchronous forward(s): report it now instead of never
-        int h = 0;
-        DPH_CUDA(cudaMemcpyAsync(&h, e->bad_ids, 4, cudaMemcpyDeviceToHost, st));
-        DPH_CUDA(cudaStreamSynchronize(st));
-        e->bad_pending = false;
-        if (h) { DPH_CUDA(cudaMemsetAsync(e->bad_ids, 0, 4, st)); dph_set_error("encoder: an earlier forward received input_ids / token_type_ids outside the embedding tables"); return 1; }
-    }
-    const long long *d_ids = (const long long*)ids, *d_mask = (const long long*)mask, *d_tt = (const long long*)tt;
-    if (mem == DPH_MEM_HOST) {
-        DPH_CUDA(cudaMemcpyAsync(e->ids, ids, T * 8, cudaMemcpyHostToDevice, st));
-        DPH_CUDA(cudaMemcpyAsync(e->mask, mask, T * 8, cudaMemcpyHostToDevice, st));
-        DPH_CUDA(cudaMemcpyAsync(e->tt, tt, T * 8, cudaMemcpyHostToDevice, st));
-        d_ids = e->ids; d_mask = e->mask; d_tt = e->tt;
-    }
-    // bf16x3 mode: (hi, lo) planes of the three T x 768 GEMM inputs (x, ctx, a) live in act_hi / act_lo; their producers (LayerNorm,
-    // attention) write them, so no separate split pass runs.  The T x 3072 FFN intermediate's planes live in ffn[] (see `linear`).
-    unsigned short *xh[2], *xl[2], *ch[2], *cl[2], *ah[2], *al[2];
-    for (int t = 0; t < 2; t++) {
-        xh[t] = reinterpret_cast<unsigned short*>(e->act_hi[t]); xl[t] = reinterpret_cast<unsigned short*>(e->act_lo[t]);
-        ch[t] = xh[t] + T * ENC_H; cl[t] = xl[t] + T * ENC_H;
-        ah[t] = ch[t] + T * ENC_H; al[t] = cl[t] + T * ENC_H;
-    }
-    {
-        EmbedArgs a;
-        a.ids = d_ids; a.tt = d_tt; a.S = S;
-        for (int t = 0; t < 2; t++) { a.word[t] = e->tw[t].word; a.pos[t] = e->tw[t].pos; a.type[t] = e->tw[t].type; a.g[t] = e->tw[t].embg; a.b[t] = e->tw[t].embb; a.out[t] = e->x[t]; }
-        a.vocab = e->vocab; a.type_vocab = e->type_vocab; a.bad = e->bad_ids;
-        for (int t = 0; t < 2; t++) { a.out_hi[t] = e->precise == 2 ? xh[t] : nullptr; a.out_lo[t] = e->precise == 2 ? xl[t] : nullptr; }
-        embed_ln_kernel<<<dim3((unsigned)T, 2), 256, 0, st>>>(a);
-        DPH_CUDA(cudaGetLastError());
-    }
-    if (e->precise == 1) DPH_TRY(ensure_split_weights(e));
-    if (e->precise == 2) DPH_TRY(ensure_bf16_weights(e));
-    // one grouped (two-tower) linear layer: out = act(in . W^T + b) + residual; m = which weight of the layer (0 qkv, 1 attn out, 2 ffn in, 3 ffn out)
-    unsigned short* const PH[3][2] = {{xh[0], xh[1]}, {ch[0], ch[1]}, {ah[0], ah[1]}};
-    unsigned short* const PL[3][2] = {{xl[0], xl[1]}, {cl[0], cl[1]}, {al[0], al[1]}};
-    // planes_ready (bf16x3 mode): the producer of `in` already wrote its (hi, lo) planes into PH[m] / PL[m]
-    auto linear = [&](int l, int m, float* const in[2], const float* const bias[2], float* const resid[2], float* const out[2], int N, int K, int act,
-                      long long rows, bool planes_ready) -> int {
-        const LayerW &L0 = e->tw[0].L[l], &L1 = e->tw[1].L[l];
-        const float* Wfull[2];
-        switch (m) { case 0: Wfull[0] = L0.Wqkv; Wfull[1] = L1.Wqkv; break; case 1: Wfull[0] = L0.Wo; Wfull[1] = L1.Wo; break;
-                     case 2: Wfull[0] = L0.Wi; Wfull[1] = L1.Wi; break; default: Wfull[0] = L0.Wo2; Wfull[1] = L1.Wo2; }
-        const float* R[2] = {resid ? resid[0] : nullptr, resid ? resid[1] : nullptr};
-        if (!e->precise) {
-            const float* A[2] = {in[0], in[1]};
-            return dph_launch_gemm_tf32(2, A, Wfull, bias, resid ? R : nullptr, out, (int)rows, N, K, act, st, nullptr, nullptr);
-        }
-        if (e->precise == 2) {
-            // bf16x3: operands as (hi, lo) bf16 planes.  The FFN intermediate never exists in fp32: the GELU epilogue of GEMM m = 2
-            // writes its planes (into the memory of `out`), GEMM m = 3 reads them; the other inputs' planes come from their producers
-            // (LayerNorm / embedding / tensor-core attention) or, failing that, from one split pass.
-            const void *Whi[2], *Wlo[2], *Ahi[2], *Alo[2];
-            void *Ohi[2] = {nullptr, nullptr}, *Olo[2] = {nullptr, nullptr};
-            for (int t = 0; t < 2; t++) {
-                bf16_ptrs(e, t, l, m, &Whi[t], &Wlo[t]);
-                if (m == 3) {                                                     // planes left by GEMM m = 2 in `in`
-                    Ahi[t] = in[t]; Alo[t] = reinterpret_cast<const unsigned short*>(in[t]) + rows * (long long)K;
-                } else {
-                    if (!planes_ready) DPH_TRY(dph_launch_split_bf16(in[t], PH[m][t], PL[m][t], rows * K, st));
-                    Ahi[t] = PH[m][t]; Alo[t] = PL[m][t];
-                }
-                if (m == 2) { Ohi[t] = out[t]; Olo[t] = reinterpret_cast<unsigned short*>(out[t]) + rows * (long long)N; }
-            }
-            return dph_launch_gemm_bf16x3(2, Ahi, Alo, Whi, Wlo, bias, resid ? R : nullptr, m == 2 ? nullptr : out, m == 2 ? Ohi : nullptr,
-                                          m == 2 ? Olo : nullptr, (int)rows, N, K, act, st);
-        }
-        const float *Whi[2], *Wlo[2];
-        for (int t = 0; t < 2; t++) {
-            split_ptrs(e, t, l, m, &Whi[t], &Wlo[t]);
-            DPH_TRY(dph_launch_split_tf32(in[t], e->act_hi[t], e->act_lo[t], rows * K, st));
-        }
-        const float* Ahi[2] = {e->act_hi[0], e->act_hi[1]}; const float* Alo[2] = {e->act_lo[0], e->act_lo[1]};
-        return dph_launch_gemm_tf32(2, Ahi, Whi, bias, resid ? R : nullptr, out, (int)rows, N, K, act, st, Alo, Wlo);
-    };
-    for (int l = 0; l < ENC_LAYERS; l++) {
-        const LayerW &L0 = e->tw[0].L[l], &L1 = e->tw[1].L[l];
-        float* X[2] = {e->x[0], e->x[1]};
-        float* QKV[2] = {e->qkv[0], e->qkv[1]};
-        float* CTX[2] = {e->ctx[0], e->ctx[1]};
-        float* A2[2] = {e->a[0], e->a[1]};
-        float* FF[2] = {e->ffn[0], e->ffn[1]};
-        const float* bqkv[2] = {L0.bqkv, L1.bqkv}; const float* bo[2] = {L0.bo, L1.bo}; const float* bi[2] = {L0.bi, L1.bi}; const float* bo2[2] = {L0.bo2, L1.bo2};
-        const bool bx = e->precise == 2;
-        DPH_TRY(linear(l, 0, X, bqkv, nullptr, QKV, 3 * ENC_H, ENC_H, 0, T, bx));          // x planes: embedding LayerNorm / previous layer's LayerNorm
-        AttnArgs aa; aa.qkv[0] = e->qkv[0]; aa.qkv[1] = e->qkv[1]; aa.ctx[0] = e->ctx[0]; aa.ctx[1] = e->ctx[1]; aa.mask = d_mask; aa.S = S;
-        bool ctx_planes = false;
-        if (e->attention_tc && S <= 64) {      // tensor cores: TF32 in the 1xTF32 mode, the bf16 (hi, lo) plane kernel (fp32-accurate) in the precise modes
-            const float* q2[2] = {e->qkv[0], e->qkv[1]}; float* c2[2] = {e->ctx[0], e->ctx[1]};
-            DPH_TRY(dph_launch_attention_tc(q2, c2, d_mask, B, S, T, st, e->precise ? 1 : 0, bx ? ch : nullptr, bx ? cl : nullptr));
-            ctx_planes = bx;
-        } else {
-            DPH_TRY(launch_attention(aa, B, st));
-        }
-        // Only position 0 of the LAST layer is returned (encoder.py:116-117): after its attention, everything (attention output
-        // projection, both LayerNorms, the FFN) runs on the B [CLS] rows instead of all B*S tokens.
-        const bool last = (l == ENC_LAYERS - 1) && S >= 2;      // (S == 1: the scratch aliasing below needs T >= 2B rows)
-        long long rows = T;
-        if (last) {
-            rows = B;
-            const unsigned gb = (unsigned)((B * (ENC_H / 4) + 255) / 256);
-            gather_cls_kernel<<<dim3(gb, 2), 256, 0, st>>>(e->ctx[0], e->ctx[1], e->ffn[0], e->ffn[1], S, B);                         // ctx rows  -> ffn[:B]  (scratch)
-            gather_cls_kernel<<<dim3(gb, 2), 256, 0, st>>>(e->x[0], e->x[1], e->ffn[0] + (size_t)B * ENC_H, e->ffn[1] + (size_t)B * ENC_H, S, B);   // residual rows
-            DPH_CUDA(cudaGetLastError());
-            CTX[0] = e->ffn[0]; CTX[1] = e->ffn[1];
-            X[0] = e->ffn[0] + (size_t)B * ENC_H; X[1] = e->ffn[1] + (size_t)B * ENC_H;
-            FF[0] = e->qkv[0]; FF[1] = e->qkv[1];                                                                                     // qkv is dead after attention: [B, 3072] fits
-        }
-        DPH_TRY(linear(l, 1, CTX, bo, X, A2, ENC_H, ENC_H, 0, rows, ctx_planes && !last));           // dense + residual (last layer: gathered rows, split here)
-        LnArgs ln1; for (int t = 0; t < 2; t++) { ln1.in[t] = e->a[t]; ln1.out[t] = e->a[t]; ln1.out_hi[t] = bx ? ah[t] : nullptr; ln1.out_lo[t] = bx ? al[t] : nullptr; }
-        ln1.g[0] = L0.ln1g; ln1.g[1] = L1.ln1g; ln1.b[0] = L0.ln1b; ln1.b[1] = L1.ln1b;
-        ln1.rows = rows; ln1.in_stride = ENC_H; ln1.out_stride = ENC_H;
-        layernorm_kernel<<<dim3((unsigned)((rows + 7) / 8), 2), 256, 0, st>>>(ln1);
-        DPH_CUDA(cudaGetLastError());
-        DPH_TRY(linear(l, 2, A2, bi, nullptr, FF, ENC_FF, ENC_H, 1, rows, bx));                          // intermediate + erf-GELU
-        float* XO[2] = {last ? e->ctx[0] : e->x[0], last ? e->ctx[1] : e->x[1]};                         // last layer: dense [B,768] result in ctx
-        DPH_TRY(linear(l, 3, FF, bo2, A2, XO, ENC_H, ENC_FF, 0, rows, bx));                              // output dense + residual
-        LnArgs ln2; for (int t = 0; t < 2; t++) { ln2.in[t] = XO[t]; ln2.out[t] = XO[t]; ln2.out_hi[t] = (bx && !last) ? xh[t] : nullptr; ln2.out_lo[t] = (bx && !last) ? xl[t] : nullptr; }
-        ln2.g[0] = L0.ln2g; ln2.g[1] = L1.ln2g; ln2.b[0] = L0.ln2b; ln2.b[1] = L1.ln2b;
-        ln2.rows = rows; ln2.in_stride = ENC_H; ln2.out_stride = ENC_H;
-        layernorm_kernel<<<dim3((unsigned)((rows + 7) / 8), 2), 256, 0, st>>>(ln2);
-        DPH_CUDA(cudaGetLastError());
-    }
+    const long long *d_ids, *d_mask, *d_tt;
+    DPH_TRY(begin_forward(e, ids, mask, tt, T, B, 2, mem, &d_ids, &d_mask, &d_tt));
+    const int tws[2] = {0, 1};
+    DPH_TRY(encoder_forward(e, tws, 2, d_ids, d_mask, d_tt, B, S, false, nullptr, nullptr));
     // hidden state at position 0 of every sequence ([:, :1, :], encoder.py:116-117)
     float* ds = mem == DPH_MEM_HOST ? e->out_s : start_out;
     float* de = mem == DPH_MEM_HOST ? e->out_e : end_out;
@@ -650,12 +748,36 @@ DPH_API int dph_encoder_embed_query(dph_encoder* e, const int64_t* ids, const in
     if (mem == DPH_MEM_HOST) {
         DPH_CUDA(cudaMemcpyAsync(start_out, ds, (size_t)B * ENC_H * 4, cudaMemcpyDeviceToHost, st));
         DPH_CUDA(cudaMemcpyAsync(end_out, de, (size_t)B * ENC_H * 4, cudaMemcpyDeviceToHost, st));
-        int h = 0;
-        DPH_CUDA(cudaMemcpyAsync(&h, e->bad_ids, 4, cudaMemcpyDeviceToHost, st));
-        DPH_CUDA(cudaStreamSynchronize(st));
-        if (h) { DPH_CUDA(cudaMemsetAsync(e->bad_ids, 0, 4, st)); dph_set_error("encoder: input_ids / token_type_ids outside the embedding tables (IndexError in torch)"); return 1; }
-    } else {
-        e->bad_pending = true;
     }
-    return 0;
+    return end_forward(e, mem);
+}
+
+// == Encoder.forward(input_ids, attention_mask, token_type_ids, return_phrase=True) (encoder.py:130-144): ids/mask/tt int64 [B,S];
+// out fp32 [B,S,768] = the phrase tower's last hidden state (both `start` and `end` of the reference); filter_out (nullable)
+// fp32 [B,S,2] = filter_linear of it (start logit, end logit).
+DPH_API int dph_encoder_embed_phrase(dph_encoder* e, const int64_t* ids, const int64_t* mask, const int64_t* tt, int B, int S, float* out,
+                                     float* filter_out, int mem) {
+    DPH_CHECK(e && e->blob[2], "phrase tower (phrase_encoder) not loaded");
+    DPH_CHECK(ids && mask && tt && out, "embed_phrase: null buffer");
+    DPH_CHECK(!filter_out || e->filt, "filter head (filter_linear) not loaded");
+    // B <= 65535: the attention kernels' grid.y; with S <= 512 every token index (and T * 3072) fits the GEMMs' 32-bit M and TMA coordinates
+    DPH_CHECK(B >= 1 && B <= 65535 && S >= 1 && S <= ENC_MAX_S_PHRASE && S <= e->max_pos,
+              "phrase path: 1 <= B <= 65535 and 1 <= S <= min(512, max_position_embeddings)");
+    DPH_CHECK(e->attention_tc || S <= ENC_MAX_S, "the SIMT attention (set_attention(0)) handles S <= 384");
+    DPH_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    const int64_t T = (int64_t)B * S;
+    const long long *d_ids, *d_mask, *d_tt;
+    DPH_TRY(begin_forward(e, ids, mask, tt, T, 0, 1, mem, &d_ids, &d_mask, &d_tt));
+    // host buffers: the last LayerNorm writes into workspace that is dead by then (ctx after the last output projection, qkv after
+    // the last attention) and the rows are copied out; device buffers: straight into the caller's tensors
+    float* d_out = mem == DPH_MEM_HOST ? e->ctx[0] : out;
+    float* d_filt = filter_out ? (mem == DPH_MEM_HOST ? e->qkv[0] : filter_out) : nullptr;
+    const int tws[1] = {2};
+    DPH_TRY(encoder_forward(e, tws, 1, d_ids, d_mask, d_tt, B, S, true, d_out, d_filt));
+    if (mem == DPH_MEM_HOST) {
+        DPH_CUDA(cudaMemcpyAsync(out, d_out, (size_t)T * ENC_H * 4, cudaMemcpyDeviceToHost, st));
+        if (filter_out) DPH_CUDA(cudaMemcpyAsync(filter_out, d_filt, (size_t)T * 2 * 4, cudaMemcpyDeviceToHost, st));
+    }
+    return end_forward(e, mem);
 }

@@ -18,7 +18,7 @@ from collections import Counter
 import numpy as np
 import torch
 
-from .encoder import BertGeometry, Encoder, random_state_dict
+from .encoder import BertGeometry, Encoder, random_phrase_state_dict, random_state_dict
 from .mips import MIPS
 from .options import Options
 from .tokenization import WordPieceTokenizer
@@ -112,9 +112,8 @@ def load_encoder(device, args, phrase_only=False):
     """-> (model, tokenizer, config) from `args.load_dir/pytorch_model.bin` + a WordPiece `vocab.txt` (single_utils.py:59-118).
     A missing checkpoint or vocabulary raises FileNotFoundError like the reference does; seeded random weights and the
     synthetic character-level vocabulary are used only when the caller opts in with `args.allow_random_init = True` or the
-    environment variable DPH_ALLOW_RANDOM_INIT=1 (tests and benchmarks: no checkpoint is reachable offline)."""
-    if phrase_only:
-        raise NotImplementedError('the phrase tower is only used offline (generate_phrase_vecs.py); out of scope')
+    environment variable DPH_ALLOW_RANDOM_INIT=1 (tests and benchmarks: no checkpoint is reachable offline).
+    phrase_only (generate_phrase_vecs.py): only the phrase tower and the filter head are loaded; the query call then raises."""
     load_dir = getattr(args, 'load_dir', '') or ''
     allow_random = bool(getattr(args, 'allow_random_init', False)) or os.environ.get('DPH_ALLOW_RANDOM_INIT', '') == '1'
     config = BertGeometry()
@@ -138,12 +137,12 @@ def load_encoder(device, args, phrase_only=False):
         sd = backward_compat(torch.load(ckpt, map_location='cpu'))
         logger.info(f'DensePhrases encoder loaded from {load_dir}')
     elif allow_random:
-        sd = random_state_dict(config, getattr(args, 'seed', 42))
-        logger.warning('no checkpoint found: query encoder initialised with seeded random weights (allow_random_init)')
+        sd = (random_phrase_state_dict if phrase_only else random_state_dict)(config, getattr(args, 'seed', 42))
+        logger.warning('no checkpoint found: %s encoder initialised with seeded random weights (allow_random_init)', 'phrase' if phrase_only else 'query')
     else:
         raise FileNotFoundError(f'{ckpt} not found (hub ids are not resolvable offline); pass allow_random_init=True for seeded random weights')
     dev_index = torch.cuda.current_device() if str(device).startswith('cuda') else 0
-    model = Encoder(config, tokenizer=tokenizer, state_dict=sd, device=dev_index)
+    model = Encoder(config, tokenizer=tokenizer, state_dict=sd, device=dev_index, phrase_only=phrase_only)
     return model, tokenizer, config
 
 
