@@ -685,7 +685,7 @@ static int search_chunk(dph_index* ix, const float* x_dev, int64_t n, int k, flo
     DPH_TRY(ix->lutmin.ensure((size_t)n * DPH_M * 4));
     DPH_TRY(ix->lutmaxv.ensure((size_t)n * DPH_M * 4));
     if (pair) {
-        DPH_TRY(ix->lutq.ensure((size_t)n * DPH_LUT_SCAN_FLOATS * 2));
+        DPH_TRY(ix->lutq.ensure((size_t)n * (group == 4 ? DPH_LUTQ8_BYTES : DPH_LUT_SCAN_FLOATS * 2)));
         DPH_TRY(ix->qparams.ensure((size_t)n * 8));
         DPH_TRY(ix->gdense.ensure((size_t)n * nprobe * 4));
         DPH_TRY(ix->pl_cnt.ensure((size_t)ix->nlist * 4));

@@ -18,6 +18,7 @@
 #define DPH_MAX_NPROBE 1024
 #define DPH_SURV_CAP 2048          // merge kernel: survivors re-scored exactly per query
 #define DPH_LUT_SCAN_FLOATS (3 * 256 * 64)   // per query: 3 segments x 256 codes x (32 + 31 dup + 1 pad)
+#define DPH_LUTQ8_BYTES (3 * 256 * 32)       // per query: the quad scan's compact 8-bit table source (prep.cu, lutq_kernel)
 #define DPH_LUT_CANON_FLOATS (96 * 256)
 // The canonical fp32 table of a query, LUT[m][code] = <xr[8m..8m+8), pq[m][code]>, is stored segment-major, code-major,
 // sub-quantizer-minor: [3 segments of 32 sub-quantizers][256 codes][32] -- i.e. already in the row order the conflict-free scan

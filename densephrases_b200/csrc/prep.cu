@@ -616,7 +616,10 @@ __global__ void __launch_bounds__(256) lut_kernel(const float* __restrict__ xr, 
 // Quantised LUT for the pair-packed scan: qv[m][j] = round((LUT[m][j] - min_m) / step) in [0, 682], one step per query
 // (step = max_m range_m / 682) so that 96 entries sum below 2^16 and two queries' tables can share one 32-bit word.
 // Written in the scan layout ([3][256][64] u16); qparams[q] = (step, sum_m min_m).
-// Quad mode (four queries per gather): the same with 8-bit entries, qv in [0, 255] (96 * 255 < 2^15), T = unsigned char.
+// Quad mode (four queries per gather): the same with 8-bit entries, qv in [0, 255] (96 * 255 < 2^15), T = unsigned char, written as
+// the COMPACT source of the quad scan's packed tables: [3][256][32] bytes (DPH_LUTQ8_BYTES per query), no wrap copies.  Byte m of
+// row `code` is stored at m ^ ((code & 3) << 2): the table build moves 16-byte chunks of four rows at once, and this swizzle of the
+// 4-byte groups inside a chunk makes its 16-byte shared-memory stores conflict-free (scan.cu, scan_quad_kernel).
 #define DPH_QMAX 682
 #define DPH_QMAX8 255
 template <class T, int QMAX>
@@ -640,9 +643,12 @@ __global__ void __launch_bounds__(256) lutq_kernel(const float* __restrict__ lut
     for (int idx = j; idx < 256 * 32; idx += 256) tile[(idx >> 5) * 33 + (idx & 31)] = __ldg(src + idx);      // coalesced
     __syncthreads();
     const float inv = 1.0f / s_step;
-    T* dst = lutq + ((size_t)q * 3 + seg) * (256 * 64);
-    for (int idx = j; idx < 256 * 64; idx += 256) {
-        const int row = idx >> 6, w = idx & 63, ml = w & 31;
+    constexpr bool QUAD = sizeof(T) == 1;
+    constexpr int RW = QUAD ? 32 : 64;               // row width in entries
+    T* dst = lutq + ((size_t)q * 3 + seg) * (256 * RW);
+    for (int idx = j; idx < 256 * RW; idx += 256) {
+        const int row = idx / RW, w = idx % RW;
+        const int ml = QUAD ? (w ^ ((row & 3) << 2)) : (w & 31);
         int qv = (int)((tile[row * 33 + ml] - s_min[ml]) * inv + 0.5f);
         qv = qv < 0 ? 0 : (qv > QMAX ? QMAX : qv);
         dst[idx] = (w < 63) ? (T)qv : (T)0;

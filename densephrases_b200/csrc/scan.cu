@@ -53,6 +53,31 @@ __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
 __device__ __forceinline__ void l2_prefetch_block(const void* p) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(p), "n"(DPH_BLK_BYTES) : "memory");
 }
+// The same two with an L2 eviction-priority policy (createpolicy): per-instruction hints only, no device-wide L2 set-aside.
+__device__ __forceinline__ uint4 ldg_stream(const uint4* p, unsigned long long pol) {
+    uint4 r;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ void l2_prefetch_block(const void* p, unsigned long long pol) {
+    asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" :: "l"(p), "n"(DPH_BLK_BYTES), "l"(pol) : "memory");
+}
+__device__ __forceinline__ uint4 ldg_policy(const uint4* p, unsigned long long pol) {
+    uint4 r;
+    asm volatile("ld.global.nc.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ unsigned long long l2_policy_evict_first() {
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ unsigned long long l2_policy_evict_last() {
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
 
 extern __shared__ __align__(1024) unsigned char dph_smem[];
 // The dynamic shared memory window of a kernel without static shared memory starts at this shared-space address on
@@ -529,10 +554,12 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(PairScanArgs a) {
 #define QCAP 512                   // QCAP - QNT = DPH_QUAD_KEEP_MAX (each warp adds <= 32 per buffer after the latch is polled)
 #define SMEM_QUAD_TABLES (3 * 65536)
 static_assert(QCAP - QNT == DPH_QUAD_KEEP_MAX, "quad latch margin");
+static_assert(offsetof(DphUnit, bend) < 32, "the run-out prefetch reads the block range from the record's first 32 bytes");
 struct QuadShared {
     unsigned long long cbuf[DPH_QUAD_ITEM_Q][QCAP];
     SelectScratch sc;
     DphUnit desc[2];                 // current item / next item (fetched with cp.async while the current one is scanned)
+    uint4 head[QNW][2];              // per warp: the first 32 bytes of the next item's record (its block range), for the run-out prefetch
     int cnt[DPH_QUAD_ITEM_Q]; unsigned thr[DPH_QUAD_ITEM_Q]; int base[DPH_QUAD_ITEM_Q]; int ndone; int ndone_snap; int unit; int full;
     long long qs[DPH_QUAD_ITEM_Q];   // the group's queries (shared copy: indexed by thread id in the publish step)
 };
@@ -624,12 +651,29 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long l
 #define QPH_MARK(i) do { } while (0)
 #endif
 
+// A warp that runs out of blocks starts the next item's stream: it waits for its copy of the next record's head (requested with
+// cp.async after this item's table build; warp 0 also waits for the whole record here) and issues the L2 prefetch of its first
+// DPH_L2_PREFETCH_ROUNDS blocks of the next item, so HBM keeps streaming while the other warps finish, compact and publish.
+__device__ __forceinline__ void quad_prefetch_next(const PairScanArgs& a, const QuadShared* sh, int total_units, unsigned long long pol) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    if (lane == 0 && sh->unit < total_units) {
+        const DphUnit* nd = reinterpret_cast<const DphUnit*>(sh->head[warp]);
+        const uint4* lb = reinterpret_cast<const uint4*>(a.codes + nd->blk * DPH_BLK_BYTES);
+        const unsigned bend = nd->bend;
+        unsigned bp = nd->bi0 + warp;
+#pragma unroll 1
+        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += QNW) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol);
+    }
+}
+
 // The scan of one item over its block range with NTAB packed tables: rounds until a candidate buffer may overflow or the warp is out
 // of blocks, then a barrier, the compaction of the buffers over keep and the refresh of the thresholds; until every warp is done.
+// The code stream is loaded with the evict_first policy `pol`: each block is read once per batch.
 template <int NTAB, int IMADL>
 __device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
-                                                 unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, unsigned long long* ph,
-                                                 unsigned long long& ph_t) {
+                                                 unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, int total_units,
+                                                 unsigned long long pol, unsigned long long* ph, unsigned long long& ph_t) {
     (void)ph; (void)ph_t;
     const int lane = threadIdx.x & 31;
     const int len = dsc->len, nq = dsc->nq;
@@ -646,13 +690,13 @@ __device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShar
 #pragma unroll
             for (int c6 = 0; c6 < 6; c6++) cur6[c6] = nxt[c6];
             const unsigned bcur = b;
-            if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16)); bp += QNW; }
+            if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16), pol); bp += QNW; }
             b += QNW;
             more = b < bend;
             if (more) {
                 const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
-                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
             }
             unsigned sr[2][4] = {}, ab[2][4] = {};
             quad_chunk<0, NTAB, IMADL>(cur6[0], rot, one, sr, ab);
@@ -687,7 +731,11 @@ __device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShar
                 }
             }
         }
-        if (!more && !counted) { counted = true; if (lane == 0) atomicAdd(&sh->ndone, 1); }
+        if (!more && !counted) {
+            counted = true;
+            quad_prefetch_next(a, sh, total_units, pol);
+            if (lane == 0) atomicAdd(&sh->ndone, 1);
+        }
         __syncthreads();
         QPH_MARK(1);
 #pragma unroll 1
@@ -706,11 +754,29 @@ __device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShar
     }
 }
 
-// Item start-up is kept off the critical path: the plan resolves every unit into one DphUnit record; the record of the NEXT unit is
-// fetched into shared memory with cp.async while the current one is scanned (its queue index is requested at the start of the current
-// item, so that the fetch can be issued right after the table build); the first code blocks of an item are requested BEFORE the
-// packed tables are built, so the HBM latency overlaps the build; the build reads only the 32 real bytes of every 64-byte row of the
-// quantised tables.
+// 4 x 4 byte transpose: word j of the result = byte j of a, b, c, d (query 0..3 of a packed table).
+__device__ __forceinline__ uint4 quad_pack(unsigned a, unsigned b, unsigned c, unsigned d) {
+    const unsigned t0 = __byte_perm(a, b, 0x5140), t1 = __byte_perm(a, b, 0x7362);     // [a0 b0 a1 b1], [a2 b2 a3 b3]
+    const unsigned u0 = __byte_perm(c, d, 0x5140), u1 = __byte_perm(c, d, 0x7362);
+    return make_uint4(__byte_perm(t0, u0, 0x5410), __byte_perm(t0, u0, 0x7632), __byte_perm(t1, u1, 0x5410), __byte_perm(t1, u1, 0x7632));
+}
+// This warp's first code block of an item into registers.
+__device__ __forceinline__ void quad_first_block(const PairScanArgs& a, const DphUnit* d, uint4 (&nxt)[6], unsigned long long pol) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned b = d->bi0 + warp;
+    if (b < d->bend) {
+        const uint4* p = reinterpret_cast<const uint4*>(a.codes + d->blk * DPH_BLK_BYTES) + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+#pragma unroll
+        for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
+    }
+}
+
+// Item start-up is kept off the critical path, so that HBM streams across item boundaries: the plan resolves every unit into one
+// DphUnit record; the record of the NEXT unit is fetched into shared memory with cp.async while the current one is scanned (its queue
+// index is requested at the start of the current item, so that the fetch can be issued right after the table build); a warp that runs
+// out of blocks prefetches its first blocks of the next item into L2 (quad_prefetch_next), and every warp loads its first block of the
+// next item into registers before the candidates are published, so those are in flight during the publish and the next table build.
+// The table sources (a few MB per batch, re-read at every item) are loaded evict_last, the code stream evict_first.
 template <int IMADL>
 __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
     unsigned char* const smem = dph_smem;
@@ -719,6 +785,7 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
     const int total_units = a.work->total_units;
     const unsigned char* lut8 = reinterpret_cast<const unsigned char*>(a.lutq);
     const unsigned one = a.one;
+    const unsigned long long pol_stream = l2_policy_evict_first(), pol_table = l2_policy_evict_last();
     unsigned rot[11];
 #pragma unroll
     for (int r = 0; r < 11; r++) {
@@ -740,82 +807,83 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
     if (any_unit && tid < (int)(sizeof(DphUnit) / 16))
         reinterpret_cast<uint4*>(&sh->desc[0])[tid] = __ldg(reinterpret_cast<const uint4*>(a.udesc + sh->unit) + tid);
     __syncthreads();
+    uint4 nxt[6];
+    if (any_unit) {      // the first item's first blocks; later items get theirs at the end of the previous item
+        const DphUnit* d = &sh->desc[0];
+        const uint4* lb = reinterpret_cast<const uint4*>(a.codes + d->blk * DPH_BLK_BYTES);
+        unsigned bp = d->bi0 + warp;
+#pragma unroll 1
+        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < d->bend; r++, bp += QNW)
+            if (lane == 0) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol_stream);
+        quad_first_block(a, d, nxt, pol_stream);
+    }
     while (any_unit) {
         int next_u = 0;
         if (tid == 0) next_u = atomicAdd(a.next_unit, 1);          // consumed after the table build (fetch of the next record)
         const DphUnit* dsc = &sh->desc[cur];
         const int nq = dsc->nq;
         const int ntab = nq > 4 ? 2 : 1;
-        const unsigned bi0 = dsc->bi0, bend = dsc->bend;
+        const unsigned bi0 = dsc->bi0;
         const uint4* lbase = reinterpret_cast<const uint4*>(a.codes + dsc->blk * DPH_BLK_BYTES);
-
-        // ---- first code blocks: L2 prefetch + this warp's first block into registers, in flight during the table build ----
-        unsigned b = bi0 + warp, bp = bi0 + warp;
-        uint4 nxt[6];
-#pragma unroll 1
-        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += QNW)
-            if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16));
-        if (b < bend) {
-            const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
-#pragma unroll
-            for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
-        }
+        // this warp's first block is in registers and its first DPH_L2_PREFETCH_ROUNDS blocks are requested into L2
+        const unsigned b = bi0 + warp, bp = bi0 + warp + DPH_L2_PREFETCH_ROUNDS * QNW;
         unsigned gq = 0xFFFFFFFFu;
         if (tid < DPH_QUAD_ITEM_Q && tid < nq) gq = *((volatile unsigned*)(a.gthr + dsc->q[tid]));
         {   // ---- packed tables: byte j of a word of table t = query 4t + j's 8-bit entry, wrap-free layout (see above) ----
-            const unsigned* src[DPH_QUAD_ITEM_Q];
-#pragma unroll
-            for (int i = 0; i < DPH_QUAD_ITEM_Q; i++) src[i] = reinterpret_cast<const unsigned*>(lut8 + (size_t)dsc->q[i] * DPH_LUT_SCAN_FLOATS);
+            // A unit = one 16-byte chunk (four words) of one source row of the table's four queries: four 16-byte loads, a 4 x 4 byte
+            // transpose per word, four 16-byte stores.  All 24 loads of a thread (96 KB per CTA) are issued before any store.  The
+            // source swizzle (prep.cu: word group g of row `code` at g ^ (code & 3) inside its chunk) spreads the eight threads of a
+            // quarter-warp over the eight 16-byte bank groups of a half-row, so the stores are conflict-free.  The empty slots of a
+            // short group repeat query 0 (their byte lanes are summed like the others and never pass: threshold +inf), so all loads are
+            // unconditional.
+            constexpr int UPT = 3 * 256 * 2 / QNT;
+            static_assert(UPT * QNT == 3 * 256 * 2, "the build's units divide evenly over the threads");
             uint4* dst = reinterpret_cast<uint4*>(smem);
-            // (table, row, group of four real words): a quarter-warp moves one 128-byte half-row.  The empty slots of a short group
-            // repeat query 0 (their byte lanes are summed like the others and never pass: threshold +inf), so all four loads are
-            // unconditional and a thread keeps 24 of them in flight.
-            constexpr int LB = 6, PER_TAB = 768 * 8;
-            static_assert(PER_TAB % (QNT * LB) == 0, "a batch of the build stays inside one table");
 #pragma unroll 1
-            for (int i0 = tid; i0 < ntab * PER_TAB; i0 += QNT * LB) {
-                const int tb = i0 >= PER_TAB;
-                const unsigned* T0p = tb ? src[4] : src[0];
-                const unsigned* T1p = tb ? src[5] : src[1];
-                const unsigned* T2p = tb ? src[6] : src[2];
-                const unsigned* T3p = tb ? src[7] : src[3];
-                const int ib = i0 - tb * PER_TAB;
-                unsigned va[LB], vb[LB], vc[LB], vd[LB];
+            for (int tb = 0; tb < ntab; tb++) {
+                const uint4* s0 = reinterpret_cast<const uint4*>(lut8 + (size_t)dsc->q[4 * tb + 0] * DPH_LUTQ8_BYTES);
+                const uint4* s1 = reinterpret_cast<const uint4*>(lut8 + (size_t)dsc->q[4 * tb + 1] * DPH_LUTQ8_BYTES);
+                const uint4* s2 = reinterpret_cast<const uint4*>(lut8 + (size_t)dsc->q[4 * tb + 2] * DPH_LUTQ8_BYTES);
+                const uint4* s3 = reinterpret_cast<const uint4*>(lut8 + (size_t)dsc->q[4 * tb + 3] * DPH_LUTQ8_BYTES);
+                uint4 va[UPT], vb[UPT], vc[UPT], vd[UPT];
 #pragma unroll
-                for (int e = 0; e < LB; e++) {
-                    const int i = ib + e * QNT, s = (i >> 3) * 16 + (i & 7);
-                    va[e] = __ldg(T0p + s); vb[e] = __ldg(T1p + s); vc[e] = __ldg(T2p + s); vd[e] = __ldg(T3p + s);
+                for (int e = 0; e < UPT; e++) {
+                    const int u = tid + e * QNT;
+                    va[e] = ldg_policy(s0 + u, pol_table); vb[e] = ldg_policy(s1 + u, pol_table);
+                    vc[e] = ldg_policy(s2 + u, pol_table); vd[e] = ldg_policy(s3 + u, pol_table);
                 }
 #pragma unroll
-                for (int e = 0; e < LB; e++) {
-                    const int i = ib + e * QNT, row = i >> 3, cg = i & 7;
-                    const int seg = row >> 8, code = row & 255;
+                for (int e = 0; e < UPT; e++) {
+                    const int u = tid + e * QNT, row = u >> 1, h = u & 1;
+                    const int seg = row >> 8, code = row & 255, sw = code & 3;
                     const int region = seg < 2 ? tb : 2, half = seg < 2 ? seg : tb;
-                    const unsigned t0 = __byte_perm(va[e], vb[e], 0x5140), t1 = __byte_perm(va[e], vb[e], 0x7362);     // [a0 b0 a1 b1], [a2 b2 a3 b3]
-                    const unsigned u0 = __byte_perm(vc[e], vd[e], 0x5140), u1 = __byte_perm(vc[e], vd[e], 0x7362);
-                    uint4 o;
-                    o.x = __byte_perm(t0, u0, 0x5410); o.y = __byte_perm(t0, u0, 0x7632);
-                    o.z = __byte_perm(t1, u1, 0x5410); o.w = __byte_perm(t1, u1, 0x7632);
-                    dst[region * 4096 + code * 16 + half * 8 + cg] = o;
+                    uint4* d = dst + region * 4096 + code * 16 + half * 8 + h * 4;
+                    d[0 ^ sw] = quad_pack(va[e].x, vb[e].x, vc[e].x, vd[e].x);
+                    d[1 ^ sw] = quad_pack(va[e].y, vb[e].y, vc[e].y, vd[e].y);
+                    d[2 ^ sw] = quad_pack(va[e].z, vb[e].z, vc[e].z, vd[e].z);
+                    d[3 ^ sw] = quad_pack(va[e].w, vb[e].w, vc[e].w, vd[e].w);
                 }
             }
         }
         if (tid < DPH_QUAD_ITEM_Q) { sh->cnt[tid] = 0; sh->qs[tid] = (long long)dsc->q[tid]; sh->thr[tid] = gq; }
-        if (tid == 0) { sh->ndone = 0; sh->ndone_snap = 0; sh->full = 0; }
+        if (tid == 0) { sh->ndone = 0; sh->ndone_snap = 0; sh->full = 0; sh->unit = next_u; }
         __syncthreads();
         QPH_MARK(0);
-        if (warp == 0) {          // the next unit's record -> the other descriptor slot (waited for at the end of this item)
-            const int nu = __shfl_sync(0xffffffffu, next_u, 0);
-            if (lane == 0) sh->unit = nu;
-            if (nu < total_units && lane < (int)(sizeof(DphUnit) / 16))
-                cp_async16(reinterpret_cast<unsigned char*>(&sh->desc[cur ^ 1]) + lane * 16, reinterpret_cast<const unsigned char*>(a.udesc + nu) + lane * 16);
-            asm volatile("cp.async.commit_group;" ::: "memory");
+        // the next unit's record: its head to every warp's slot (for the run-out prefetch), all of it to the other descriptor slot
+        const int nu = sh->unit;
+        if (nu < total_units) {
+            const unsigned char* rec = reinterpret_cast<const unsigned char*>(a.udesc + nu);
+            if (lane == 0) { cp_async16(&sh->head[warp][0], rec); cp_async16(&sh->head[warp][1], rec + 16); }
+            if (warp == 0 && lane < (int)(sizeof(DphUnit) / 16)) cp_async16(reinterpret_cast<unsigned char*>(&sh->desc[cur ^ 1]) + lane * 16, rec + lane * 16);
         }
-        if (ntab == 2) quad_item_rounds<2, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, ph, ph_t);
-        else quad_item_rounds<1, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, ph, ph_t);
+        asm volatile("cp.async.commit_group;" ::: "memory");
+        if (ntab == 2) quad_item_rounds<2, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t);
+        else quad_item_rounds<1, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t);
+        // every warp waited for its copies before the rounds' last barrier: the next record is visible
+        any_unit = nu < total_units;
+        if (any_unit) quad_first_block(a, &sh->desc[cur ^ 1], nxt, pol_stream);
         // ---- publish the candidate sets: the (up to) eight region reservations go out together, one barrier ----
         if (tid < nq) sh->base[tid] = atomicAdd(a.cand_cnt + sh->qs[tid], sh->cnt[tid]);
-        if (warp == 0) asm volatile("cp.async.wait_all;" ::: "memory");
         __syncthreads();
 #pragma unroll 1
         for (int i = 0; i < nq; i++) {
@@ -826,7 +894,6 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
             for (int c = tid; c < cnt; c += QNT)
                 if (basep + c < cap) a.cand[off + basep + c] = sh->cbuf[i][c];
         }
-        any_unit = sh->unit < total_units;
         __syncthreads();             // buffers, counters, sh->unit and the descriptor slots are reused by the next item
         QPH_MARK(3);
         cur ^= 1;
