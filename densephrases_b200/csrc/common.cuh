@@ -108,6 +108,8 @@ __host__ __device__ __forceinline__ int dph_blk_addr(int lane, int m) {
     int t = seg * 32 + s;
     return (t >> 4) * 512 + lane * 16 + (t & 15);
 }
+// The inverse: the sub-quantizer held at position t (0..95) of lane `lane`'s row.
+__host__ __device__ __forceinline__ int dph_blk_sub(int lane, int t) { return (t & ~31) + ((lane + (t & 31)) & 31); }
 
 // Segment descriptor produced by the plan kernel: one per (query, probe rank); 32 bytes.
 struct __align__(16) DphSeg {

@@ -36,6 +36,21 @@ struct DevBuf {            // grow-only device buffer
     template <class T> T* as() const { return (T*)p; }
 };
 
+// The shard's lists as tightly packed 32-row code blocks, derived from the lengths of all lists (DESIGN.md 3).  set_lists, add,
+// remove and sync_list_len build one; dph_commit_layout makes it the handle's (dph_index::lay).
+struct DphLayout {
+    int64_t lo = 0, hi = 0;             // the shard's lists
+    std::vector<int32_t> len;           // [nlist]
+    std::vector<int64_t> start;         // [nlist+1] global list-major row of each list's first vector
+    std::vector<int64_t> blk_off;       // [nlist]   first code block of the list in the shard (-1 outside it)
+    std::vector<int64_t> row_start;     // [max(hi-lo, 1)] shard-local row of each shard list's first vector
+    int64_t nblocks = 0, rows = 0;      // of the shard
+    // Fails with `what` (the index unchanged) unless 0 <= list_len[l] < 2^31 for every list.
+    int build(const dph_index* ix, const int64_t* list_len, const char* what);
+    // Staging chunks: runs of whole lists of at most dph_chunk_rows() rows (a longer list is a chunk alone), no empty chunk.
+    struct Chunk { int64_t row0, rows, blk0, blk1; };      // shard-local rows [row0, row0 + rows), blocks [blk0, blk1)
+    std::vector<Chunk> chunks(int64_t* max_rows) const;
+};
 struct dph_index {
     int device = 0;
     int d = DPH_D, M = DPH_M;
@@ -61,10 +76,9 @@ struct dph_index {
     int64_t* dm_ids = nullptr;
     int64_t* dm_rows = nullptr;
     int64_t dm_n = 0;
-    int64_t dm_cap = -1;                // entries allocated for dm_ids / dm_rows (-1: as set_lists sized them, ntotal_local)
-    std::vector<int64_t> h_list_len;    // host copies
-    std::vector<int64_t> h_list_start;
-    int64_t bytes = 0;
+    int64_t dm_cap = 0;                 // entries allocated for dm_ids / dm_rows
+    int64_t blk_cap = 0;                // blocks allocated for codes / ids (a remove does not shrink them)
+    DphLayout lay;                      // host copy of the committed layout
 
     // per-batch workspace
     DevBuf xdev, xr, S, key, cd, lut_canon, lutmax, segs, wpre, qinfo, cand, cand_off, cand_cnt, gthr, flags,
@@ -81,13 +95,18 @@ struct dph_index {
     bool profile = false;              // CUDA events around the scan kernel of the last search chunk
     cudaEvent_t ev0[DPH_PROF_RING] = {}, ev1[DPH_PROF_RING] = {};
     int64_t prof_n = 0;
-    cudaEvent_t aev[6] = {};           // profiled adds and removes: stage boundaries (encode.cu, index.cu, remove.cu)
+    cudaEvent_t aev[6] = {};           // profiled adds and removes: stage boundaries (encode.cu, lists.cu, remove.cu)
     float add_ms[4] = {};              // last add: rotation, coarse, PQ encode, re-layout + scatter (ms)
-    float remove_ms[3] = {};
-    float train_ms[3] = {};            // last train_coarse / train_pq: assign, sort + update, split + renorm (ms, summed over iterations)           // last remove: mark + plan, row moves + block shift, direct map (ms)
+    float remove_ms[3] = {};           // last remove: mark + plan, row moves + block shift, direct map (ms)
+    float train_ms[3] = {};            // last train_coarse / train_pq: assign, sort + update, split + renorm (ms, summed over iterations)
     int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
-    int64_t blk_cap = -1;              // blocks allocated for codes / ids (-1: nblocks_local; a remove does not shrink them)
 };
+
+// Writes list_len / list_start / blk_off of `L` to the device and makes `L` the handle's layout, totals included; the only code
+// that does.
+int dph_commit_layout(dph_index* ix, DphLayout L);
+void dph_free_lists(dph_index* ix);            // the handle's list arrays go; it then has no lists
+int check_ready(dph_index* ix, int k);
 
 // Block -> list lookup inside the shard: last l in [lo,hi) with blk_off[l] <= blk.
 __device__ __forceinline__ long long list_of_block(const long long* blk_off, long long lo, long long hi, long long blk) {
@@ -99,9 +118,8 @@ __device__ __forceinline__ void dph_store_row(uint8_t* codes, long long blk, int
 #pragma unroll
     for (int c = 0; c < 6; c++) {
         unsigned char bytes[16];
-        const int seg = c >> 1;
 #pragma unroll
-        for (int b = 0; b < 16; b++) { const int t = c * 16 + b; bytes[b] = row[seg * 32 + ((lane + (t & 31)) & 31)]; }
+        for (int b = 0; b < 16; b++) bytes[b] = row[dph_blk_sub(lane, c * 16 + b)];
         uint4 v;
         memcpy(&v, bytes, 16);
         *reinterpret_cast<uint4*>(codes + blk * DPH_BLK_BYTES + c * 512 + lane * 16) = v;
@@ -114,9 +132,8 @@ __device__ __forceinline__ void dph_load_row(const uint8_t* codes, long long blk
         const uint4 v = *reinterpret_cast<const uint4*>(codes + blk * DPH_BLK_BYTES + c * 512 + lane * 16);
         unsigned char bytes[16];
         memcpy(bytes, &v, 16);
-        const int seg = c >> 1;
 #pragma unroll
-        for (int b = 0; b < 16; b++) { const int t = c * 16 + b; row[seg * 32 + ((lane + (t & 31)) & 31)] = bytes[b]; }
+        for (int b = 0; b < 16; b++) row[dph_blk_sub(lane, c * 16 + b)] = bytes[b];
     }
 }
 
@@ -142,7 +159,7 @@ struct DevTmp {            // the device allocations of one call, freed on every
 
 // Rows per staging chunk of set_lists / copy_lists / remove (about 256 MB of code rows; DPH_UPLOAD_CHUNK_ROWS overrides it for tests).
 int64_t dph_chunk_rows();
-// Block re-layout of the add (index.cu), also the remove's block shift: blocks [blk0, blk0 + gridDim.x) of the layout boff_new are
+// Block re-layout of the add (lists.cu), also the remove's block shift: blocks [blk0, blk0 + gridDim.x) of the layout boff_new are
 // written to dst[0 ..) from the same list's block in boff_old (whole, same rows and lanes; zeros / -1 past the list's old end).
 __global__ void relayout_codes_kernel(uint8_t* dst, long long blk0, const long long* boff_new, const long long* boff_old, const int* len_old,
                                       long long lo, long long hi, const uint8_t* codes_old);

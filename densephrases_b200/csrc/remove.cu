@@ -141,6 +141,7 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[0], st));
 
     // 0. implicit labels become explicit (list_start[l] + j), exactly as the first add does, into new arrays
+    const DphLayout& old = ix->lay;
     const int64_t nb = ix->nblocks_local;
     const long long* bo = (const long long*)ix->blk_off;
     long long *w_ids = (long long*)ix->ids, *w_dm_ids = (long long*)ix->dm_ids, *w_dm_rows = (long long*)ix->dm_rows;
@@ -148,12 +149,10 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     const bool was_implicit = ix->ids == nullptr;
     if (was_implicit) {
         const char* oom0 = "remove_ids: not enough device memory for the labels and direct map of an index with sequential labels; the index is unchanged";
-        std::vector<int64_t> lrs(std::max<int64_t>(hi - lo, 1), 0);
-        for (int64_t l = lo, rows = 0; l < hi; l++) { lrs[l - lo] = rows; rows += ix->h_list_len[l]; }
         int64_t* d_lrs;
         DPH_TRY(conv.alloc(&w_ids, (size_t)nb * 32, oom0)); DPH_TRY(conv.alloc(&w_dm_ids, ix->ntotal_local, oom0));
-        DPH_TRY(conv.alloc(&w_dm_rows, ix->ntotal_local, oom0)); DPH_TRY(tmp.alloc(&d_lrs, lrs.size(), oom));
-        DPH_CUDA(cudaMemcpyAsync(d_lrs, lrs.data(), lrs.size() * 8, cudaMemcpyHostToDevice, st));
+        DPH_TRY(conv.alloc(&w_dm_rows, ix->ntotal_local, oom0)); DPH_TRY(tmp.alloc(&d_lrs, old.row_start.size(), oom));
+        DPH_CUDA(cudaMemcpyAsync(d_lrs, old.row_start.data(), old.row_start.size() * 8, cudaMemcpyHostToDevice, st));
         if (nb > 0)
             relayout_ids_kernel<<<(unsigned)nb, 32, 0, st>>>(w_ids, 0, bo, bo, ix->list_len, lo, hi, nullptr, (const long long*)ix->list_start,
                                                            (const long long*)d_lrs, w_dm_ids, w_dm_rows);
@@ -223,19 +222,15 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
         DPH_CUDA(cudaStreamSynchronize(st));
     }
 
-    // 2. plan: new lengths, list starts and block offsets; the first block that moves
-    std::vector<int64_t> len_new(ix->h_list_len), start_new(nlist + 1, 0), boff_new(nlist, -1), rm_off(nlist, 0);
-    std::vector<int32_t> len32(nlist);
-    int64_t nb_new = 0, d_first = -1, acc = 0;
-    for (int64_t l = lo, ob = 0; l < hi; l++) {
-        len_new[l] -= h_cnt[l];
-        rm_off[l] = acc; acc += h_cnt[l];
-        boff_new[l] = nb_new;
-        if (d_first < 0 && nb_new != ob) d_first = nb_new;
-        nb_new += (len_new[l] + 31) / 32; ob += (ix->h_list_len[l] + 31) / 32;
-    }
-    if (d_first < 0) d_first = nb_new;
-    for (int64_t l = 0; l < nlist; l++) { start_new[l + 1] = start_new[l] + len_new[l]; len32[l] = (int32_t)len_new[l]; }
+    // 2. plan: the new layout; the first block that moves
+    std::vector<int64_t> len_new(old.len.begin(), old.len.end()), rm_off(nlist, 0);
+    for (int64_t l = lo, acc = 0; l < hi; l++) { len_new[l] -= h_cnt[l]; rm_off[l] = acc; acc += h_cnt[l]; }
+    DphLayout L;
+    DPH_TRY(L.build(ix, len_new.data(), "remove_ids: bad list length; the index is unchanged"));
+    const int64_t nb_new = L.nblocks;
+    int64_t d_first = nb_new;
+    for (int64_t l = lo; l < hi; l++)
+        if (L.blk_off[l] != old.blk_off[l]) { d_first = L.blk_off[l]; break; }
     const int64_t dm_new = dm_n - R;
     // one staging buffer (<= ~256 MB) serves the block shift (codes + labels of chunk_blocks blocks) and the direct map (pairs)
     const int64_t max_blocks = std::max<int64_t>(1, dph_chunk_rows() * DPH_CODE / (DPH_BLK_BYTES + 256));
@@ -245,7 +240,7 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     uint8_t* stage = nullptr;
     if (R > 0) {
         DPH_TRY(tmp.alloc(&stage, (size_t)stage_bytes, oom));
-        DPH_CUDA(cudaMemcpyAsync(d_boff_new, boff_new.data(), nlist * 8, cudaMemcpyHostToDevice, st));
+        DPH_CUDA(cudaMemcpyAsync(d_boff_new, L.blk_off.data(), nlist * 8, cudaMemcpyHostToDevice, st));
         DPH_CUDA(cudaMemcpyAsync(d_rm_off, rm_off.data(), nlist * 8, cudaMemcpyHostToDevice, st));
         rm_plan_moves_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(rm_prow, R, bo, ix->list_len, d_cnt, d_rm_off, lo, hi, mv_src, mv_dst);
         DPH_CUDA(cudaGetLastError());
@@ -293,22 +288,14 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[3], st));
     DPH_CUDA(cudaStreamSynchronize(st));
 
-    // 6. commit: tables, then the label arrays an implicit-label index gained
-    if (R > 0) {
-        DPH_CUDA(cudaMemcpy(ix->blk_off, d_boff_new, nlist * 8, cudaMemcpyDeviceToDevice));
-        DPH_CUDA(cudaMemcpy(ix->list_len, len32.data(), nlist * 4, cudaMemcpyHostToDevice));
-        DPH_CUDA(cudaMemcpy(ix->list_start, start_new.data(), (nlist + 1) * 8, cudaMemcpyHostToDevice));
-    }
+    // 6. commit: the label arrays an implicit-label index gained, then the layout
     if (was_implicit) {
         ix->ids = (int64_t*)w_ids; ix->dm_ids = (int64_t*)w_dm_ids; ix->dm_rows = (int64_t*)w_dm_rows;
         for (void* p : {(void*)w_ids, (void*)w_dm_ids, (void*)w_dm_rows}) conv.release(p);
-        ix->bytes += std::max<int64_t>(nb * 32, 1) * 8 + 2 * std::max<int64_t>(ix->ntotal_local, 1) * 8;
         ix->dm_cap = ix->ntotal_local;
     }
-    if (ix->blk_cap < 0) ix->blk_cap = nb;
+    if (R > 0) DPH_TRY(dph_commit_layout(ix, std::move(L)));
     ix->dm_n = dm_new;
-    ix->h_list_len = len_new; ix->h_list_start = start_new;
-    ix->ntotal = start_new[nlist]; ix->ntotal_local -= R; ix->nblocks_local = nb_new;
     ix->remove_tmp_peak = tmp.peak;
     if (prof)
         for (int s = 0; s < 3; s++) DPH_CUDA(cudaEventElapsedTime(&ix->remove_ms[s], ix->aev[s], ix->aev[s + 1]));
@@ -319,27 +306,19 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
 
 DPH_API int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len) {
     DPH_CHECK(ix && ix->list_len, "sync_list_len: lists are not set");
-    const int64_t nlist = ix->nlist;
+    DphLayout L;
+    DPH_TRY(L.build(ix, list_len, "sync_list_len: bad list length; the index is unchanged"));
     bool changed = false;
-    for (int64_t l = 0; l < nlist; l++) {
-        DPH_CHECK(list_len[l] >= 0 && list_len[l] < (1ll << 31), "sync_list_len: bad list length; the index is unchanged");
+    for (int64_t l = 0; l < ix->nlist; l++) {
         if (l >= ix->list_lo && l < ix->list_hi)
-            DPH_CHECK(list_len[l] == ix->h_list_len[l], "sync_list_len: a list of this shard has another length here; the index is unchanged");
-        changed |= list_len[l] != ix->h_list_len[l];
+            DPH_CHECK(list_len[l] == ix->lay.len[l], "sync_list_len: a list of this shard has another length here; the index is unchanged");
+        changed |= list_len[l] != ix->lay.len[l];
     }
     if (!changed) return 0;
     DPH_CHECK(ix->ids != nullptr, "sync_list_len: the labels of this shard are sequential and would move; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
-    std::vector<int64_t> start(nlist + 1, 0);
-    std::vector<int32_t> len32(nlist);
-    for (int64_t l = 0; l < nlist; l++) { start[l + 1] = start[l] + list_len[l]; len32[l] = (int32_t)list_len[l]; }
     DPH_CUDA(cudaStreamSynchronize(ix->stream));
-    DPH_CUDA(cudaMemcpy(ix->list_len, len32.data(), nlist * 4, cudaMemcpyHostToDevice));
-    DPH_CUDA(cudaMemcpy(ix->list_start, start.data(), (nlist + 1) * 8, cudaMemcpyHostToDevice));
-    ix->h_list_len.assign(list_len, list_len + nlist);
-    ix->h_list_start = start;
-    ix->ntotal = start[nlist];
-    return 0;
+    return dph_commit_layout(ix, std::move(L));
 }
 
 DPH_API int dph_index_last_remove_ms(const dph_index* ix, float* ms_out) {

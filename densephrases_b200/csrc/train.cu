@@ -329,7 +329,6 @@ static int commit_table(dph_index* ix, float** dst, float* src, size_t count, De
         DPH_CUDA(cudaStreamSynchronize(ix->stream));
     } else {
         *dst = src; tmp.release(src);
-        ix->bytes += (int64_t)(std::max<size_t>(count, 1) * 4);
     }
     return 0;
 }

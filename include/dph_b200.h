@@ -155,6 +155,7 @@ int dph_index_set_scan_mode(dph_index* ix, int mode);
  * 1 (default): used when the shape allows (lists % 128 == 0, batch >= 32, nprobe + margin <= 1024); 0: always the exact SIMT GEMM. */
 int dph_index_set_coarse_tc(dph_index* ix, int on);
 int dph_index_get_opq(const dph_index* ix, float* A_out, int mem);
+/* Bytes of the index's resident arrays (model tables, lists, labels, direct map), without the per-batch workspace. */
 int64_t dph_index_device_bytes(const dph_index* ix);
 /* Measurement hook: when on, CUDA events bracket the scan kernel of each search (last chunk); last_scan_ms waits
  * for it and returns the kernel's duration in milliseconds (bench.py roofline). */
