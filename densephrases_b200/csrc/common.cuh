@@ -125,7 +125,7 @@ struct __align__(16) DphSeg {
 struct DphWork {       // device scalars written by the plan kernel
     long long total_blocks;
 };
-struct DphPairWork {   // pair mode: the work queue of (list, block segment, item) units the scan CTAs pull from
+struct DphGroupWork {  // grouped modes (pair, quad): the work queue of (list, block segment, item) units the scan CTAs pull from
     long long total_blocks;         // sum over items of the list's blocks
     long long per;                  // blocks per segment (a list longer than this is cut into several units per item)
     int total_units;
@@ -145,5 +145,5 @@ struct __align__(16) DphUnit {
     float base[DPH_QUAD_ITEM_Q];    // <xr, centroid> + the query's quantisation offset
     float step[DPH_QUAD_ITEM_Q];    // the query's quantisation step
 };
-#define DPH_PAIR_SEG_MIN 128        // shortest segment worth rebuilding the packed 192 KB LUT for
-#define DPH_PAIR_UNITS_PER_CTA 16   // lists are cut only when the batch has fewer than this many whole-list units per CTA
+#define DPH_GROUP_SEG_MIN 128       // shortest segment worth rebuilding the packed 192 KB LUT for
+#define DPH_GROUP_UNITS_PER_CTA 16  // lists are cut only when the batch has fewer than this many whole-list units per CTA

@@ -1,4 +1,4 @@
-// index.cu -- the dph_index handle: construction, the model tables, getters, search orchestration, reconstruct (lists: lists.cu).
+// index.cu -- the dph_index handle: construction, the model tables, getters, reconstruct (lists: lists.cu, search: search.cu).
 // C ABI declared in include/dph_b200.h (each entry point cites the reference call it replaces).
 #include "index_internal.cuh"
 #include <algorithm>
@@ -24,7 +24,6 @@ int DevBuf::ensure(size_t bytes) {
     cap = want;
     return 0;
 }
-void DevBuf::release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 
 // -------------------------------------------------------------------------------------------------
 // generators (bit-identical to oracle/ivfpq_ref.c)
@@ -58,15 +57,9 @@ DPH_API void dph_index_free(dph_index* ix) {
     cudaSetDevice(ix->device);
     for (void* p : {ix->A, ix->C, ix->pq}) if (p) cudaFree(p);
     dph_free_lists(ix);
-    DevBuf* bufs[] = {&ix->xdev, &ix->xr, &ix->S, &ix->key, &ix->cd, &ix->lut_canon, &ix->lutmax, &ix->segs, &ix->wpre, &ix->qinfo,
-                      &ix->cand, &ix->cand_off, &ix->cand_cnt, &ix->gthr, &ix->flags, &ix->work, &ix->Dp, &ix->Ip, &ix->Gp, &ix->Dh, &ix->Ih, &ix->eps, &ix->nseg, &ix->lutmin, &ix->lutmaxv, &ix->lutq, &ix->qparams, &ix->gdense,
-                      &ix->pl_cnt, &ix->pl_fill, &ix->pl_off, &ix->pl_blockpre, &ix->pl_entries, &ix->pl_unitpre, &ix->pl_units, &ix->pl_udesc, &ix->pairwork, &ix->csplit, &ix->xsplit, &ix->candkeys, &ix->cflags, &ix->selkeys, &ix->recbuf,
-                      &ix->rb_ids, &ix->rb_out, &ix->rb_found, &ix->ws_q, &ix->ws_id, &ix->ws_out, &ix->ws_xq, &ix->enc_key, &ix->enc_cd,
-                      &ix->enc_list, &ix->enc_codes};
-    for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < DPH_PROF_RING; i++) { if (ix->ev0[i]) cudaEventDestroy(ix->ev0[i]); if (ix->ev1[i]) cudaEventDestroy(ix->ev1[i]); }
     for (cudaEvent_t e : ix->aev) if (e) cudaEventDestroy(e);
-    delete ix;
+    delete ix;                                      // the workspace DevBufs free themselves, on the device set above
 }
 DPH_API int dph_index_set_stream(dph_index* ix, void* s) { ix->stream = (cudaStream_t)s; return 0; }
 
@@ -159,7 +152,7 @@ DPH_API int dph_index_profile_scan_ms(dph_index* ix, float* ms_out, int max_out)
         DPH_CUDA(cudaEventSynchronize(ix->ev1[i]));
         DPH_CUDA(cudaEventElapsedTime(ms_out + j, ix->ev0[i], ix->ev1[i]));
     }
-    return n < 0 ? 0 : 0 * n;
+    return 0;
 }
 DPH_API int dph_index_profile_count(const dph_index* ix) { return (int)std::min<int64_t>(ix->prof_n, DPH_PROF_RING); }
 DPH_API int64_t dph_index_device_bytes(const dph_index* ix) {
@@ -189,229 +182,9 @@ DPH_API int dph_index_copy_last(dph_index* ix, int which, void* dst_host, int64_
     return 0;
 }
 
-// -------------------------------------------------------------------------------------------------
-// search
-// -------------------------------------------------------------------------------------------------
-// stage: 0 = whole search; 1 = only rotation + this shard's coarse candidates (keys64 out); 2 = everything after the coarse
-// quantizer, probes (key, cd) already in ix->key / ix->cd and rotated queries in ix->xr (sharded coarse quantizer, see sharded.py);
-// 3 = only rotation + the coarse quantizer over ALL lists (query-split sharded search: this rank's slice of the batch)
-static int search_chunk(dph_index* ix, const float* x_dev, int64_t n, int k, float* D, int64_t* I, uint32_t* G, int stage = 0,
-                        unsigned long long* keys64 = nullptr) {
-    cudaStream_t st = ix->stream;
-    const int nprobe = ix->nprobe;
-    const int grid = ix->num_sms;
-    // candidates kept per CTA: k + slack.  The proof needs T_k - (k+slack)-th score > 2 eps; the pair filter's eps is dominated by
-    // the 10-bit quantisation, so its slack grows with k (order statistics: the gap between ranks k and 1.5k is ~0.1 sigma).
-    const int keep_single = k + DPH_KEEP_SLACK;
-    const int keep_pair = k + (k / 2 > DPH_KEEP_SLACK ? k / 2 : DPH_KEEP_SLACK);
-    // quad filter: 8-bit entries, eps ~2.7x the pair filter's: 2 eps ~ 0.26 sigma of the scores.  The drop threshold is some unit's
-    // keep-th best, i.e. at global rank >= keep; the proof needs score(rank k) - score(rank keep) > 2 eps.  Order statistics of the
-    // top of ~6 M scores: rank 10 -> rank 110 is ~0.5 sigma, which leaves a 2x margin (7-bit entries would need keep ~ 400).
-    const int keep_quad = k + (2 * k > 100 ? 2 * k : 100);
-    const int keep_max = keep_quad > keep_pair ? keep_quad : keep_pair;
-    DPH_TRY(ix->xr.ensure((size_t)n * ix->d * 4));
-    DPH_TRY(ix->S.ensure((size_t)n * ix->nlist * 4));
-    DPH_TRY(ix->key.ensure((size_t)n * nprobe * 4));
-    DPH_TRY(ix->cd.ensure((size_t)n * nprobe * 4));
-    DPH_TRY(ix->lut_canon.ensure((size_t)n * DPH_LUT_CANON_FLOATS * 4));
-    DPH_TRY(ix->lutmax.ensure((size_t)n * DPH_M * 4));
-    DPH_TRY(ix->segs.ensure((size_t)n * nprobe * sizeof(DphSeg)));
-    DPH_TRY(ix->wpre.ensure((size_t)(n + 1) * 8));
-    DPH_TRY(ix->qinfo.ensure((size_t)n * 4));
-    DPH_TRY(ix->eps.ensure((size_t)n * 4));
-    DPH_TRY(ix->nseg.ensure((size_t)n * 4));
-    // sharing gathers between the queries that probe a list pays when lists are probed by >= ~1.5 queries of the batch on average
-    const int64_t eff_probe = std::min<int64_t>(nprobe, ix->nlist);
-    // ... and when lists are long enough to amortise rebuilding the packed 192 KB LUT at every (list, query group) item
-    const int64_t nl_local = std::max<int64_t>(ix->list_hi - ix->list_lo, 1);
-    const bool long_lists = ix->ntotal_local / nl_local >= 4096;
-    const bool shared = long_lists && n * eff_probe * 2 >= ix->nlist * 3;
-    int group = 1;                                  // queries per gather: 1, 2 (pair-packed) or 4 (quad-packed)
-    if (ix->scan_mode == DPH_SCAN_PAIR) group = 2;
-    else if (ix->scan_mode == DPH_SCAN_QUAD) group = 4;
-    else if (ix->scan_mode == DPH_SCAN_FAST && shared) group = 4;
-    if (group == 4 && keep_quad > DPH_QUAD_KEEP_MAX) group = 2;
-    if (group == 2 && keep_pair > 1536 - DPH_SCAN_THREADS) group = 1;
-    const bool pair = group > 1;
-    const int keep_fast = group == 4 ? keep_quad : (group == 2 ? keep_pair : keep_single);
-    // group modes: query q's region holds nseg_q + blocks_q / per + 1 units of keep (plan_scan_kernel); summed over the batch,
-    // sum_q blocks_q <= (queries per item) * sum over items of blocks <= (queries per item) * per * UNITS_PER_CTA * grid
-    const size_t item_q = group == 4 ? DPH_QUAD_ITEM_Q : 2;
-    DPH_TRY(ix->cand.ensure(((size_t)(2 * grid + 2 * n + 2) + (pair ? (size_t)(n * nprobe + item_q * DPH_PAIR_UNITS_PER_CTA * grid + 2 * n + 16) : 0)) * keep_max * 8));
-    DPH_TRY(ix->cand_off.ensure((size_t)(n + 1) * 8));
-    DPH_TRY(ix->cand_cnt.ensure((size_t)n * 4));
-    DPH_TRY(ix->gthr.ensure((size_t)n * 4));
-    DPH_TRY(ix->flags.ensure((size_t)n * 4));
-    DPH_TRY(ix->work.ensure(sizeof(DphWork)));
-    DPH_TRY(ix->lutmin.ensure((size_t)n * DPH_M * 4));
-    DPH_TRY(ix->lutmaxv.ensure((size_t)n * DPH_M * 4));
-    if (pair) {
-        DPH_TRY(ix->lutq.ensure((size_t)n * (group == 4 ? DPH_LUTQ8_BYTES : DPH_LUT_SCAN_FLOATS * 2)));
-        DPH_TRY(ix->qparams.ensure((size_t)n * 8));
-        DPH_TRY(ix->gdense.ensure((size_t)n * nprobe * 4));
-        DPH_TRY(ix->pl_cnt.ensure((size_t)ix->nlist * 4));
-        DPH_TRY(ix->pl_fill.ensure((size_t)ix->nlist * 4));
-        DPH_TRY(ix->pl_off.ensure((size_t)(ix->nlist + 1) * 4));
-        DPH_TRY(ix->pl_blockpre.ensure((size_t)(ix->nlist + 1) * 8));
-        DPH_TRY(ix->pl_entries.ensure((size_t)n * nprobe * 4));
-        DPH_TRY(ix->pl_unitpre.ensure((size_t)(ix->nlist + 1) * 4));
-        // units <= sum_l items_l * (blocks_l / seg + 1) <= total_blocks / seg + items <= UNITS_PER_CTA * grid + n * nprobe
-        DPH_TRY(ix->pl_units.ensure((size_t)(n * nprobe + DPH_PAIR_UNITS_PER_CTA * grid + 16) * 8));
-        if (group == 4) DPH_TRY(ix->pl_udesc.ensure((size_t)(n * nprobe + DPH_PAIR_UNITS_PER_CTA * grid + 16) * sizeof(DphUnit)));
-        DPH_TRY(ix->pairwork.ensure(sizeof(DphPairWork)));
-    }
-    ix->last_n = n;
-    if (stage != 1 && stage != 3) ix->last_group = group;
-    if (stage == 1) ix->last_coarse_n = n;
-
-    if (stage == 1) {
-        const int64_t nl = ix->list_hi - ix->list_lo;
-        DPH_TRY(dph_launch_sgemm_nt_seq(x_dev, n, ix->A, ix->d, ix->d, ix->xr.as<float>(), st));                   // OPQ rotation
-        if (ix->coarse_tc) {
-            int rc = dph_coarse_tc(ix, n, ix->list_lo, nl, nprobe, keys64, nullptr, nullptr, st);
-            if (rc == 0) return 0;
-            if (rc != 1) return rc;
-        }
-        DPH_TRY(dph_launch_sgemm_nt_seq(ix->xr.as<float>(), n, ix->C + ix->list_lo * ix->d, nl, ix->d, ix->S.as<float>(), st));   // this shard's centroids only
-        DPH_TRY(dph_launch_coarse_select(ix->S.as<float>(), n, nl, nprobe, nullptr, nullptr, st, keys64, (unsigned)ix->list_lo));
-        return 0;
-    }
-    if (stage == 0 || stage == 3) {
-        DPH_TRY(dph_launch_sgemm_nt_seq(x_dev, n, ix->A, ix->d, ix->d, ix->xr.as<float>(), st));                   // OPQ rotation
-        int rc = ix->coarse_tc ? dph_coarse_tc(ix, n, 0, ix->nlist, nprobe, nullptr, ix->key.as<int32_t>(), ix->cd.as<float>(), st) : 1;
-        if (rc > 1) return rc;
-        if (rc == 1) {
-            DPH_TRY(dph_launch_sgemm_nt_seq(ix->xr.as<float>(), n, ix->C, ix->nlist, ix->d, ix->S.as<float>(), st));   // coarse scores
-            DPH_TRY(dph_launch_coarse_select(ix->S.as<float>(), n, ix->nlist, nprobe, ix->key.as<int32_t>(), ix->cd.as<float>(), st, nullptr, 0u, nullptr, 0,
-                                             &ix->selkeys));
-        }
-        if (stage == 3) return 0;
-    }
-    DPH_TRY(dph_launch_lut(ix->xr.as<float>(), n, ix->pq, ix->lut_canon.as<float>(), ix->lutmax.as<float>(),
-                           ix->lutmin.as<float>(), ix->lutmaxv.as<float>(), pair ? ix->lutq.p : nullptr,
-                           pair ? ix->qparams.as<float2>() : nullptr, st, group));
-    if (ix->scan_mode != DPH_SCAN_EXACT) {
-        DPH_TRY(dph_launch_plan(ix, n, k, keep_fast, grid, nullptr, st, group));
-        if (ix->profile) DPH_CUDA(cudaEventRecord(ix->ev0[ix->prof_n % DPH_PROF_RING], st));
-        if (pair) DPH_TRY(dph_launch_scan_pair(ix, n, keep_fast, grid, st, group));
-        else DPH_TRY(dph_launch_scan(ix, n, k, keep_fast, DPH_SCAN_FAST, grid, st));
-        if (ix->profile) { DPH_CUDA(cudaEventRecord(ix->ev1[ix->prof_n % DPH_PROF_RING], st)); ix->prof_n++; }
-        DPH_TRY(dph_launch_merge(ix, n, k, DPH_SCAN_FAST, nullptr, D, I, G, st));
-        // fallback for queries whose filter could not be proven exact (no-op launches when no flag is set)
-        DPH_TRY(dph_launch_plan(ix, n, k, k, grid, ix->flags.as<int32_t>(), st, 1));
-        DPH_TRY(dph_launch_scan(ix, n, k, k, DPH_SCAN_EXACT, grid, st));
-        DPH_TRY(dph_launch_merge(ix, n, k, DPH_SCAN_EXACT, ix->flags.as<int32_t>(), D, I, G, st));
-    } else {
-        DPH_CUDA(cudaMemsetAsync(ix->flags.p, 0, (size_t)n * 4, st));
-        DPH_TRY(dph_launch_plan(ix, n, k, k, grid, nullptr, st, 1));
-        if (ix->profile) DPH_CUDA(cudaEventRecord(ix->ev0[ix->prof_n % DPH_PROF_RING], st));
-        DPH_TRY(dph_launch_scan(ix, n, k, k, DPH_SCAN_EXACT, grid, st));
-        if (ix->profile) { DPH_CUDA(cudaEventRecord(ix->ev1[ix->prof_n % DPH_PROF_RING], st)); ix->prof_n++; }
-        DPH_TRY(dph_launch_merge(ix, n, k, DPH_SCAN_EXACT, nullptr, D, I, G, st));
-    }
-    return 0;
-}
-
 int check_ready(dph_index* ix, int k) {
     DPH_CHECK(ix && ix->A && ix->C && ix->pq && ix->list_len, "index is not fully constructed (opq/centroids/pq/lists)");
     DPH_CHECK(k >= 1 && k <= DPH_MAX_K, "k must be in [1,1024]");
-    return 0;
-}
-static int64_t chunk_size(const dph_index* ix, int64_t n) {
-    int64_t c = (1ll << 28) / std::max<int64_t>(ix->nlist, 1);   // S chunk <= 1 GiB
-    c = std::max<int64_t>(1, std::min<int64_t>(c, 4096));
-    return std::min(c, n);
-}
-
-DPH_API int dph_index_search_partial(dph_index* ix, const float* x_dev, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
-    DPH_TRY(check_ready(ix, k));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    const int64_t cs = chunk_size(ix, n);
-    for (int64_t o = 0; o < n; o += cs) {
-        int64_t m = std::min(cs, n - o);
-        DPH_TRY(search_chunk(ix, x_dev + o * ix->d, m, k, D + o * k, I + o * k, G + o * k));
-    }
-    return 0;
-}
-
-// ---- sharded coarse quantizer (every rank scores only its own lists' centroids; SURVEY.md 8e "Partitioning") ----
-DPH_API int dph_index_coarse_local(dph_index* ix, const float* x_dev, int64_t n, uint64_t* keys_dev) {
-    DPH_TRY(check_ready(ix, 1));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    DPH_CHECK(n <= chunk_size(ix, n), "coarse_local: batch too large for one chunk");
-    return search_chunk(ix, x_dev, n, 1, nullptr, nullptr, nullptr, 1, (unsigned long long*)keys_dev);
-}
-DPH_API int dph_index_search_preassigned(dph_index* ix, const uint64_t* keys_gathered_dev, int nshards, int64_t n, int k, float* D_dev,
-                                         int64_t* I_dev, uint32_t* G_dev) {
-    DPH_TRY(check_ready(ix, k));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    DPH_CHECK(n == ix->last_coarse_n, "search_preassigned must follow coarse_local with the same batch");
-    DPH_TRY(ix->key.ensure((size_t)n * ix->nprobe * 4));
-    DPH_TRY(ix->cd.ensure((size_t)n * ix->nprobe * 4));
-    DPH_TRY(dph_launch_coarse_merge((const unsigned long long*)keys_gathered_dev, nshards, n, ix->nprobe, ix->key.as<int32_t>(), ix->cd.as<float>(),
-                                    ix->stream));
-    return search_chunk(ix, nullptr, n, k, D_dev, I_dev, G_dev, 2, nullptr);
-}
-
-// ---- query-split sharded search (sharded.py): every rank rotates and assigns ITS SLICE of the batch over ALL lists, the ranks
-// exchange one record per query -- [768 f32 rotated query | nprobe i32 lists | nprobe f32 coarse scores] -- and then scan their own
-// lists.  Against the list-split coarse quantizer above it removes the replicated rotation and exact re-rank (each done for n / W
-// queries instead of n) and the merge of per-shard candidates; it needs the full centroid table on every rank (it is replicated).
-__global__ void pack_records_kernel(const float* __restrict__ xr, const int* __restrict__ key, const float* __restrict__ cd, int nprobe, float* __restrict__ rec) {
-    const long long q = blockIdx.x;
-    const int R = DPH_D + 2 * nprobe;
-    float* o = rec + q * R;
-    for (int t = threadIdx.x; t < R; t += blockDim.x)
-        o[t] = t < DPH_D ? xr[q * DPH_D + t] : (t < DPH_D + nprobe ? __int_as_float(key[q * nprobe + t - DPH_D]) : cd[q * nprobe + t - DPH_D - nprobe]);
-}
-__global__ void unpack_records_kernel(const float* __restrict__ rec, int nprobe, float* __restrict__ xr, int* __restrict__ key, float* __restrict__ cd) {
-    const long long q = blockIdx.x;
-    const int R = DPH_D + 2 * nprobe;
-    const float* r = rec + q * R;
-    for (int t = threadIdx.x; t < R; t += blockDim.x) {
-        const float v = r[t];
-        if (t < DPH_D) xr[q * DPH_D + t] = v;
-        else if (t < DPH_D + nprobe) key[q * nprobe + t - DPH_D] = __float_as_int(v);
-        else cd[q * nprobe + t - DPH_D - nprobe] = v;
-    }
-}
-DPH_API int dph_index_record_floats(const dph_index* ix) { return ix->d + 2 * ix->nprobe; }
-DPH_API int dph_index_coarse_split(dph_index* ix, const float* x_dev, int64_t n_local, float* rec_dev) {
-    DPH_TRY(check_ready(ix, 1));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    if (n_local == 0) return 0;
-    DPH_CHECK(n_local <= chunk_size(ix, n_local), "coarse_split: slice too large for one chunk");
-    DPH_TRY(search_chunk(ix, x_dev, n_local, 1, nullptr, nullptr, nullptr, 3, nullptr));
-    pack_records_kernel<<<(unsigned)n_local, 256, 0, ix->stream>>>(ix->xr.as<float>(), ix->key.as<int>(), ix->cd.as<float>(), ix->nprobe, rec_dev);
-    DPH_CUDA(cudaGetLastError());
-    return 0;
-}
-DPH_API int dph_index_search_assigned(dph_index* ix, const float* rec_dev, int64_t n, int k, float* D_dev, int64_t* I_dev, uint32_t* G_dev) {
-    DPH_TRY(check_ready(ix, k));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    if (n == 0) return 0;
-    DPH_TRY(ix->xr.ensure((size_t)n * ix->d * 4));
-    DPH_TRY(ix->key.ensure((size_t)n * ix->nprobe * 4));
-    DPH_TRY(ix->cd.ensure((size_t)n * ix->nprobe * 4));
-    unpack_records_kernel<<<(unsigned)n, 256, 0, ix->stream>>>(rec_dev, ix->nprobe, ix->xr.as<float>(), ix->key.as<int>(), ix->cd.as<float>());
-    DPH_CUDA(cudaGetLastError());
-    return search_chunk(ix, nullptr, n, k, D_dev, I_dev, G_dev, 2, nullptr);
-}
-
-DPH_API int dph_index_search(dph_index* ix, const float* x, int64_t n, int k, float* D, int64_t* I, int mem) {
-    DPH_TRY(check_ready(ix, k));
-    DPH_CUDA(cudaSetDevice(ix->device));
-    if (n == 0) return 0;
-    DPH_TRY(ix->Gp.ensure((size_t)n * k * 4));
-    if (mem == DPH_MEM_DEVICE) return dph_index_search_partial(ix, x, n, k, D, I, ix->Gp.as<uint32_t>());
-    DPH_TRY(ix->xdev.ensure((size_t)n * ix->d * 4));
-    DPH_TRY(ix->Dp.ensure((size_t)n * k * 4));
-    DPH_TRY(ix->Ip.ensure((size_t)n * k * 8));
-    DPH_CUDA(cudaMemcpyAsync(ix->xdev.p, x, (size_t)n * ix->d * 4, cudaMemcpyHostToDevice, ix->stream));
-    DPH_TRY(dph_index_search_partial(ix, ix->xdev.as<float>(), n, k, ix->Dp.as<float>(), ix->Ip.as<int64_t>(), ix->Gp.as<uint32_t>()));
-    DPH_CUDA(cudaMemcpyAsync(D, ix->Dp.p, (size_t)n * k * 4, cudaMemcpyDeviceToHost, ix->stream));
-    DPH_CUDA(cudaMemcpyAsync(I, ix->Ip.p, (size_t)n * k * 8, cudaMemcpyDeviceToHost, ix->stream));
-    DPH_CUDA(cudaStreamSynchronize(ix->stream));
     return 0;
 }
 

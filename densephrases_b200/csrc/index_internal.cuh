@@ -1,4 +1,4 @@
-// index_internal.cuh -- the dph_index handle and the internal kernel-launch prototypes.
+// index_internal.cuh -- the dph_index handle, the search plan and the internal kernel-launch prototypes.
 #pragma once
 #include "common.cuh"
 #include "../../include/dph_b200.h"
@@ -8,8 +8,8 @@
 
 #define DPH_SCAN_THREADS 512
 #define DPH_SCAN_WARPS (DPH_SCAN_THREADS / 32)
-#define DPH_CAND_CAP 3072          // shared-memory candidate buffer (u64 keys) per scan CTA
-#define DPH_PAIR_CAP 1280          // pair mode: one buffer per query of the pair
+#define DPH_CAND_CAP 3072          // one-query scan: shared-memory candidate buffer (u64 keys) per CTA; holds every k's keep (scan.cu)
+#define DPH_PAIR_KEEP_MAX 1024      // pair mode: PCAP (1536) - pair scan threads (512), see scan.cu
 #define DPH_QUAD_KEEP_MAX 256       // quad mode: QCAP (512) - quad scan threads (256), see scan.cu
 
 #define DPH_KEEP_SLACK 32          // fast mode keeps k + slack candidates per CTA
@@ -28,11 +28,14 @@
 #define DPH_SEG_SMEM 256            // segment descriptors of one query kept in shared memory by the scan kernel
 #define DPH_L2_PREFETCH_ROUNDS 2    // scan kernels: bulk L2 prefetch distance, in rounds (one 3 KB block per warp per round; tools/scan_floor.cu)
 
-struct DevBuf {            // grow-only device buffer
+struct DevBuf {            // grow-only device buffer; freed with its owner, on the owner's device (which must be current)
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     int ensure(size_t bytes);
-    void release();
     template <class T> T* as() const { return (T*)p; }
 };
 
@@ -82,14 +85,14 @@ struct dph_index {
 
     // per-batch workspace
     DevBuf xdev, xr, S, key, cd, lut_canon, lutmax, segs, wpre, qinfo, cand, cand_off, cand_cnt, gthr, flags,
-        work, Dp, Ip, Gp, Dh, Ih, eps, nseg,
-        lutmin, lutmaxv, lutq, qparams, gdense, pl_cnt, pl_fill, pl_off, pl_blockpre, pl_entries, pl_unitpre, pl_units, pl_udesc, pairwork,
-        csplit, xsplit, candkeys, cflags, selkeys, recbuf,
+        work, Dp, Ip, Gp, eps, nseg,
+        lutmin, lutmaxv, lutq, qparams, gdense,
+        grp_cnt, grp_fill, grp_off, grp_blockpre, grp_entries, grp_unitpre, grp_units, grp_udesc, groupwork,   // grouped plan (prep.cu)
+        csplit, xsplit, candkeys, cflags, selkeys,
         rb_ids, rb_out, rb_found, ws_q, ws_id, ws_out, ws_xq,        // reconstruct_batch / window_scores staging (host-buffer calls)
         enc_key, enc_cd, enc_list, enc_codes;                        // encode / add: top-1 coarse result, host-call output staging
     int64_t csplit_lo = -1, csplit_nl = -1;
     int coarse_tc = 1;                 // tensor-core coarse quantizer with exact re-rank (0: always the SIMT sequential-k GEMM)
-    int64_t last_n = 0;
     int last_group = 1;                // queries per gather used by the last search (1, 2 or 4)
     int64_t last_coarse_n = -1;
     bool profile = false;              // CUDA events around the scan kernel of the last search chunk
@@ -167,6 +170,20 @@ __global__ void relayout_ids_kernel(long long* dst, long long blk0, const long l
                                     long long lo, long long hi, const long long* ids_old, const long long* list_start_old,
                                     const long long* lrs_old, long long* dm_ids, long long* dm_rows);
 
+// What the scan stage of one batch runs (search.cu).  The FAST pass keeps `keep` candidates per scan CTA and query and its merge
+// flags the queries it cannot prove exact; the EXACT pass (scan_kernel<EXACT>, keep = k) re-runs those, or runs alone in EXACT mode.
+struct DphSearchPlan {
+    int k;
+    bool exact_only;    // EXACT scan mode: no fast pass, the exact pass scans every query
+    int group;          // fast pass: queries per gather -- 1 (fp32 LUT), 2 (pair-packed u16 LUTs) or 4 (quad-packed u8 LUTs)
+    int keep;           // fast pass: candidates kept per scan CTA and query
+    int item_q;         // fast pass: queries per work item -- 2 (pair), DPH_QUAD_ITEM_Q (quad), 1 (one query: no items)
+    int grid;           // scan CTAs: one persistent CTA per SM
+    bool grouped() const { return group > 1; }
+    int pass_group(bool exact) const { return exact ? 1 : group; }
+    int pass_keep(bool exact) const { return exact ? k : keep; }
+};
+
 // process-wide variant selection (dph_set_tuning, measurement hook): [0] quad-scan IMAD level, [1] SGEMM tile
 extern int g_dph_tune[8];
 // ---- prep.cu ----
@@ -180,14 +197,13 @@ int dph_launch_coarse_merge(const unsigned long long* keys, int W, int64_t n, in
                             unsigned long long* keys64 = nullptr);
 int dph_launch_lut(const float* xr, int64_t n, const float* pq, float* lut_canon, float* lutmax, float* lutmin, float* lutmaxv,
                    void* lutq, float2* qparams, cudaStream_t st, int group);
-// group: queries per gather of the scan -- 1 (fp32 LUT, one query), 2 (pair-packed u16 LUTs), 4 (quad-packed u8 LUTs)
-int dph_launch_plan(dph_index* ix, int64_t n, int k, int keep, int grid, const int32_t* only_flagged, cudaStream_t st, int group);
-int dph_launch_scan_pair(dph_index* ix, int64_t n, int keep, int grid, cudaStream_t st, int group);
+// One pass of plan p (only_flagged, nullable: only the queries whose flag is set): segments, work, candidate areas, eps, group queue.
+int dph_launch_plan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, const int32_t* only_flagged, cudaStream_t st);
 // ---- scan.cu ----
-int dph_launch_scan(dph_index* ix, int64_t n, int k, int keep, int mode, int grid, cudaStream_t st);
+// One pass: scan_kernel<EXACT> (exact), else by p.group scan_kernel<FAST>, scan_pair_kernel or scan_quad_kernel<IMADL>.
+int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, cudaStream_t st);
 int dph_launch_merge(dph_index* ix, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,
                      uint32_t* G, cudaStream_t st);
-int dph_scan_setup_attrs();
 // ---- encode.cu ----
 int64_t dph_encode_chunk(const dph_index* ix);
 int dph_encode_rows(dph_index* ix, const float* x_dev, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad);

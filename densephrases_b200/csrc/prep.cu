@@ -691,8 +691,8 @@ struct PlanArgs {
     const int* only_flagged;       // nullable: plan work only for queries with flag != 0
     const float* lutmax;
     DphSeg* segs; unsigned* qblocks; int* nseg; float* eps;
-    unsigned* gdense;              // nullable: canonical scan position of every (query, probe), dense [n, nprobe] (pair mode)
-    const float2* qparams;         // nullable: quantisation (step, base) -> the pair filter's extra error term
+    unsigned* gdense;              // nullable: canonical scan position of every (query, probe), dense [n, nprobe] (grouped modes)
+    const float2* qparams;         // nullable: quantisation (step, base) -> the grouped filter's extra error term
 };
 // One warp per query.  Writes the COMPACTED list of in-shard, non-empty segments (probe-rank order) to
 // segs[q][0..nseg[q]); gstart stays the canonical scan position over ALL probed lists (tie-break key across shards).
@@ -752,7 +752,7 @@ __global__ void __launch_bounds__(256) plan_segs_kernel(PlanArgs a) {
         // inflated by 1.01 for the fp32 evaluation of the bound itself.
         const float gamma96 = 5.7221e-6f;
         float e = 2.0f * gamma96 * (dmax + lsum) * 1.01f;
-        // pair mode: every quantised entry is within 0.5 step of the fp32 entry (+ rounding of the dequantisation) -> 96 * 0.502 * step
+        // grouped modes: every quantised entry is within 0.5 step of the fp32 entry (+ rounding of the dequantisation) -> 96 * 0.502 * step
         if (a.qparams) e += 96.0f * 0.502f * a.qparams[q].x + 8e-6f * (dmax + lsum);
         a.eps[q] = e;
     }
@@ -761,7 +761,7 @@ __global__ void __launch_bounds__(256) plan_segs_kernel(PlanArgs a) {
 struct PlanScanArgs {
     const unsigned* qblocks; long long n; int keep; int grid;
     long long* qpre; long long* cand_off; int* cand_cnt; unsigned* gthr; DphWork* work;
-    const DphPairWork* pairwork; const int* nseg;     // pair mode (nullable): a query is flushed once per (list, segment) unit it is part of
+    const DphGroupWork* groupwork; const int* nseg;   // grouped modes (nullable): a query is flushed once per (list, segment) unit it is part of
 };
 __global__ void __launch_bounds__(1024) plan_scan_kernel(PlanScanArgs a) {
     __shared__ long long wsum[32];
@@ -792,9 +792,10 @@ __global__ void __launch_bounds__(1024) plan_scan_kernel(PlanScanArgs a) {
     }
     if (tid == 0) { total = carry; a.qpre[a.n] = carry; a.work->total_blocks = carry; carry = 0; }
     __syncthreads();
-    // pass 2: candidate-region offsets; a query spanning `parts` scan CTAs may receive parts*keep entries
+    // pass 2: candidate-region offsets; a query spanning `parts` scan CTAs or units may receive parts*keep entries.  The area these
+    // regions share is sized by the bound on the batch's sum of parts derived at search.cu: cand_entries.
     const long long T = total;
-    const long long per = a.pairwork ? a.pairwork->per : (T / a.grid > 0 ? T / a.grid : 1);
+    const long long per = a.groupwork ? a.groupwork->per : (T / a.grid > 0 ? T / a.grid : 1);
     for (long long base = 0; base < a.n; base += 1024) {
         long long q = base + tid;
         long long v = 0;
@@ -802,7 +803,7 @@ __global__ void __launch_bounds__(1024) plan_scan_kernel(PlanScanArgs a) {
             long long qb = (long long)a.qblocks[q];
             if (qb > 0) {
                 long long parts = qb / per + 2;
-                if (a.pairwork) parts = (long long)a.nseg[q] + qb / per + 1;        // sum over its lists of ceil(blocks / segment)
+                if (a.groupwork) parts = (long long)a.nseg[q] + qb / per + 1;        // sum over its lists of ceil(blocks / segment)
                 else if (parts > a.grid) parts = a.grid;
                 v = parts * a.keep;
             }
@@ -829,26 +830,26 @@ __global__ void __launch_bounds__(1024) plan_scan_kernel(PlanScanArgs a) {
 }
 
 // =================================================================================================
-// pair plan: invert (query -> probed lists) into (list -> probing queries), pair the probes of each list two by two into
-// work items, and emit the work queue of the pair-packed scan kernel: units (list, block segment, item), items of the same
-// list segment ADJACENT in the queue.  The scan CTAs pull units in queue order, so the items of a list are scanned at the
+// group plan (pair and quad modes): invert (query -> probed lists) into (list -> probing queries), group the probes of each list
+// into work items of gsz queries, and emit the work queue of the grouped scan kernels: units (list, block segment, item), items of
+// the same list segment ADJACENT in the queue.  The scan CTAs pull units in queue order, so the items of a list are scanned at the
 // same time by different CTAs and all but the first reader of a code block hit L2 instead of HBM.
 // =================================================================================================
-struct PairPlanArgs {
+struct GroupPlanArgs {
     const int* key; long long nq_probes; int nprobe; const int* list_len; long long list_lo, list_hi, nlist; int grid;
-    int* cnt; int* fill; int* off; long long* blockpre; unsigned* entries; DphPairWork* work;
+    int* cnt; int* fill; int* off; long long* blockpre; unsigned* entries; DphGroupWork* work;
     int* unitpre; unsigned long long* units;
     int gsz;                       // queries per work item: 2 (pair-packed scan) or DPH_QUAD_ITEM_Q (quad-packed scan)
     DphUnit* udesc;                // quad mode (nullable): resolved unit descriptors, parallel to `units`
     const long long* blk_off; const float* cd; const unsigned* gdense; const float2* qparams;
 };
-__global__ void pair_count_kernel(PairPlanArgs a) {
+__global__ void group_count_kernel(GroupPlanArgs a) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.nq_probes) return;
     const int l = a.key[i];
     if (l >= a.list_lo && l < a.list_hi && a.list_len[l] > 0) atomicAdd(&a.cnt[l], 1);
 }
-__global__ void __launch_bounds__(1024) pair_scan_kernel(PairPlanArgs a) {
+__global__ void __launch_bounds__(1024) group_scan_kernel(GroupPlanArgs a) {
     __shared__ long long wsa[32], wsb[32];
     __shared__ long long ca, cb;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -889,8 +890,8 @@ __global__ void __launch_bounds__(1024) pair_scan_kernel(PairPlanArgs a) {
     __shared__ long long segb_s;
     if (tid == 0) {
         a.off[a.list_hi] = (int)ca; a.blockpre[a.list_hi] = cb;
-        long long segb = (cb + (long long)a.grid * DPH_PAIR_UNITS_PER_CTA - 1) / ((long long)a.grid * DPH_PAIR_UNITS_PER_CTA);
-        if (segb < DPH_PAIR_SEG_MIN) segb = DPH_PAIR_SEG_MIN;
+        long long segb = (cb + (long long)a.grid * DPH_GROUP_UNITS_PER_CTA - 1) / ((long long)a.grid * DPH_GROUP_UNITS_PER_CTA);
+        if (segb < DPH_GROUP_SEG_MIN) segb = DPH_GROUP_SEG_MIN;
         a.work->total_blocks = cb;
         a.work->per = segb;
         segb_s = segb; ca = 0;
@@ -927,7 +928,7 @@ __global__ void __launch_bounds__(1024) pair_scan_kernel(PairPlanArgs a) {
 }
 // one thread per list: unit = list | item << 32 | segment << 48, ordered (segment, item) inside the list; quad mode also gets the
 // resolved descriptor of every unit (DphUnit)
-__global__ void pair_units_kernel(PairPlanArgs a) {
+__global__ void group_units_kernel(GroupPlanArgs a) {
     const long long l = a.list_lo + (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (l >= a.list_hi) return;
     const int cnt = a.cnt[l];
@@ -962,7 +963,7 @@ __global__ void pair_units_kernel(PairPlanArgs a) {
         }
     }
 }
-__global__ void pair_fill_kernel(PairPlanArgs a) {
+__global__ void group_fill_kernel(GroupPlanArgs a) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= a.nq_probes) return;
     const int l = a.key[i];
@@ -972,38 +973,38 @@ __global__ void pair_fill_kernel(PairPlanArgs a) {
     }
 }
 
-int dph_launch_plan(dph_index* ix, int64_t n, int k, int keep, int grid, const int32_t* only_flagged, cudaStream_t st, int group) {
-    const bool pair = group > 1;
-    (void)k;
+int dph_launch_plan(dph_index* ix, const DphSearchPlan& sp, int64_t n, bool exact, const int32_t* only_flagged, cudaStream_t st) {
+    const int group = sp.pass_group(exact);
+    const bool grouped = group > 1;
     if (n == 0) return 0;
     PlanArgs a;
     a.key = ix->key.as<int>(); a.cd = ix->cd.as<float>(); a.list_len = ix->list_len; a.blk_off = (const long long*)ix->blk_off;
     a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.n = n; a.only_flagged = only_flagged;
     a.lutmax = ix->lutmax.as<float>(); a.segs = ix->segs.as<DphSeg>(); a.qblocks = ix->qinfo.as<unsigned>(); a.nseg = ix->nseg.as<int>(); a.eps = ix->eps.as<float>();
-    a.gdense = pair ? ix->gdense.as<unsigned>() : nullptr; a.qparams = pair ? ix->qparams.as<float2>() : nullptr;
+    a.gdense = grouped ? ix->gdense.as<unsigned>() : nullptr; a.qparams = grouped ? ix->qparams.as<float2>() : nullptr;
     plan_segs_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(a);
     DPH_CUDA(cudaGetLastError());
-    if (pair) {
-        PairPlanArgs p;
+    if (grouped) {
+        GroupPlanArgs p;
         p.key = ix->key.as<int>(); p.nq_probes = n * ix->nprobe; p.nprobe = ix->nprobe; p.list_len = ix->list_len; p.list_lo = ix->list_lo;
-        p.list_hi = ix->list_hi; p.nlist = ix->nlist; p.grid = grid; p.cnt = ix->pl_cnt.as<int>(); p.fill = ix->pl_fill.as<int>();
-        p.off = ix->pl_off.as<int>(); p.blockpre = ix->pl_blockpre.as<long long>(); p.entries = ix->pl_entries.as<unsigned>();
-        p.work = ix->pairwork.as<DphPairWork>(); p.unitpre = ix->pl_unitpre.as<int>(); p.units = ix->pl_units.as<unsigned long long>();
-        p.gsz = group == 4 ? DPH_QUAD_ITEM_Q : group;         // quad mode: an item runs one code read through two packed tables
-        p.udesc = group == 4 ? ix->pl_udesc.as<DphUnit>() : nullptr;
+        p.list_hi = ix->list_hi; p.nlist = ix->nlist; p.grid = sp.grid; p.cnt = ix->grp_cnt.as<int>(); p.fill = ix->grp_fill.as<int>();
+        p.off = ix->grp_off.as<int>(); p.blockpre = ix->grp_blockpre.as<long long>(); p.entries = ix->grp_entries.as<unsigned>();
+        p.work = ix->groupwork.as<DphGroupWork>(); p.unitpre = ix->grp_unitpre.as<int>(); p.units = ix->grp_units.as<unsigned long long>();
+        p.gsz = sp.item_q;
+        p.udesc = group == 4 ? ix->grp_udesc.as<DphUnit>() : nullptr;
         p.blk_off = (const long long*)ix->blk_off; p.cd = ix->cd.as<float>(); p.gdense = ix->gdense.as<unsigned>(); p.qparams = ix->qparams.as<float2>();
         DPH_CUDA(cudaMemsetAsync(p.cnt, 0, (size_t)ix->nlist * 4, st));
         DPH_CUDA(cudaMemsetAsync(p.fill, 0, (size_t)ix->nlist * 4, st));
         const unsigned nb = (unsigned)((p.nq_probes + 255) / 256);
-        pair_count_kernel<<<nb, 256, 0, st>>>(p);
-        pair_scan_kernel<<<1, 1024, 0, st>>>(p);
-        pair_fill_kernel<<<nb, 256, 0, st>>>(p);
-        if (ix->list_hi > ix->list_lo) pair_units_kernel<<<(unsigned)((ix->list_hi - ix->list_lo + 255) / 256), 256, 0, st>>>(p);
+        group_count_kernel<<<nb, 256, 0, st>>>(p);
+        group_scan_kernel<<<1, 1024, 0, st>>>(p);
+        group_fill_kernel<<<nb, 256, 0, st>>>(p);
+        if (ix->list_hi > ix->list_lo) group_units_kernel<<<(unsigned)((ix->list_hi - ix->list_lo + 255) / 256), 256, 0, st>>>(p);
         DPH_CUDA(cudaGetLastError());
     }
     PlanScanArgs b;
-    b.pairwork = pair ? ix->pairwork.as<DphPairWork>() : nullptr; b.nseg = ix->nseg.as<int>();
-    b.qblocks = ix->qinfo.as<unsigned>(); b.n = n; b.keep = keep; b.grid = grid; b.qpre = ix->wpre.as<long long>();
+    b.groupwork = grouped ? ix->groupwork.as<DphGroupWork>() : nullptr; b.nseg = ix->nseg.as<int>();
+    b.qblocks = ix->qinfo.as<unsigned>(); b.n = n; b.keep = sp.pass_keep(exact); b.grid = sp.grid; b.qpre = ix->wpre.as<long long>();
     b.cand_off = ix->cand_off.as<long long>(); b.cand_cnt = ix->cand_cnt.as<int>(); b.gthr = ix->gthr.as<unsigned>();
     b.work = ix->work.as<DphWork>();
     plan_scan_kernel<<<1, 1024, 0, st>>>(b);

@@ -18,8 +18,9 @@
 // dropped could have been in the top-k (T_k - max drop threshold > 2 eps); otherwise the query is flagged and re-run through
 // EXACT mode.
 //
-// PAIR (scan_pair_kernel, further down): two queries that probe the same list share every gather through int16-packed quantised
-// LUTs -- the default whenever lists are shared by the batch (the reference's nprobe = 256).
+// GROUPED (further down): QUAD (scan_quad_kernel, four queries per gather, 8-bit LUTs) is the default whenever long lists are shared
+// by the batch (the reference's nprobe = 256); PAIR (scan_pair_kernel, two per gather, u16 LUTs) serves the k whose keep does not fit
+// the quad kernel's candidate buffers.  search.cu (search_plan) picks the mode per batch.
 //
 // EXACT: canonical m-ascending fp32 sum for every code (bank conflicts and all) -- fallback/cross-check.
 #include "index_internal.cuh"
@@ -43,6 +44,7 @@ struct ScanShared {   // tail of the dynamic shared memory
     SelectScratch sc;
     int cnt; unsigned thr; int base; int ndone; int ndone_snap; int pad[3];
 };
+static_assert(DPH_MAX_K + DPH_KEEP_SLACK <= DPH_CAND_CAP - NT, "one-query latch margin: the largest keep fits below the latch (scan_kernel)");
 
 __device__ __forceinline__ uint4 ldg_stream(const uint4* p) {
     uint4 r;
@@ -333,16 +335,17 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 // Work: the plan inverts probes into per-list query groups and pairs them; an item = (list, query pair), linearised by
 // blocks; a CTA takes a contiguous block range, rebuilding the packed LUT (192 KB, from L2) at every item boundary.
 // =================================================================================================
-struct PairScanArgs {
+struct GroupScanArgs {     // both grouped kernels (scan_pair_kernel, scan_quad_kernel)
     const uint8_t* codes; const long long* blk_off; const int* list_len;
-    const int* pl_cnt; const int* pl_off; const unsigned long long* units; const unsigned* entries; const DphPairWork* work; int* next_unit;
+    const int* grp_cnt; const int* grp_off; const unsigned long long* units; const unsigned* entries; const DphGroupWork* work; int* next_unit;
     const unsigned short* lutq; const float2* qparams; const float* cd; const unsigned* gdense;
     unsigned* gthr; unsigned long long* cand; const long long* cand_off; int* cand_cnt;
     long long list_lo, list_hi; int nprobe; int keep;
     const DphUnit* udesc;          // quad mode: resolved unit records (plan)
     unsigned one;                  // the constant 1, as a run-time value (imad_add)
 };
-#define PCAP 1536
+#define PCAP 1536                  // PCAP - NT = DPH_PAIR_KEEP_MAX (each warp adds <= 32 per buffer after the latch is polled)
+static_assert(PCAP - NT == DPH_PAIR_KEEP_MAX, "pair latch margin");
 struct PairShared {
     unsigned long long cbuf[2][PCAP];
     SelectScratch sc;
@@ -398,7 +401,7 @@ __device__ __forceinline__ void warp_append(bool pass, unsigned long long key, u
     }
 }
 
-__global__ void __launch_bounds__(NT, 1) scan_pair_kernel(PairScanArgs a) {
+__global__ void __launch_bounds__(NT, 1) scan_pair_kernel(GroupScanArgs a) {
     unsigned char* const smem = dph_smem;
     PairShared* sh = reinterpret_cast<PairShared*>(smem + SMEM_LUT_FAST);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -420,8 +423,8 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(PairScanArgs a) {
         const unsigned nb = (unsigned)((len + 31) >> 5);
         const unsigned bi0 = (unsigned)(ud >> 48) * segb;
         const unsigned bend = (nb - bi0 < segb) ? nb : bi0 + segb;
-        const int e0 = a.pl_off[l] + 2 * it;
-        const bool has_b = (2 * it + 1) < a.pl_cnt[l];
+        const int e0 = a.grp_off[l] + 2 * it;
+        const bool has_b = (2 * it + 1) < a.grp_cnt[l];
         const unsigned ea = a.entries[e0], eb = has_b ? a.entries[e0 + 1] : ea;
         const long long qa = ea >> 10, qb = eb >> 10;
         const int ra = (int)(ea & 1023u), rb = (int)(eb & 1023u);
@@ -654,7 +657,7 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long l
 // A warp that runs out of blocks starts the next item's stream: it waits for its copy of the next record's head (requested with
 // cp.async after this item's table build; warp 0 also waits for the whole record here) and issues the L2 prefetch of its first
 // DPH_L2_PREFETCH_ROUNDS blocks of the next item, so HBM keeps streaming while the other warps finish, compact and publish.
-__device__ __forceinline__ void quad_prefetch_next(const PairScanArgs& a, const QuadShared* sh, int total_units, unsigned long long pol) {
+__device__ __forceinline__ void quad_prefetch_next(const GroupScanArgs& a, const QuadShared* sh, int total_units, unsigned long long pol) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     asm volatile("cp.async.wait_all;" ::: "memory");
     if (lane == 0 && sh->unit < total_units) {
@@ -671,7 +674,7 @@ __device__ __forceinline__ void quad_prefetch_next(const PairScanArgs& a, const 
 // of blocks, then a barrier, the compaction of the buffers over keep and the refresh of the thresholds; until every warp is done.
 // The code stream is loaded with the evict_first policy `pol`: each block is read once per batch.
 template <int NTAB, int IMADL>
-__device__ __forceinline__ void quad_item_rounds(const PairScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
+__device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
                                                  unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, int total_units,
                                                  unsigned long long pol, unsigned long long* ph, unsigned long long& ph_t) {
     (void)ph; (void)ph_t;
@@ -761,7 +764,7 @@ __device__ __forceinline__ uint4 quad_pack(unsigned a, unsigned b, unsigned c, u
     return make_uint4(__byte_perm(t0, u0, 0x5410), __byte_perm(t0, u0, 0x7632), __byte_perm(t1, u1, 0x5410), __byte_perm(t1, u1, 0x7632));
 }
 // This warp's first code block of an item into registers.
-__device__ __forceinline__ void quad_first_block(const PairScanArgs& a, const DphUnit* d, uint4 (&nxt)[6], unsigned long long pol) {
+__device__ __forceinline__ void quad_first_block(const GroupScanArgs& a, const DphUnit* d, uint4 (&nxt)[6], unsigned long long pol) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned b = d->bi0 + warp;
     if (b < d->bend) {
@@ -778,7 +781,7 @@ __device__ __forceinline__ void quad_first_block(const PairScanArgs& a, const Dp
 // next item into registers before the candidates are published, so those are in flight during the publish and the next table build.
 // The table sources (a few MB per batch, re-read at every item) are loaded evict_last, the code stream evict_first.
 template <int IMADL>
-__global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
+__global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
     unsigned char* const smem = dph_smem;
     QuadShared* sh = reinterpret_cast<QuadShared*>(smem + SMEM_QUAD_TABLES);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -916,8 +919,10 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(PairScanArgs a) {
 #undef QPH_MARK
 
 __global__ void smem_base_probe_kernel(unsigned* out) { *out = (unsigned)__cvta_generic_to_shared(dph_smem); }
+// scan_quad_kernel by IMAD level, knob 0 of dph_set_tuning (out of range: the default, 1)
+static void (*const quad_kernels[4])(GroupScanArgs) = {scan_quad_kernel<0>, scan_quad_kernel<1>, scan_quad_kernel<2>, scan_quad_kernel<3>};
 
-int dph_scan_setup_attrs() {
+static int dph_scan_setup_attrs() {
     static DphPerDeviceOnce once;
     if (!once.first()) return 0;
     {
@@ -932,51 +937,35 @@ int dph_scan_setup_attrs() {
     DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(ScanShared)));
     DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
     DPH_CUDA(cudaFuncSetAttribute(scan_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_quad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    for (auto f : quad_kernels) DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
     return 0;
 }
 
-int dph_launch_scan(dph_index* ix, int64_t n, int k, int keep, int mode, int grid, cudaStream_t st) {
-    (void)k;
+int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, cudaStream_t st) {
     if (n == 0) return 0;
     DPH_TRY(dph_scan_setup_attrs());
-    ScanArgs a;
-    a.codes = ix->codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
-    a.lut_canon = ix->lut_canon.as<float>(); a.gthr = ix->gthr.as<unsigned>();
-    a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
-    a.n = n; a.nprobe = ix->nprobe; a.keep = keep;
-    if (mode == DPH_SCAN_FAST)
-        scan_kernel<DPH_SCAN_FAST><<<grid, NT, SMEM_LUT_FAST + sizeof(ScanShared), st>>>(a);
-    else
-        scan_kernel<DPH_SCAN_EXACT><<<grid, NT, SMEM_LUT_EXACT + sizeof(ScanShared), st>>>(a);
-    DPH_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int dph_launch_scan_pair(dph_index* ix, int64_t n, int keep, int grid, cudaStream_t st, int group) {
-    if (n == 0) return 0;
-    DPH_TRY(dph_scan_setup_attrs());
-    PairScanArgs a;
-    a.codes = ix->codes; a.blk_off = (const long long*)ix->blk_off; a.list_len = ix->list_len; a.pl_cnt = ix->pl_cnt.as<int>();
-    a.pl_off = ix->pl_off.as<int>(); a.units = ix->pl_units.as<unsigned long long>(); a.entries = ix->pl_entries.as<unsigned>();
-    a.work = ix->pairwork.as<DphPairWork>(); a.next_unit = &ix->pairwork.as<DphPairWork>()->next_unit; a.lutq = ix->lutq.as<unsigned short>(); a.qparams = ix->qparams.as<float2>();
-    a.cd = ix->cd.as<float>(); a.gdense = ix->gdense.as<unsigned>(); a.gthr = ix->gthr.as<unsigned>();
-    a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
-    a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.keep = keep;
-    a.udesc = ix->pl_udesc.as<DphUnit>(); a.one = 1u;
-    if (group == 4) {
-        const size_t sm = SMEM_QUAD_TABLES + sizeof(QuadShared);
-        switch (g_dph_tune[0]) {
-            case 0: scan_quad_kernel<0><<<grid, QNT, sm, st>>>(a); break;
-            case 2: scan_quad_kernel<2><<<grid, QNT, sm, st>>>(a); break;
-            case 3: scan_quad_kernel<3><<<grid, QNT, sm, st>>>(a); break;
-            default: scan_quad_kernel<1><<<grid, QNT, sm, st>>>(a); break;
-        }
+    const int grid = p.grid, group = p.pass_group(exact), keep = p.pass_keep(exact);
+    if (group == 1) {
+        ScanArgs a;
+        a.codes = ix->codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
+        a.lut_canon = ix->lut_canon.as<float>(); a.gthr = ix->gthr.as<unsigned>();
+        a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
+        a.n = n; a.nprobe = ix->nprobe; a.keep = keep;
+        if (exact) scan_kernel<DPH_SCAN_EXACT><<<grid, NT, SMEM_LUT_EXACT + sizeof(ScanShared), st>>>(a);
+        else scan_kernel<DPH_SCAN_FAST><<<grid, NT, SMEM_LUT_FAST + sizeof(ScanShared), st>>>(a);
+    } else {
+        GroupScanArgs a;
+        a.codes = ix->codes; a.blk_off = (const long long*)ix->blk_off; a.list_len = ix->list_len; a.grp_cnt = ix->grp_cnt.as<int>();
+        a.grp_off = ix->grp_off.as<int>(); a.units = ix->grp_units.as<unsigned long long>(); a.entries = ix->grp_entries.as<unsigned>();
+        a.work = ix->groupwork.as<DphGroupWork>(); a.next_unit = &ix->groupwork.as<DphGroupWork>()->next_unit; a.lutq = ix->lutq.as<unsigned short>(); a.qparams = ix->qparams.as<float2>();
+        a.cd = ix->cd.as<float>(); a.gdense = ix->gdense.as<unsigned>(); a.gthr = ix->gthr.as<unsigned>();
+        a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
+        a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.keep = keep;
+        a.udesc = ix->grp_udesc.as<DphUnit>(); a.one = 1u;
+        const int lv = g_dph_tune[0] >= 0 && g_dph_tune[0] <= 3 ? g_dph_tune[0] : 1;
+        if (group == 4) quad_kernels[lv]<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
+        else scan_pair_kernel<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
     }
-    else scan_pair_kernel<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
     DPH_CUDA(cudaGetLastError());
     return 0;
 }

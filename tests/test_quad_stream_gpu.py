@@ -12,7 +12,7 @@ from tests.test_search_gpu import make_pair
 pytestmark = pytest.mark.gpu
 
 NLIST, NPROBE, BATCH = 4096, 32, 512
-SEG_BLOCKS = 128                          # shortest block segment of a split list (DPH_PAIR_SEG_MIN)
+SEG_BLOCKS = 128                          # shortest block segment of a split list (DPH_GROUP_SEG_MIN)
 
 
 def test_quad_item_chains_match_oracle(oracle):

@@ -328,19 +328,18 @@ def test_tensor_core_coarse_repair_path(oracle):
 
 def test_quad_mode_is_the_default_for_shared_long_lists(oracle):
     """Lists of >= 4096 vectors probed by several queries of the batch -> four queries share every gather (scan_quad_kernel);
-    groups of 1, 2, 3 and 4 queries per list all occur (33 queries x 6 probes over 12 lists), k + slack stays within the buffers."""
+    groups of 1, 2, 3 and 4 queries per list all occur (33 queries x 6 probes over 12 lists).  The mode follows from which
+    buffers keep fits: quad while k + max(2k, 100) <= 256 (k <= 85), pair while k + max(k // 2, 32) <= 1024 (k <= 683), then one
+    query per gather; both boundaries are checked from each side."""
     lens = uniform_lens(12 * 4500, 12)
     ref, gpu = make_pair(oracle, 12, lens)
     gpu.nprobe = 6
     x = near_queries(ref, 33, 21)
-    for k in (10, 40):
+    for k, group in ((10, 4), (40, 4), (85, 4), (86, 2), (300, 2), (683, 2), (684, 1)):
         D, I = gpu.search(x, k)
-        assert gpu.last_group_size() == 4
+        assert gpu.last_group_size() == group, f"k={k}"
         Dr, Ir = ref.search(x, k, 6)
-        assert_topk_equal(D, I, Dr, Ir, f"quad k={k}")
-    D, I = gpu.search(x, 300)                  # k + slack no longer fits the quad buffers -> pair-packed
-    assert gpu.last_group_size() == 2
-    assert_topk_equal(D, I, *ref.search(x, 300, 6), "pair fallback")
+        assert_topk_equal(D, I, Dr, Ir, f"k={k}, {group} queries per gather")
 
 
 def test_merge_shards_many_candidates():
