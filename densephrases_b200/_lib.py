@@ -84,6 +84,8 @@ _SIGS = {
     "dph_index_sync_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_remove_ms": (_i32, [_vp, _vp]),
     "dph_index_last_remove_tmp_bytes": (_i64, [_vp]),
+    "dph_index_merge_from": (_i32, [_vp, _vp, _i32, _i64]),
+    "dph_index_last_merge_ms": (_i32, [_vp, _vp]),
     "dph_index_train_coarse": (_i32, [_vp, _vp, _i64, _i32, _u64, _i64, _i32, _i32, _vp, _vp]),
     "dph_index_train_pq": (_i32, [_vp, _vp, _i64, _i32, _u64, _i64, _i32, _i32, _i32]),
     "dph_index_encode_pq": (_i32, [_vp, _vp, _i64, _vp, _i32]),

@@ -27,6 +27,10 @@ Updating a document (DESIGN.md 3.2): its phrases carry consecutive labels [first
     ix.remove_ids(range(first, first + n))       # faiss remove_ids(IDSelectorRange); a label array drops a set of documents
     ix.add_with_ids(x_new, ids_new)              # the document's new phrase vectors
 Keeping idx2id and the phrase metadata in step with re-added documents is the caller's job.
+Merging sub-indexes (the merge stage of build_phrase_index.py:282-338, DESIGN.md 3.4), e.g. one read from a %d.faiss file:
+    sub = artifacts.read_faiss_index(path)       # same OPQ matrix, centroids and PQ codebooks as ix
+    ix.merge_from(IvfPqIndex.from_arrays(sub["A"], sub["centroids"], sub["pq"], sub["list_len"], sub["codes"], sub["ids"]))
+    # several at once: ix.merge_from([a, b, c], add_id=offset) appends them in order, labels + offset; the sources stay as they were
 add_to_index below is the PyTorch encoder that runs without a GPU; its argmax / argmin have no fixed floating-point order, so on
 ties and near-ties it may pick other lists or codewords than IvfPqIndex.encode."""
 import numpy as np

@@ -98,9 +98,10 @@ struct dph_index {
     bool profile = false;              // CUDA events around the scan kernel of the last search chunk
     cudaEvent_t ev0[DPH_PROF_RING] = {}, ev1[DPH_PROF_RING] = {};
     int64_t prof_n = 0;
-    cudaEvent_t aev[6] = {};           // profiled adds and removes: stage boundaries (encode.cu, lists.cu, remove.cu)
+    cudaEvent_t aev[6] = {};           // profiled adds, removes and merges: stage boundaries (encode.cu, lists.cu, remove.cu, merge.cu)
     float add_ms[4] = {};              // last add: rotation, coarse, PQ encode, re-layout + scatter (ms)
     float remove_ms[3] = {};           // last remove: mark + plan, row moves + block shift, direct map (ms)
+    float merge_ms[4] = {};            // last merge: plan + alloc, block moves, source rows, direct map (ms)
     float train_ms[3] = {};            // last train_coarse / train_pq: assign, sort + update, split + renorm (ms, summed over iterations)
     int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
 };

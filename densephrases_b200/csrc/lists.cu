@@ -219,7 +219,8 @@ __global__ void __launch_bounds__(192) relayout_codes_kernel(uint8_t* dst, long 
     reinterpret_cast<uint4*>(dst + (long long)blockIdx.x * DPH_BLK_BYTES)[threadIdx.x] = v;
 }
 // labels of the new layout's old rows (-1 elsewhere; the new rows are written by add_scatter_kernel).  Implicit labels (ids_old null)
-// become explicit: list_start_old[l] + j, with their direct-map pairs at the row's old local position (already in label order).
+// become explicit: list_start_old[l] + j, with their direct-map pairs at the row's old local position (already in label order) unless
+// dm_ids is null (the merge builds its direct map from the labels' order instead).
 __global__ void relayout_ids_kernel(long long* dst, long long blk0, const long long* boff_new, const long long* boff_old, const int* len_old,
                                     long long lo, long long hi, const long long* ids_old, const long long* list_start_old,
                                     const long long* lrs_old, long long* dm_ids, long long* dm_rows) {
@@ -231,8 +232,10 @@ __global__ void relayout_ids_kernel(long long* dst, long long blk0, const long l
         if (ids_old) id = ids_old[(boff_old[l] + b) * 32 + threadIdx.x];
         else {
             id = list_start_old[l] + j;
-            dm_ids[lrs_old[l - lo] + j] = id;
-            dm_rows[lrs_old[l - lo] + j] = blk * 32 + threadIdx.x;
+            if (dm_ids) {
+                dm_ids[lrs_old[l - lo] + j] = id;
+                dm_rows[lrs_old[l - lo] + j] = blk * 32 + threadIdx.x;
+            }
         }
     }
     dst[(long long)blockIdx.x * 32 + threadIdx.x] = id;

@@ -202,6 +202,26 @@ class IvfPqIndex:
         """The largest total of the last remove's temporary device allocations, in bytes."""
         return int(L.lib().dph_index_last_remove_tmp_bytes(self._h))
 
+    # ---- merging indexes (invlists.merge_from of build_phrase_index.py:282-338; DESIGN.md 3.4) --------------
+    def merge_from(self, sources, add_id=0):
+        """== faiss index.merge_from(other, add_id) for one IvfPqIndex or a list of them, in order: every list gets each source's rows
+        of that list behind its own, labels shifted by add_id.  The sources are not modified (faiss empties `other`).  Raises
+        RuntimeError, leaving the index unchanged, on an incompatible source (d, nlist, device, shard range, or any bit of the OPQ
+        matrix, centroids or PQ codebooks), the index itself as a source, a label + add_id outside [0, 2^63) or too little device
+        memory.  Sources with no rows make it a no-op."""
+        sources = [sources] if isinstance(sources, IvfPqIndex) else list(sources)
+        for s in sources:
+            if not isinstance(s, IvfPqIndex):
+                raise TypeError(f"merge_from: sources must be IvfPqIndex handles, got {type(s)!r}")
+        arr = (C.c_void_p * max(len(sources), 1))(*[s._h for s in sources])
+        L.check(L.lib().dph_index_merge_from(self._h, arr, len(sources), int(add_id)))
+
+    def last_merge_ms(self):
+        """With set_profile(True): stage times of the last merge in ms (plan + alloc, block moves, source rows, direct map)."""
+        out = np.zeros(4, dtype=np.float32)
+        L.check(L.lib().dph_index_last_merge_ms(self._h, _np_ptr(out)))
+        return out
+
     # ---- training (faiss index.train, build_phrase_index.py:96-142; DESIGN.md 3.3) -------------------------
     def _train_input(self, x):
         """-> (pointer, n, mem, keepalive) for numpy or a CUDA float32 tensor [n, d]."""

@@ -159,6 +159,20 @@ class ShardedIvfPq:
         self.local.sync_list_len(before - removed)
         return int(removed.sum())
 
+    def merge_from(self, sources, add_id=0):
+        """== faiss index.merge_from (IvfPqIndex.merge_from) for one ShardedIvfPq or a list of them; a collective by convention: every
+        rank passes the same sources.  Each rank merges its own shard of each source, which must hold the same list range.  No
+        exchange is needed: every handle holds the global list lengths, so every rank reaches the same global lengths and list
+        starts.  A rejection that depends only on the handles' shapes and tables is the same on every rank; one that depends on this
+        rank's rows (a label + add_id out of range) or on its device memory leaves only that rank unchanged."""
+        sources = [sources] if isinstance(sources, ShardedIvfPq) else list(sources)
+        for s in sources:
+            if not isinstance(s, ShardedIvfPq):
+                raise TypeError(f"merge_from: sources must be ShardedIvfPq, got {type(s)!r}")
+            if (s.rank, s.world) != (self.rank, self.world) or getattr(s, "range", None) != getattr(self, "range", None):
+                raise RuntimeError("merge_from: a source is sharded differently (rank, world size or list range); the index is unchanged")
+        self.local.merge_from([s.local for s in sources], add_id)
+
     # ---- the slice of the faiss index API that MIPS uses (index.py:30-33,200,286,296) ----
     @property
     def ntotal(self):

@@ -16,6 +16,7 @@
  *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
  *   dph_index_remove_ids        <- index.remove_ids(IDSelectorBatch(ids) | IDSelectorRange(lo, hi)) (faiss 1.6.x IndexIVF)
  *   dph_index_sync_list_len     <- (sharded remove) the list lengths faiss keeps in one process, exchanged between shards
+ *   dph_index_merge_from        <- invlists.merge_from(sub_index.invlists, offset)            build_phrase_index.py:282-338
  *   dph_index_train_coarse      <- the coarse quantizer's k-means inside index.train(x)   build_phrase_index.py:96-142
  *   dph_index_train_pq          <- ProductQuantizer::train inside index.train(x) (and OPQMatrix::train's PQ)
  *   dph_index_encode_pq         <- OPQMatrix::train's pq_regular.compute_codes (PQ codes without a coarse residual)
@@ -116,6 +117,24 @@ int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len);
  * empty selector resets both to zero. */
 int dph_index_last_remove_ms(const dph_index* ix, float* ms_out /* [3] */);
 int64_t dph_index_last_remove_tmp_bytes(const dph_index* ix);
+
+/* ---- merging indexes (replaces the merge stage of build_phrase_index.py:282-338: invlists.merge_from of every sub-index, and
+ * faiss IndexIVF::merge_from(other, add_id); DESIGN.md 3.4 "Merging indexes") ----
+ * Appends the rows of the n_src sources src[0 .. n_src) to this index: for every list l the result holds this index's rows, then
+ * source 0's rows of l, then source 1's, and so on, each in its stored order.  A source row's label is its stored label (sequential:
+ * list_start_src[l] + j) plus add_id.  The device state afterwards is byte-identical to set_lists of the concatenated list-major
+ * arrays.  The sources are not modified (faiss empties `other`).  An index with sequential labels turns them into explicit ones on any
+ * merge that adds rows; the direct map is the stable merge of this index's map and each source's map in argument order, so
+ * reconstruct returns the latest source's row of a label present twice.  Sources with no rows make the call a no-op.  On a shard,
+ * every source must hold the same list range; the other lists' rows only count into the list lengths, so every rank merging its
+ * shards of the same sources reaches the same global state.  Rejected, with the index unchanged: a source with another d, nlist, M,
+ * device or shard range, or whose OPQ matrix, centroids or PQ codebooks differ in any bit (compared on the device); this index as its
+ * own source; a label + add_id that is negative or overflows; a list longer than 2^31 - 1 rows; too little device memory for the old
+ * and the new code, label and direct-map buffers of the shard at once (the peak of an add).  Synchronises the streams of this index
+ * and of the sources. */
+int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int n_src, int64_t add_id);
+/* Measurement hook: with profiling on, the stage times of the last merge in ms: plan + alloc, block moves, source rows, direct map. */
+int dph_index_last_merge_ms(const dph_index* ix, float* ms_out /* [4] */);
 
 /* ---- training (replaces index.train(x) of build_phrase_index.py:96-142: faiss Clustering with cp.spherical over IndexFlatIP and
  * ProductQuantizer::train on residuals; DESIGN.md 3.3 "Training the index") ----
