@@ -1,6 +1,7 @@
 // coarse_tc.cu -- coarse quantizer (faiss IndexFlatIP top-nprobe, reference call site densephrases/index.py:200) on the tensor
 // cores WITHOUT giving up the bit-exact sequential-FMA definition of the scores (oracle/ivfpq_ref.c):
-//   1. approximate scores  S~ = xr . C^T  with the 3xTF32 wgmma GEMM (gemm_tf32.cu), error <= B(q) = c |xr_q| max_l |C_l|;
+//   1. approximate scores  S~ = xr . C^T  with the 3xTF32 wgmma GEMM (gemm_tf32.cu), error <= B(q) = c |xr_q| max_l |C_l| plus an
+//      absolute term for subnormal operands, products and sums (tiny queries), norms in fp64;
 //   2. candidates = top-(nprobe + margin) of S~ per query;
 //   3. candidates are re-scored EXACTLY (one sequential fp32 FMA chain each, identical to sgemm_nt_seq / the oracle);
 //   4. top-nprobe of the exact scores, (score desc, list asc); the result is provably the global top-nprobe when
@@ -53,21 +54,19 @@ struct CoarseTcArgs {
 __global__ void __launch_bounds__(256, 3) coarse_tc_finish_kernel(CoarseTcArgs a) {     // <= 85 registers: room for 16 row loads in flight
     __shared__ float xq[DPH_D];
     __shared__ unsigned long long sel[DPH_MAX_NPROBE];
-    __shared__ float red[8];
+    __shared__ double red[8];
     const long long q = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    float n2 = 0.f;
-    for (int t = tid; t < DPH_D; t += 256) { const float v = a.xr[q * DPH_D + t]; xq[t] = v; n2 = fmaf(v, v, n2); }
+    // |xr_q| in fp64: the fp32 squares of a query with |xr| below ~2^-75 underflow (the norm would be 0 and so would the bound), and
+    // above ~2^64 they overflow
+    double n2 = 0.0;
+    for (int t = tid; t < DPH_D; t += 256) { const float v = a.xr[q * DPH_D + t]; xq[t] = v; n2 = fma((double)v, (double)v, n2); }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) n2 += __shfl_xor_sync(0xffffffffu, n2, off);
     if (lane == 0) red[warp] = n2;
     const int p2 = dph_next_pow2(a.ncand);
     for (int i = tid; i < p2; i += 256) sel[i] = 0ull;
     __syncthreads();
-    float qn = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; w++) qn += red[w];
-    qn = sqrtf(qn);
     unsigned amin_key = 0xFFFFFFFFu;          // smallest approximate score among the candidates
     for (int c = tid; c < a.ncand; c += 256) {
         const unsigned long long ck = a.cand_keys[q * a.ncand + c];
@@ -90,9 +89,17 @@ __global__ void __launch_bounds__(256, 3) coarse_tc_finish_kernel(CoarseTcArgs a
     // proof: the candidate set is complete unless a non-candidate could reach the nprobe-th exact score
     int flag = 0;
     if (a.nl > a.ncand) {
-        const float bound = 3.0e-4f * qn * (*a.cnorm_max);      // >= 3 K 2^-23 |x||c| (3xTF32 products + fp32 accumulation), K = 768
-        const float amin = dph_fkey_inv(s_amin);
-        const float te = dph_fkey_inv((unsigned)(sel[take - 1] >> 32));
+        // relative part: >= 3 K 2^-23 |x||c| (3xTF32 products + fp32 accumulation), K = 768, valid while every split operand,
+        // product and partial sum is a normal number.  Absolute part: a subnormal operand, product or partial sum that the tensor
+        // cores flush is off by less than 2^-126 (times the other operand): <= 2^-126 (3 sqrt(K) (|x| + |c|) + 4 K), doubled.
+        double qn = 0.0;
+#pragma unroll
+        for (int w = 0; w < 8; w++) qn += red[w];
+        qn = sqrt(qn);
+        const double cn = *a.cnorm_max;
+        const double bound = 3.0e-4 * qn * cn + 0x1p-125 * (3.0 * 27.72 * (qn + cn) + 4.0 * DPH_D);
+        const double amin = dph_fkey_inv(s_amin);
+        const double te = dph_fkey_inv((unsigned)(sel[take - 1] >> 32));
         if (!(amin + bound < te)) flag = 1;
     }
     if (tid == 0) a.flags[q] = flag;
@@ -116,15 +123,16 @@ __global__ void __launch_bounds__(256, 3) coarse_tc_repair_kernel(CoarseTcArgs a
 }
 
 __global__ void cnorm_max_kernel(const float* C, long long nl, float* out) {
-    // max_l |C_l|^2 -> sqrt; one warp per list, atomicMax on the (non-negative) float bits
+    // max_l |C_l|^2 -> sqrt, in fp64 and rounded up to fp32 (no underflow of tiny centroids); one warp per list, atomicMax on the
+    // (non-negative) float bits
     const long long l = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int lane = threadIdx.x & 31;
     if (l >= nl) return;
-    float s = 0.f;
-    for (int t = lane; t < DPH_D; t += 32) { const float v = C[l * DPH_D + t]; s = fmaf(v, v, s); }
+    double s = 0.0;
+    for (int t = lane; t < DPH_D; t += 32) { const double v = C[l * DPH_D + t]; s = fma(v, v, s); }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-    if (lane == 0) atomicMax(reinterpret_cast<unsigned*>(out), __float_as_uint(sqrtf(s)));
+    if (lane == 0) atomicMax(reinterpret_cast<unsigned*>(out), __float_as_uint(__double2float_ru(sqrt(s))));
 }
 
 // Coarse top-nprobe over lists [lo, lo+nl) of the index.  Writes keys64 (sharded path) or key/cd.  Returns 1 if the tensor-core
