@@ -102,7 +102,10 @@ class Encoder(object):
         """'bf16x3' (default of this class): meets the north star's 1e-3 tolerance on the query vectors at nearly the speed of 'tf32';
         'tf32' / False: 1xTF32 GEMMs (== torch 1.9's default for fp32 matmuls on Ampere+), fastest, ~2e-2;
         '3xtf32' / True: 3xTF32 split, fp32-accurate; 'bf16x3': bf16 (hi, lo) planes, three bf16 MMAs per product -- both meet
-        the 1e-3 tolerance of the north star, bf16x3 at the speed of 'tf32'."""
+        the 1e-3 tolerance of the north star, bf16x3 at the speed of 'tf32'.
+        Shown against fp64 (tests/test_encoder_limits_gpu.py, DESIGN §4.4) on random weights and on trained-like ones (saturated
+        heads, outlier dimensions, GELU tails): 'bf16x3' and '3xtf32' within 1e-3 (relative to the vector's largest entry) except on
+        vectors where torch fp32 itself loses ~2e-4; 'tf32' ~2e-2, but up to 0.13 (cosine 0.992) when outlier dimensions are present."""
         mode = precise if isinstance(precise, str) else ('3xtf32' if precise else 'tf32')
         if mode not in self.MODES:
             raise ValueError(f'unknown precision mode {mode!r}; choose one of {sorted(self.MODES)}')
@@ -119,7 +122,8 @@ class Encoder(object):
         return {'tf32': 1.0, '3xtf32': 3.0, 'bf16x3': 1.5}[mode]
 
     def default_mode(self):
-        """The fastest mode that meets the north star's 1e-3 tolerance on the [CLS] vectors (tests/test_encoder.py)."""
+        """The fastest mode that meets the north star's 1e-3 tolerance on the [CLS] vectors (tests/test_encoder.py; against fp64 on
+        trained-like weights as well, tests/test_encoder_limits_gpu.py, where '3xtf32' is not more accurate than 'bf16x3')."""
         return 'bf16x3' if 'bf16x3' in self.MODES else '3xtf32'
 
     def set_attention(self, tensor_core=True):

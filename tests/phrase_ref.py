@@ -8,9 +8,10 @@ import torch.nn.functional as F
 from oracle.encoder_ref import tower_forward
 
 
-def embed_phrase(sd, ids, mask, tt):
-    """-> (start [B,S,768], end (the same tensor), filter_start_logits [B,S], filter_end_logits [B,S]), fp32 on ids.device."""
+def embed_phrase(sd, ids, mask, tt, dtype=torch.float32):
+    """-> (start [B,S,768], end (the same tensor), filter_start_logits [B,S], filter_end_logits [B,S]) in `dtype` (fp32: the
+    restatement; fp64: the high-precision truth) on ids.device."""
     with torch.no_grad():
-        x = tower_forward(sd, 'phrase_encoder', ids, mask, tt)
-        logits = F.linear(x, sd['filter_linear.weight'].to(ids.device, torch.float32), sd['filter_linear.bias'].to(ids.device, torch.float32))
+        x = tower_forward(sd, 'phrase_encoder', ids, mask, tt, dtype=dtype)
+        logits = F.linear(x, sd['filter_linear.weight'].to(ids.device, dtype), sd['filter_linear.bias'].to(ids.device, dtype))
     return x, x, logits[..., 0], logits[..., 1]
