@@ -80,6 +80,10 @@ _SIGS = {
     "dph_index_copy_lists": (_i32, [_vp, _vp, _vp]),
     "dph_index_get_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_add_ms": (_i32, [_vp, _vp]),
+    "dph_index_set_code_residency": (_i32, [_vp, _i32, _i64]),
+    "dph_index_set_resident_lists": (_i32, [_vp, _vp, _i64]),
+    "dph_index_last_fetch": (_i32, [_vp, _vp, _vp]),
+    "dph_index_host_bytes": (_i64, [_vp]),
     "dph_index_remove_ids": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
     "dph_index_sync_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_remove_ms": (_i32, [_vp, _vp]),

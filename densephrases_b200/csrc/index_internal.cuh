@@ -104,7 +104,23 @@ struct dph_index {
     float merge_ms[4] = {};            // last merge: plan + alloc, block moves, source rows, direct map (ms)
     float train_ms[3] = {};            // last train_coarse / train_pq: assign, sort + update, split + renorm (ms, summed over iterations)
     int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
+
+    // Codes in host memory (host_codes.cu, DESIGN.md 3.5).  `codes` is then the device pointer of the mapped host array host_codes,
+    // and `region` holds in HBM the resident lists' blocks [0, res_blocks), then the stream region [res_blocks, + stream_blocks).
+    bool on_host = false;
+    uint8_t* host_codes = nullptr;
+    uint8_t* region = nullptr;
+    int64_t res_blocks = 0, stream_blocks = 0;
+    std::vector<int64_t> res_off;      // [nlist] block of a resident list in `region`, else -1
+    int64_t* res_off_dev = nullptr;    // [nlist] device copy
+    int64_t max_stream_blocks = 0;     // the shard's largest non-resident list, in blocks
+    int64_t fetch_counts[4] = {};      // last search: slices, lists fetched, blocks fetched, resident lists scanned
+    float fetch_ms = 0.f;              // last search: time of its fetch kernels (profiling on)
+    DevBuf view, fdesc, hs_D, hs_I, hs_G;   // per slice: block-offset view, fetch descriptors, the running top-k and the slice's
 };
+
+// Where the scan stage reads the codes of lists [lo, hi): the handle's own blocks, or in host mode the view of one slice.
+struct DphCodeSrc { const uint8_t* codes; const long long* blk_off; int64_t lo, hi; };
 
 // Writes list_len / list_start / blk_off of `L` to the device and makes `L` the handle's layout, totals included; the only code
 // that does.
@@ -199,12 +215,30 @@ int dph_launch_coarse_merge(const unsigned long long* keys, int W, int64_t n, in
 int dph_launch_lut(const float* xr, int64_t n, const float* pq, float* lut_canon, float* lutmax, float* lutmin, float* lutmaxv,
                    void* lutq, float2* qparams, cudaStream_t st, int group);
 // One pass of plan p (only_flagged, nullable: only the queries whose flag is set): segments, work, candidate areas, eps, group queue.
-int dph_launch_plan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, const int32_t* only_flagged, cudaStream_t st);
+int dph_launch_plan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, bool exact, const int32_t* only_flagged,
+                    cudaStream_t st);
 // ---- scan.cu ----
 // One pass: scan_kernel<EXACT> (exact), else by p.group scan_kernel<FAST>, scan_pair_kernel or scan_quad_kernel<IMADL>.
-int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, cudaStream_t st);
-int dph_launch_merge(dph_index* ix, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,
+int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, bool exact, cudaStream_t st);
+// Labels are read through the shard's own layout (ix->blk_off), the codes of the exact re-scoring from `codes`.
+int dph_launch_merge(dph_index* ix, const uint8_t* codes, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,
                      uint32_t* G, cudaStream_t st);
+// Dg/Ig/Gg [nshards, n, k] -> D/I [n, k] and, when G is non-null, G [n, k] (0xFFFFFFFF on an empty slot); order score desc, scan
+// position asc.
+int dph_launch_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* Gg, int nshards, int64_t n, int k, float* D, int64_t* I,
+                            uint32_t* G, cudaStream_t st);
+// ---- search.cu ----
+// The plan, scan and merge passes of the scan stage over the codes of src (the tables of the chunk are built).
+int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
+// ---- host_codes.cu ----
+// Host mode: the scan stage of one chunk, slice by slice (DESIGN.md 3.5).
+int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
+// Host mode after set_lists: the HBM region (stream only) and the resident table (empty).
+int dph_host_lists_ready(dph_index* ix);
+// ---- lists.cu ----
+__global__ void fill_blocks_kernel(uint8_t* codes, long long nblocks, const long long* blk_off, const int* list_len, long long list_lo,
+                                   long long list_hi, const uint8_t* raw, const long long* local_row_start, uint64_t seed, long long blk0,
+                                   long long raw_row0, long long out0);
 // ---- encode.cu ----
 int64_t dph_encode_chunk(const dph_index* ix);
 int dph_encode_rows(dph_index* ix, const float* x_dev, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad);

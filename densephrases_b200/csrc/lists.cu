@@ -56,9 +56,11 @@ int dph_commit_layout(dph_index* ix, DphLayout L) {
 
 // One thread per (block, lane, 16-byte chunk): writes the interleaved/rotated layout (common.cuh).
 // raw != nullptr: gather from list-major rows [*,96] (row index = local_row_start[l] + j); else synthesise from seed.
+// codes holds the shard's blocks from block out0 on (0: all of them; a staging chunk: its first block).
 __global__ void __launch_bounds__(192) fill_blocks_kernel(uint8_t* codes, long long nblocks, const long long* blk_off, const int* list_len,
                                                           long long list_lo, long long list_hi, const uint8_t* raw,
-                                                          const long long* local_row_start, uint64_t seed, long long blk0, long long raw_row0) {
+                                                          const long long* local_row_start, uint64_t seed, long long blk0, long long raw_row0,
+                                                          long long out0) {
     const long long blk = blk0 + blockIdx.x;                  // this launch covers blocks [blk0, nblocks)
     if (blk >= nblocks) return;
     const int lane = threadIdx.x & 31, c = threadIdx.x >> 5;   // c in 0..5
@@ -89,7 +91,7 @@ __global__ void __launch_bounds__(192) fill_blocks_kernel(uint8_t* codes, long l
     }
     uint4 v;
     memcpy(&v, bytes, 16);
-    *reinterpret_cast<uint4*>(codes + blk * DPH_BLK_BYTES + c * 512 + lane * 16) = v;
+    *reinterpret_cast<uint4*>(codes + (blk - out0) * DPH_BLK_BYTES + c * 512 + lane * 16) = v;
 }
 
 // labels of the padded rows of blocks [blk0, nblocks) + the direct-map pairs (label, padded row) of the real rows
@@ -108,10 +110,13 @@ __global__ void fill_ids_kernel(long long* ids, long long nblocks, const long lo
 }
 
 void dph_free_lists(dph_index* ix) {
+    if (ix->host_codes) { cudaFreeHost(ix->host_codes); ix->host_codes = nullptr; ix->codes = nullptr; }
     void** ptrs[] = {(void**)&ix->list_len, (void**)&ix->list_start, (void**)&ix->blk_off, (void**)&ix->codes, (void**)&ix->ids,
-                     (void**)&ix->dm_ids, (void**)&ix->dm_rows};
+                     (void**)&ix->dm_ids, (void**)&ix->dm_rows, (void**)&ix->region, (void**)&ix->res_off_dev};
     for (void** p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
     ix->blk_cap = ix->dm_cap = ix->dm_n = 0;
+    ix->res_blocks = ix->max_stream_blocks = 0;
+    ix->res_off.clear();
 }
 
 static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_t* codes, const int64_t* ids, bool synthetic, uint64_t seed) {
@@ -125,7 +130,10 @@ static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_
     // needs room for one copy of the codes; if an allocation fails, the handle is left without lists.
     dph_free_lists(ix);
     auto alloc = [](auto** p, int64_t count) { return cudaMalloc((void**)p, std::max<int64_t>(count, 1) * sizeof(**p)); };
-    DPH_CUDA(alloc(&ix->codes, nb * DPH_BLK_BYTES));
+    if (ix->on_host) {      // page-locked and mapped: the scan's fetch, reconstruct and copy_lists read it through its device pointer
+        DPH_CUDA(cudaHostAlloc((void**)&ix->host_codes, (size_t)std::max<int64_t>(nb, 1) * DPH_BLK_BYTES, cudaHostAllocMapped));
+        DPH_CUDA(cudaHostGetDevicePointer((void**)&ix->codes, ix->host_codes, 0));
+    } else DPH_CUDA(alloc(&ix->codes, nb * DPH_BLK_BYTES));
     if (labels) {
         DPH_CUDA(alloc(&ix->ids, nb * 32));
         DPH_CUDA(alloc(&ix->dm_ids, rows));
@@ -137,32 +145,41 @@ static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_
     DPH_CUDA(alloc(&ix->blk_off, nlist));
     ix->blk_cap = nb;
     DPH_TRY(dph_commit_layout(ix, std::move(L)));
+    if (ix->on_host) DPH_TRY(dph_host_lists_ready(ix));
     if (nb == 0) return 0;
     const DphLayout& lay = ix->lay;
     const long long* bo = (const long long*)ix->blk_off;
-    if (synthetic) {
+    if (synthetic && !ix->on_host) {
         for (int64_t b0 = 0; b0 < nb; b0 += (1ll << 30)) {          // grid.x limit
             const unsigned g = (unsigned)std::min<int64_t>(nb - b0, 1ll << 30);
-            fill_blocks_kernel<<<g, 192, 0, ix->stream>>>(ix->codes, std::min<int64_t>(nb, b0 + g), bo, ix->list_len, lo, hi, nullptr, nullptr, seed, b0, 0);
+            fill_blocks_kernel<<<g, 192, 0, ix->stream>>>(ix->codes, std::min<int64_t>(nb, b0 + g), bo, ix->list_len, lo, hi, nullptr, nullptr, seed, b0, 0, 0);
         }
         DPH_CUDA(cudaGetLastError());
     } else {
         // Upload in chunks of whole lists through a bounded staging buffer (<= ~256 MB of rows): the raw list-major copy never
         // sits on the device next to the blocked one.  Labels go the same way; the direct map (faiss DirectMap::Hashtable,
-        // build_phrase_index.py:139-141) is filled by the same kernel and sorted ON THE DEVICE.
-        int64_t max_rows;
+        // build_phrase_index.py:139-141) is filled by the same kernel and sorted ON THE DEVICE.  In host mode each chunk's blocks
+        // (uploaded or generated) are laid out in a device staging buffer and copied to the host array.
+        int64_t max_rows, max_blocks = 0;
         const std::vector<DphLayout::Chunk> chunks = lay.chunks(&max_rows);
+        for (const DphLayout::Chunk& c : chunks) max_blocks = std::max(max_blocks, c.blk1 - c.blk0);
         DevTmp tmp;
         const char* oom = "set_lists: staging";
-        uint8_t* d_raw; int64_t *d_lrs, *d_rawids = nullptr;
-        DPH_TRY(tmp.alloc(&d_raw, (size_t)max_rows * DPH_CODE, oom));
+        uint8_t *d_raw = nullptr, *d_blocks = nullptr; int64_t *d_lrs, *d_rawids = nullptr;
+        if (!synthetic) DPH_TRY(tmp.alloc(&d_raw, (size_t)max_rows * DPH_CODE, oom));
+        if (ix->on_host) DPH_TRY(tmp.alloc(&d_blocks, (size_t)max_blocks * DPH_BLK_BYTES, oom));
         DPH_TRY(tmp.alloc(&d_lrs, lay.row_start.size(), oom));
         if (labels) DPH_TRY(tmp.alloc(&d_rawids, (size_t)max_rows, oom));
         DPH_CUDA(cudaMemcpy(d_lrs, lay.row_start.data(), lay.row_start.size() * 8, cudaMemcpyHostToDevice));
         for (const DphLayout::Chunk& c : chunks) {
-            DPH_CUDA(cudaMemcpyAsync(d_raw, codes + (size_t)c.row0 * DPH_CODE, (size_t)c.rows * DPH_CODE, cudaMemcpyHostToDevice, ix->stream));
-            fill_blocks_kernel<<<(unsigned)(c.blk1 - c.blk0), 192, 0, ix->stream>>>(ix->codes, c.blk1, bo, ix->list_len, lo, hi, d_raw,
-                                                                                     (const long long*)d_lrs, 0, c.blk0, c.row0);
+            if (!synthetic)
+                DPH_CUDA(cudaMemcpyAsync(d_raw, codes + (size_t)c.row0 * DPH_CODE, (size_t)c.rows * DPH_CODE, cudaMemcpyHostToDevice, ix->stream));
+            fill_blocks_kernel<<<(unsigned)(c.blk1 - c.blk0), 192, 0, ix->stream>>>(ix->on_host ? d_blocks : ix->codes, c.blk1, bo, ix->list_len, lo,
+                                                                                     hi, d_raw, (const long long*)d_lrs, seed, c.blk0, c.row0,
+                                                                                     ix->on_host ? c.blk0 : 0);
+            if (ix->on_host)
+                DPH_CUDA(cudaMemcpyAsync(ix->host_codes + (size_t)c.blk0 * DPH_BLK_BYTES, d_blocks, (size_t)(c.blk1 - c.blk0) * DPH_BLK_BYTES,
+                                         cudaMemcpyDeviceToHost, ix->stream));
             if (labels) {
                 DPH_CUDA(cudaMemcpyAsync(d_rawids, ids + c.row0, (size_t)c.rows * 8, cudaMemcpyHostToDevice, ix->stream));
                 fill_ids_kernel<<<(unsigned)(c.blk1 - c.blk0), 32, 0, ix->stream>>>((long long*)ix->ids, c.blk1, bo, ix->list_len, lo, hi,
@@ -276,6 +293,7 @@ __global__ void add_scatter_kernel(long long n, const long long* sorted_list, co
 DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem) {
     DPH_TRY(check_ready(ix, 1));
     DPH_CHECK(n >= 0, "add_with_ids: n must be >= 0");
+    DPH_CHECK(!ix->on_host, "add_with_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
     if (n == 0) return 0;
     cudaStream_t st = ix->stream;

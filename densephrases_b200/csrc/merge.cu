@@ -88,6 +88,7 @@ static bool label_ok(int64_t v, int64_t add_id) {
 DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int n_src, int64_t add_id) {
     DPH_TRY(check_ready(ix, 1));
     DPH_CHECK(n_src >= 0 && (src != nullptr || n_src == 0), "merge_from: bad source list; the index is unchanged");
+    DPH_CHECK(!ix->on_host, "merge_from: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
     for (float& a : ix->merge_ms) a = 0.f;
     cudaStream_t st = ix->stream;
@@ -101,6 +102,7 @@ DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int
         const dph_index* o = src[s];
         DPH_CHECK(o != nullptr, "merge_from: a source is null; the index is unchanged");
         DPH_CHECK(o != ix, "merge_from: the index cannot be its own source; the index is unchanged");
+        DPH_CHECK(!o->on_host, "merge_from: a source keeps its codes in host memory, which a merge does not read; the index is unchanged");
         DPH_CHECK(o->A && o->C && o->pq && o->list_len, "merge_from: a source is not fully constructed (opq/centroids/pq/lists); the index is unchanged");
         DPH_CHECK(o->d == ix->d && o->M == ix->M && o->nlist == nlist && o->device == ix->device,
                   "merge_from: a source has another d, nlist, M or device; the index is unchanged");

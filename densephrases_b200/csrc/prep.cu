@@ -973,33 +973,34 @@ __global__ void group_fill_kernel(GroupPlanArgs a) {
     }
 }
 
-int dph_launch_plan(dph_index* ix, const DphSearchPlan& sp, int64_t n, bool exact, const int32_t* only_flagged, cudaStream_t st) {
+int dph_launch_plan(dph_index* ix, const DphSearchPlan& sp, const DphCodeSrc& src, int64_t n, bool exact, const int32_t* only_flagged,
+                    cudaStream_t st) {
     const int group = sp.pass_group(exact);
     const bool grouped = group > 1;
     if (n == 0) return 0;
     PlanArgs a;
-    a.key = ix->key.as<int>(); a.cd = ix->cd.as<float>(); a.list_len = ix->list_len; a.blk_off = (const long long*)ix->blk_off;
-    a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.n = n; a.only_flagged = only_flagged;
+    a.key = ix->key.as<int>(); a.cd = ix->cd.as<float>(); a.list_len = ix->list_len; a.blk_off = src.blk_off;
+    a.list_lo = src.lo; a.list_hi = src.hi; a.nprobe = ix->nprobe; a.n = n; a.only_flagged = only_flagged;
     a.lutmax = ix->lutmax.as<float>(); a.segs = ix->segs.as<DphSeg>(); a.qblocks = ix->qinfo.as<unsigned>(); a.nseg = ix->nseg.as<int>(); a.eps = ix->eps.as<float>();
     a.gdense = grouped ? ix->gdense.as<unsigned>() : nullptr; a.qparams = grouped ? ix->qparams.as<float2>() : nullptr;
     plan_segs_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(a);
     DPH_CUDA(cudaGetLastError());
     if (grouped) {
         GroupPlanArgs p;
-        p.key = ix->key.as<int>(); p.nq_probes = n * ix->nprobe; p.nprobe = ix->nprobe; p.list_len = ix->list_len; p.list_lo = ix->list_lo;
-        p.list_hi = ix->list_hi; p.nlist = ix->nlist; p.grid = sp.grid; p.cnt = ix->grp_cnt.as<int>(); p.fill = ix->grp_fill.as<int>();
+        p.key = ix->key.as<int>(); p.nq_probes = n * ix->nprobe; p.nprobe = ix->nprobe; p.list_len = ix->list_len; p.list_lo = src.lo;
+        p.list_hi = src.hi; p.nlist = ix->nlist; p.grid = sp.grid; p.cnt = ix->grp_cnt.as<int>(); p.fill = ix->grp_fill.as<int>();
         p.off = ix->grp_off.as<int>(); p.blockpre = ix->grp_blockpre.as<long long>(); p.entries = ix->grp_entries.as<unsigned>();
         p.work = ix->groupwork.as<DphGroupWork>(); p.unitpre = ix->grp_unitpre.as<int>(); p.units = ix->grp_units.as<unsigned long long>();
         p.gsz = sp.item_q;
         p.udesc = group == 4 ? ix->grp_udesc.as<DphUnit>() : nullptr;
-        p.blk_off = (const long long*)ix->blk_off; p.cd = ix->cd.as<float>(); p.gdense = ix->gdense.as<unsigned>(); p.qparams = ix->qparams.as<float2>();
+        p.blk_off = src.blk_off; p.cd = ix->cd.as<float>(); p.gdense = ix->gdense.as<unsigned>(); p.qparams = ix->qparams.as<float2>();
         DPH_CUDA(cudaMemsetAsync(p.cnt, 0, (size_t)ix->nlist * 4, st));
         DPH_CUDA(cudaMemsetAsync(p.fill, 0, (size_t)ix->nlist * 4, st));
         const unsigned nb = (unsigned)((p.nq_probes + 255) / 256);
         group_count_kernel<<<nb, 256, 0, st>>>(p);
         group_scan_kernel<<<1, 1024, 0, st>>>(p);
         group_fill_kernel<<<nb, 256, 0, st>>>(p);
-        if (ix->list_hi > ix->list_lo) group_units_kernel<<<(unsigned)((ix->list_hi - ix->list_lo + 255) / 256), 256, 0, st>>>(p);
+        if (src.hi > src.lo) group_units_kernel<<<(unsigned)((src.hi - src.lo + 255) / 256), 256, 0, st>>>(p);
         DPH_CUDA(cudaGetLastError());
     }
     PlanScanArgs b;

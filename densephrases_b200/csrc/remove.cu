@@ -124,6 +124,7 @@ __global__ void rm_dm_gather_kernel(long long d0, long long n, const long long* 
 DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_ids, int64_t range_lo, int64_t range_hi, int mem,
                                  int64_t* n_removed_out, int64_t* removed_per_list_out) {
     DPH_CHECK(ix && ix->list_len, "remove_ids: lists are not set");
+    DPH_CHECK(!ix->on_host, "remove_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CHECK(n_ids >= 0, "remove_ids: n_ids must be >= 0; the index is unchanged");
     DPH_CHECK(!(ids && (range_lo != 0 || range_hi != 0)), "remove_ids: give a label set or a label range, not both; the index is unchanged");
     DPH_CHECK(ids || n_ids == 0, "remove_ids: n_ids > 0 without labels; the index is unchanged");
@@ -306,6 +307,7 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
 
 DPH_API int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len) {
     DPH_CHECK(ix && ix->list_len, "sync_list_len: lists are not set");
+    DPH_CHECK(!ix->on_host, "sync_list_len: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DphLayout L;
     DPH_TRY(L.build(ix, list_len, "sync_list_len: bad list length; the index is unchanged"));
     bool changed = false;

@@ -941,13 +941,13 @@ static int dph_scan_setup_attrs() {
     return 0;
 }
 
-int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact, cudaStream_t st) {
+int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, bool exact, cudaStream_t st) {
     if (n == 0) return 0;
     DPH_TRY(dph_scan_setup_attrs());
     const int grid = p.grid, group = p.pass_group(exact), keep = p.pass_keep(exact);
     if (group == 1) {
         ScanArgs a;
-        a.codes = ix->codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
+        a.codes = src.codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
         a.lut_canon = ix->lut_canon.as<float>(); a.gthr = ix->gthr.as<unsigned>();
         a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
         a.n = n; a.nprobe = ix->nprobe; a.keep = keep;
@@ -955,12 +955,12 @@ int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, bool exact
         else scan_kernel<DPH_SCAN_FAST><<<grid, NT, SMEM_LUT_FAST + sizeof(ScanShared), st>>>(a);
     } else {
         GroupScanArgs a;
-        a.codes = ix->codes; a.blk_off = (const long long*)ix->blk_off; a.list_len = ix->list_len; a.grp_cnt = ix->grp_cnt.as<int>();
+        a.codes = src.codes; a.blk_off = src.blk_off; a.list_len = ix->list_len; a.grp_cnt = ix->grp_cnt.as<int>();
         a.grp_off = ix->grp_off.as<int>(); a.units = ix->grp_units.as<unsigned long long>(); a.entries = ix->grp_entries.as<unsigned>();
         a.work = ix->groupwork.as<DphGroupWork>(); a.next_unit = &ix->groupwork.as<DphGroupWork>()->next_unit; a.lutq = ix->lutq.as<unsigned short>(); a.qparams = ix->qparams.as<float2>();
         a.cd = ix->cd.as<float>(); a.gdense = ix->gdense.as<unsigned>(); a.gthr = ix->gthr.as<unsigned>();
         a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
-        a.list_lo = ix->list_lo; a.list_hi = ix->list_hi; a.nprobe = ix->nprobe; a.keep = keep;
+        a.list_lo = src.lo; a.list_hi = src.hi; a.nprobe = ix->nprobe; a.keep = keep;
         a.udesc = ix->grp_udesc.as<DphUnit>(); a.one = 1u;
         const int lv = g_dph_tune[0] >= 0 && g_dph_tune[0] <= 3 ? g_dph_tune[0] : 1;
         if (group == 4) quad_kernels[lv]<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
@@ -978,6 +978,7 @@ struct MergeArgs {
     const unsigned long long* cand; const long long* cand_off; const int* cand_cnt; const unsigned* gthr; const float* eps;
     const DphSeg* segs; const int* nseg; int nprobe; int k; int mode;
     const uint8_t* codes; const float* lut_canon; const long long* ids; const long long* list_start;
+    const long long* lab_off;       // the shard's first block of each list: labels follow its layout whatever `codes` is
     float* D; long long* I; unsigned* G; int* flags; const int* only_flagged;
 };
 
@@ -1068,20 +1069,21 @@ __global__ void __launch_bounds__(256) merge_kernel(MergeArgs a) {
             gi = dph_ckey_gidx(e); d = dph_ckey_score(e);
             const DphSeg s = segs[find_seg(sgs, nsg, gi)];
             const unsigned j = gi - s.gstart;
-            id = a.ids ? a.ids[s.blk * 32 + j] : a.list_start[s.list] + (long long)j;
+            id = a.ids ? a.ids[a.lab_off[s.list] * 32 + j] : a.list_start[s.list] + (long long)j;
         }
         a.D[q * k + i] = d; a.I[q * k + i] = id; a.G[q * k + i] = gi;
     }
     if (a.mode == DPH_SCAN_FAST && tid == 0) a.flags[q] = flag;
 }
 
-int dph_launch_merge(dph_index* ix, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I, uint32_t* G,
-                     cudaStream_t st) {
+int dph_launch_merge(dph_index* ix, const uint8_t* codes, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,
+                     uint32_t* G, cudaStream_t st) {
     if (n == 0) return 0;
     MergeArgs a;
     a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
     a.gthr = ix->gthr.as<unsigned>(); a.eps = ix->eps.as<float>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.nprobe = ix->nprobe; a.k = k; a.mode = mode;
-    a.codes = ix->codes; a.lut_canon = ix->lut_canon.as<float>(); a.ids = (const long long*)ix->ids; a.list_start = (const long long*)ix->list_start;
+    a.codes = codes; a.lut_canon = ix->lut_canon.as<float>(); a.ids = (const long long*)ix->ids; a.list_start = (const long long*)ix->list_start;
+    a.lab_off = (const long long*)ix->blk_off;
     a.D = D; a.I = (long long*)I; a.G = G; a.flags = ix->flags.as<int>(); a.only_flagged = only_flagged;
     merge_kernel<<<(unsigned)n, 256, 0, st>>>(a);
     DPH_CUDA(cudaGetLastError());
@@ -1146,7 +1148,7 @@ DPH_API int dph_merge_shards_packed(const int64_t* Pg, int nshards, int64_t n, i
 // merge_shards: all-gathered per-shard top-k -> global top-k, order (score desc, scan position asc).
 // =================================================================================================
 __global__ void __launch_bounds__(256) merge_shards_kernel(const float* Dg, const long long* Ig, const unsigned* Gg, int nshards, long long n,
-                                                            int k, float* D, long long* I) {
+                                                            int k, float* D, long long* I, unsigned* G) {
     extern __shared__ unsigned long long ms[];     // keys [p2] then payload index is recovered from a parallel array
     const long long q = blockIdx.x;
     const int tid = threadIdx.x;
@@ -1169,8 +1171,9 @@ __global__ void __launch_bounds__(256) merge_shards_kernel(const float* Dg, cons
     for (int i = tid; i < k; i += blockDim.x) {
         float d = DPH_NEUTRAL; long long id = -1;
         unsigned long long key = keys[i];
+        unsigned gi = 0xFFFFFFFFu;
         if (key != 0ull) {
-            unsigned gi = dph_ckey_gidx(key);
+            gi = dph_ckey_gidx(key);
             d = dph_ckey_score(key);
             for (int s = 0; s < nshards && id < 0; s++)
                 for (int r = 0; r < k; r++) {
@@ -1179,17 +1182,23 @@ __global__ void __launch_bounds__(256) merge_shards_kernel(const float* Dg, cons
                 }
         }
         D[q * k + i] = d; I[q * k + i] = id;
+        if (G) G[q * k + i] = gi;
     }
 }
 
-DPH_API int dph_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* Gg, int nshards, int64_t n, int k, float* D, int64_t* I,
-                                void* cuda_stream) {
+int dph_launch_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* Gg, int nshards, int64_t n, int k, float* D, int64_t* I,
+                            uint32_t* G, cudaStream_t st) {
     if (n == 0) return 0;
     DPH_CHECK(nshards >= 1 && k >= 1 && (long long)nshards * k <= 8192, "merge_shards: nshards*k must be <= 8192");
     int p2 = 1; while (p2 < nshards * k) p2 <<= 1;
     static DphPerDeviceOnce once;
     if (once.first()) { DPH_CUDA(cudaFuncSetAttribute(merge_shards_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 8)); }
-    merge_shards_kernel<<<(unsigned)n, 256, p2 * 8, (cudaStream_t)cuda_stream>>>(Dg, (const long long*)Ig, Gg, nshards, n, k, D, (long long*)I);
+    merge_shards_kernel<<<(unsigned)n, 256, p2 * 8, st>>>(Dg, (const long long*)Ig, Gg, nshards, n, k, D, (long long*)I, G);
     DPH_CUDA(cudaGetLastError());
     return 0;
+}
+
+DPH_API int dph_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* Gg, int nshards, int64_t n, int k, float* D, int64_t* I,
+                                void* cuda_stream) {
+    return dph_launch_merge_shards(Dg, Ig, Gg, nshards, n, k, D, I, nullptr, (cudaStream_t)cuda_stream);
 }

@@ -96,9 +96,27 @@ static int coarse_stage(dph_index* ix, const float* x_dev, int64_t n, unsigned l
     return 0;
 }
 
-// Scan stage, from the rotated queries in xr and the probes in (key, cd): tables, then the fast pass (plan, scan, merge) and the
-// exact re-run of the queries its merge flagged (launches that exit at once when none is), or the exact pass alone in EXACT mode.
-// Writes D, I, G [n, k]; the profiling events bracket the first pass's scan kernel.
+// The fast pass (plan, scan, merge) over the codes of src and the exact re-run of the queries its merge flagged (launches that exit
+// at once when none is), or the exact pass alone in EXACT mode.  Writes D, I, G [n, k]; the profiling events bracket the first
+// pass's scan kernel.
+int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
+    cudaStream_t st = ix->stream;
+    const bool exact = p.exact_only;
+    if (exact) DPH_CUDA(cudaMemsetAsync(ix->flags.p, 0, (size_t)n * 4, st));
+    DPH_TRY(dph_launch_plan(ix, p, src, n, exact, nullptr, st));
+    if (ix->profile) DPH_CUDA(cudaEventRecord(ix->ev0[ix->prof_n % DPH_PROF_RING], st));
+    DPH_TRY(dph_launch_scan(ix, p, src, n, exact, st));
+    if (ix->profile) { DPH_CUDA(cudaEventRecord(ix->ev1[ix->prof_n % DPH_PROF_RING], st)); ix->prof_n++; }
+    DPH_TRY(dph_launch_merge(ix, src.codes, n, k, exact ? DPH_SCAN_EXACT : DPH_SCAN_FAST, nullptr, D, I, G, st));
+    if (exact) return 0;
+    DPH_TRY(dph_launch_plan(ix, p, src, n, true, ix->flags.as<int32_t>(), st));
+    DPH_TRY(dph_launch_scan(ix, p, src, n, true, st));
+    DPH_TRY(dph_launch_merge(ix, src.codes, n, k, DPH_SCAN_EXACT, ix->flags.as<int32_t>(), D, I, G, st));
+    return 0;
+}
+
+// Scan stage, from the rotated queries in xr and the probes in (key, cd): the tables, then the passes over the shard's codes -- in
+// host mode slice by slice, the tables built once for all slices.
 static int scan_stage(dph_index* ix, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
     cudaStream_t st = ix->stream;
     const DphSearchPlan p = search_plan(ix, n, k);
@@ -107,18 +125,15 @@ static int scan_stage(dph_index* ix, int64_t n, int k, float* D, int64_t* I, uin
     DPH_TRY(dph_launch_lut(ix->xr.as<float>(), n, ix->pq, ix->lut_canon.as<float>(), ix->lutmax.as<float>(),
                            ix->lutmin.as<float>(), ix->lutmaxv.as<float>(), p.grouped() ? ix->lutq.p : nullptr,
                            p.grouped() ? ix->qparams.as<float2>() : nullptr, st, p.group));
-    const bool exact = p.exact_only;
-    if (exact) DPH_CUDA(cudaMemsetAsync(ix->flags.p, 0, (size_t)n * 4, st));
-    DPH_TRY(dph_launch_plan(ix, p, n, exact, nullptr, st));
-    if (ix->profile) DPH_CUDA(cudaEventRecord(ix->ev0[ix->prof_n % DPH_PROF_RING], st));
-    DPH_TRY(dph_launch_scan(ix, p, n, exact, st));
-    if (ix->profile) { DPH_CUDA(cudaEventRecord(ix->ev1[ix->prof_n % DPH_PROF_RING], st)); ix->prof_n++; }
-    DPH_TRY(dph_launch_merge(ix, n, k, exact ? DPH_SCAN_EXACT : DPH_SCAN_FAST, nullptr, D, I, G, st));
-    if (exact) return 0;
-    DPH_TRY(dph_launch_plan(ix, p, n, true, ix->flags.as<int32_t>(), st));
-    DPH_TRY(dph_launch_scan(ix, p, n, true, st));
-    DPH_TRY(dph_launch_merge(ix, n, k, DPH_SCAN_EXACT, ix->flags.as<int32_t>(), D, I, G, st));
-    return 0;
+    if (ix->on_host) return dph_host_scan(ix, p, n, k, D, I, G);
+    const DphCodeSrc src{ix->codes, (const long long*)ix->blk_off, ix->list_lo, ix->list_hi};
+    return dph_scan_passes(ix, p, src, n, k, D, I, G);
+}
+
+// Host mode: the fetch counters describe the last search call.
+static void reset_fetch(dph_index* ix) {
+    std::fill(ix->fetch_counts, ix->fetch_counts + 4, 0);
+    ix->fetch_ms = 0.f;
 }
 
 static int64_t chunk_size(const dph_index* ix, int64_t n) {
@@ -130,6 +145,7 @@ static int64_t chunk_size(const dph_index* ix, int64_t n) {
 DPH_API int dph_index_search_partial(dph_index* ix, const float* x_dev, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
     DPH_TRY(check_ready(ix, k));
     DPH_CUDA(cudaSetDevice(ix->device));
+    reset_fetch(ix);
     const int64_t cs = chunk_size(ix, n);
     for (int64_t o = 0; o < n; o += cs) {
         const int64_t m = std::min(cs, n - o);
@@ -169,6 +185,7 @@ DPH_API int dph_index_search_preassigned(dph_index* ix, const uint64_t* keys_gat
     DPH_TRY(check_ready(ix, k));
     DPH_CUDA(cudaSetDevice(ix->device));
     DPH_CHECK(n == ix->last_coarse_n, "search_preassigned must follow coarse_local with the same batch");
+    reset_fetch(ix);
     DPH_TRY(size_coarse(ix, n));
     DPH_TRY(dph_launch_coarse_merge((const unsigned long long*)keys_gathered_dev, nshards, n, ix->nprobe, ix->key.as<int32_t>(), ix->cd.as<float>(),
                                     ix->stream));
@@ -212,6 +229,7 @@ DPH_API int dph_index_search_assigned(dph_index* ix, const float* rec_dev, int64
     DPH_TRY(check_ready(ix, k));
     DPH_CUDA(cudaSetDevice(ix->device));
     if (n == 0) return 0;
+    reset_fetch(ix);
     DPH_TRY(size_coarse(ix, n));
     unpack_records_kernel<<<(unsigned)n, 256, 0, ix->stream>>>(rec_dev, ix->nprobe, ix->xr.as<float>(), ix->key.as<int>(), ix->cd.as<float>());
     DPH_CUDA(cudaGetLastError());

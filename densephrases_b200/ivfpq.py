@@ -15,6 +15,13 @@ def _np_ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def default_stream_bytes(list_len, lo=0, hi=None):
+    """The stream region a host-mode index gets when none is given: 1 GiB, or the largest list of lists [lo, hi) if that is more."""
+    list_len = np.asarray(list_len, dtype=np.int64)[lo:hi]
+    largest = int(list_len.max()) if len(list_len) else 0
+    return max(1 << 30, (largest + 31) // 32 * 3072)
+
+
 class IvfPqIndex:
     def __init__(self, nlist, d=768, M=96, nbits=8, device=0):
         self._h = C.c_void_p()
@@ -27,14 +34,18 @@ class IvfPqIndex:
             L._lib.dph_index_free(h)
 
     @classmethod
-    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, device=0, shard=None):
-        """Build from the arrays a faiss IndexPreTransform(OPQ)->IndexIVFPQ file holds (index.py:30)."""
+    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, device=0, shard=None, codes_on_host=False, stream_bytes=None):
+        """Build from the arrays a faiss IndexPreTransform(OPQ)->IndexIVFPQ file holds (index.py:30).  codes_on_host: keep the codes in
+        page-locked host memory and stream the probed lists through a device region of stream_bytes (None: default_stream_bytes);
+        see set_code_residency."""
         ix = cls(len(list_len), device=device)
         ix.set_opq(A)
         ix.set_centroids(centroids)
         ix.set_pq(pq)
         if shard is not None:
             ix.set_shard(*shard)
+        if codes_on_host:
+            ix.set_code_residency(True, default_stream_bytes(list_len, *(shard or (0, None))) if stream_bytes is None else stream_bytes)
         ix.set_lists(list_len, codes, ids)
         return ix
 
@@ -73,6 +84,35 @@ class IvfPqIndex:
     def set_lists_synthetic(self, list_len, seed):
         list_len = np.ascontiguousarray(list_len, dtype=np.int64)
         L.check(L.lib().dph_index_set_lists_synthetic(self._h, _np_ptr(list_len), seed))
+
+    # ---- codes in host memory (DESIGN.md 3.5) ---------------------------------------------------
+    def set_code_residency(self, on_host, stream_bytes=0):
+        """on_host=True (before set_lists): the codes live in page-locked host memory; every search copies the probed lists that are
+        not resident into a device stream region of stream_bytes, slice by slice, with results bit-identical to a device-resident
+        index.  stream_bytes may be changed later.  The index is then read-only: add, remove and merge raise RuntimeError."""
+        L.check(L.lib().dph_index_set_code_residency(self._h, int(bool(on_host)), int(stream_bytes)))
+
+    def set_resident_lists(self, lists):
+        """Host mode: keep these lists of this shard in device memory (replaces the previous set; [] empties it).  To choose them,
+        count the probes of a sample search: ``np.bincount(ix.last_probes(n).ravel() + 1, minlength=nlist + 1)[1:]`` after
+        ``ix.search(sample, k)``, and take the most probed lists whose code bytes (ceil(len / 32) * 3072 each) fit the device memory
+        you can spare.  Raises RuntimeError, leaving the index unchanged, on a list outside the shard or too little device memory."""
+        lists = np.ascontiguousarray(np.asarray(lists, dtype=np.int64).ravel())
+        L.check(L.lib().dph_index_set_resident_lists(self._h, _np_ptr(lists), len(lists)))
+
+    def last_fetch(self):
+        """Host mode: what the last search fetched, summed over its chunks -> dict(slices, lists_fetched, blocks_fetched,
+        resident_lists_scanned, fetch_ms); fetch_ms is measured with set_profile(True) only."""
+        counts = np.zeros(4, dtype=np.int64)
+        ms = C.c_float(0)
+        L.check(L.lib().dph_index_last_fetch(self._h, _np_ptr(counts), C.byref(ms)))
+        return dict(slices=int(counts[0]), lists_fetched=int(counts[1]), blocks_fetched=int(counts[2]), resident_lists_scanned=int(counts[3]),
+                    fetch_ms=ms.value)
+
+    @property
+    def host_bytes(self):
+        """Bytes of page-locked host memory holding the codes (0 unless the codes are in host memory)."""
+        return L.lib().dph_index_host_bytes(self._h)
 
     # ---- growing the index (faiss add_with_ids, build_phrase_index.py:145-150) --------------------
     def _rows(self, x):

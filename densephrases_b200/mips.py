@@ -102,6 +102,11 @@ class MIPS(object):
         from . import artifacts, synthetic_dump
         rank, world, dev = distributed_context()
         index_dir = os.path.dirname(index_path)
+        # DPH_CODES_ON_HOST=<GiB>: keep the codes in page-locked host memory, streaming probed lists through a device region of that
+        # size (DESIGN.md 3.5), for indexes larger than the GPU.  The drivers construct MIPS without options, as with
+        # DPH_ALLOW_RANDOM_INIT.  Unset: the codes are in device memory.
+        gib = os.environ.get('DPH_CODES_ON_HOST')
+        residency = dict(codes_on_host=gib is not None, stream_bytes=int(float(gib) * (1 << 30)) if gib else None)
         container, spec = os.path.join(index_dir, 'index.dph.npz'), os.path.join(index_dir, 'index.dph.json')
         if os.path.exists(spec):                                         # synthetic index generated on the GPU(s) (synthetic_dump.py)
             sp = json.load(open(spec))['synthetic_index']
@@ -109,7 +114,7 @@ class MIPS(object):
             rng = np.random.default_rng(sp['opq_seed'])
             A = np.linalg.qr(rng.standard_normal((768, 768)))[0].astype(np.float32)
             index = ShardedIvfPq(sp['nlist'], rank=rank, world=world, device=dev)
-            index.build_synthetic(A, synthetic_dump.uniform_list_lengths(sp['N'], sp['nlist']), sp['seed'])
+            index.build_synthetic(A, synthetic_dump.uniform_list_lengths(sp['N'], sp['nlist']), sp['seed'], **residency)
         else:
             if os.path.exists(container):
                 logger.info(f'Reading {container}')
@@ -123,7 +128,7 @@ class MIPS(object):
             else:
                 raise RuntimeError(f'neither {container}, {spec} nor {index_path} found')
             index = ShardedIvfPq.from_arrays(parts['A'], parts['centroids'], parts['pq'], parts['list_len'], parts['codes'], parts.get('ids'),
-                                             rank=rank, world=world, device=dev)
+                                             rank=rank, world=world, device=dev, **residency)
         dump_root = phrase_dump_dir[:phrase_dump_dir.index('/phrase')] if '/phrase' in phrase_dump_dir else phrase_dump_dir
         doc_groups = None
         if 'PQ' in index_path:                                          # in-RAM metadata only with PQ indexes (index.py:69-74)

@@ -7,7 +7,7 @@ With world_size 1 it degenerates to IvfPqIndex.  This is the call a user (MIPS.s
 import numpy as np
 import torch
 
-from .ivfpq import IvfPqIndex, merge_shards, merge_shards_packed, pack_topk
+from .ivfpq import IvfPqIndex, default_stream_bytes, merge_shards, merge_shards_packed, pack_topk
 
 
 def shard_ranges(list_len, world):
@@ -112,7 +112,11 @@ class ShardedIvfPq:
         self._pinned_out = None
         self.query_split = None          # None: use_query_split() decides per batch; True / False force one protocol (tests, measurements)
 
-    def build_synthetic(self, A, list_len, seed, centroid_sigma=0.5, pq_sigma=0.25):
+    def _residency(self, list_len, codes_on_host, stream_bytes):
+        if codes_on_host:
+            self.local.set_code_residency(True, default_stream_bytes(list_len, *self.range) if stream_bytes is None else stream_bytes)
+
+    def build_synthetic(self, A, list_len, seed, centroid_sigma=0.5, pq_sigma=0.25, codes_on_host=False, stream_bytes=None):
         lo, hi = shard_ranges(list_len, self.world)[self.rank]
         self.range = (lo, hi)
         ix = self.local
@@ -121,13 +125,15 @@ class ShardedIvfPq:
         ix.gen_pq(seed, pq_sigma)
         if self.world > 1:
             ix.set_shard(lo, hi)
+        self._residency(list_len, codes_on_host, stream_bytes)
         ix.set_lists_synthetic(list_len, seed)
         return self
 
     @classmethod
-    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, rank=0, world=1, device=0, group=None):
+    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, rank=0, world=1, device=0, group=None, codes_on_host=False,
+                    stream_bytes=None):
         """The arrays of a faiss IndexPreTransform(OPQ) -> IndexIVFPQ file (index.py:30), list-major rows of ALL lists; this rank
-        uploads only the rows of its own list range."""
+        uploads only the rows of its own list range.  codes_on_host / stream_bytes: IvfPqIndex.from_arrays, per rank."""
         list_len = np.asarray(list_len, dtype=np.int64)
         self = cls(len(list_len), rank=rank, world=world, device=device, group=group)
         lo, hi = shard_ranges(list_len, world)[rank]
@@ -139,6 +145,7 @@ class ShardedIvfPq:
         ix.set_pq(pq)
         if world > 1:
             ix.set_shard(lo, hi)
+        self._residency(list_len, codes_on_host, stream_bytes)
         ix.set_lists(list_len, codes[off[lo]:off[hi]], None if ids is None else ids[off[lo]:off[hi]])
         return self
 
@@ -172,6 +179,12 @@ class ShardedIvfPq:
             if (s.rank, s.world) != (self.rank, self.world) or getattr(s, "range", None) != getattr(self, "range", None):
                 raise RuntimeError("merge_from: a source is sharded differently (rank, world size or list range); the index is unchanged")
         self.local.merge_from([s.local for s in sources], add_id)
+
+    def set_resident_lists(self, lists):
+        """Host mode: every rank keeps in device memory the given lists that fall in its own range (IvfPqIndex.set_resident_lists)."""
+        lists = np.asarray(lists, dtype=np.int64).ravel()
+        lo, hi = self.range
+        self.local.set_resident_lists(lists[(lists >= lo) & (lists < hi)])
 
     # ---- the slice of the faiss index API that MIPS uses (index.py:30-33,200,286,296) ----
     @property

@@ -93,6 +93,28 @@ int dph_index_get_list_len(const dph_index* ix, int64_t* list_len_out);
 /* Measurement hook: with profiling on, the stage times of the last add in ms: rotation, coarse, PQ encode, re-layout + scatter. */
 int dph_index_last_add_ms(const dph_index* ix, float* ms_out /* [4] */);
 
+/* ---- codes in host memory (DESIGN.md 3.5 "Codes in host memory") ----
+ * on_host = 1: set_lists / set_lists_synthetic put the shard's code blocks in page-locked, device-mapped host memory (same 32-row block
+ * layout); labels, direct map, list tables and model tables stay in device memory.  Device memory holds two code regions: the resident
+ * lists (dph_index_set_resident_lists) and a stream region of stream_bytes (rounded down to whole 3 KB blocks).  Each search chunk is
+ * scanned in slices: the probed lists in ascending id, a new slice whenever the next non-resident list would overflow the stream region;
+ * a slice's non-resident probed lists are copied into the stream region and scanned, and the slices' partial top-k are merged (score
+ * desc, scan position asc).  Results are bit-identical to the same index in device memory.  A search is rejected when the stream region
+ * is smaller than the shard's largest non-resident list.  Host mode costs one copy of the probes to the host and one synchronisation
+ * per search chunk.  It is read-only after set_lists: add_with_ids, remove_ids, sync_list_len and merge_from (as destination or source)
+ * are rejected with the index unchanged.  on_host must be chosen before set_lists (like set_shard); stream_bytes may be changed later
+ * (the region is reallocated, resident lists kept); on_host = 0 needs stream_bytes = 0.  set_lists drops the resident set. */
+int dph_index_set_code_residency(dph_index* ix, int on_host, int64_t stream_bytes);
+/* Host mode, after set_lists: copy lists [n] (this shard's; any order, duplicates ignored) into an exact-size device region that replaces
+ * the previous resident set (n = 0 empties it).  Rejected, with the index unchanged: a list outside [list_lo, list_hi), too little device
+ * memory for the new resident region next to the old one.  Synchronises the stream. */
+int dph_index_set_resident_lists(dph_index* ix, const int64_t* lists, int64_t n);
+/* Host mode: what the last search call fetched, summed over its chunks: counts [4] = slices, lists fetched, blocks fetched, resident
+ * lists scanned; ms (may be NULL) = time of its fetch kernels with profiling on (0 otherwise). */
+int dph_index_last_fetch(const dph_index* ix, int64_t* counts, float* ms);
+/* Bytes of page-locked host memory holding the codes (0 unless host mode). */
+int64_t dph_index_host_bytes(const dph_index* ix);
+
 /* ---- removing vectors (replaces index.remove_ids(faiss.IDSelectorBatch(ids)) / remove_ids(faiss.IDSelectorRange(lo, hi)) of faiss
  * 1.6.x IndexIVF; DESIGN.md 3.2 "Removing vectors") ----
  * Selector: the label set ids [n_ids] (mem says where it lives; any order, duplicates allowed, absent or negative labels match nothing)
@@ -174,7 +196,8 @@ int dph_index_set_scan_mode(dph_index* ix, int mode);
  * 1 (default): used when the shape allows (lists % 128 == 0, batch >= 32, nprobe + margin <= 1024); 0: always the exact SIMT GEMM. */
 int dph_index_set_coarse_tc(dph_index* ix, int on);
 int dph_index_get_opq(const dph_index* ix, float* A_out, int mem);
-/* Bytes of the index's resident arrays (model tables, lists, labels, direct map), without the per-batch workspace. */
+/* Bytes of the index's resident arrays (model tables, lists, labels, direct map; in host mode the resident and stream regions instead
+ * of the codes), without the per-batch workspace. */
 int64_t dph_index_device_bytes(const dph_index* ix);
 /* Measurement hook: when on, CUDA events bracket the scan kernel of each search (last chunk); last_scan_ms waits
  * for it and returns the kernel's duration in milliseconds (bench.py roofline). */
