@@ -84,6 +84,8 @@ _SIGS = {
     "dph_index_set_resident_lists": (_i32, [_vp, _vp, _i64]),
     "dph_index_last_fetch": (_i32, [_vp, _vp, _vp]),
     "dph_index_host_bytes": (_i64, [_vp]),
+    "dph_index_reserve_host_codes": (_i32, [_vp, _i64]),
+    "dph_index_last_host_move": (_i32, [_vp, _vp, _vp]),
     "dph_index_remove_ids": (_i32, [_vp, _vp, _i64, _i64, _i64, _i32, _vp, _vp]),
     "dph_index_sync_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_remove_ms": (_i32, [_vp, _vp]),

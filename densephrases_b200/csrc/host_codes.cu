@@ -74,6 +74,17 @@ int dph_host_lists_ready(dph_index* ix) {
     DPH_CUDA(cudaMalloc((void**)&ix->res_off_dev, nlist * 8));
     DPH_CUDA(cudaMemcpy(ix->res_off_dev, ix->res_off.data(), nlist * 8, cudaMemcpyHostToDevice));
     DPH_TRY(alloc_region(&ix->region, ix->stream_blocks, "set_lists: the stream region"));
+    ix->region_blocks = ix->stream_blocks;
+    update_max_stream_blocks(ix);
+    return 0;
+}
+
+int dph_host_after_mutation(dph_index* ix, bool shard_changed) {
+    if (shard_changed) {                           // the region keeps its size; the stream region takes all of it
+        std::fill(ix->res_off.begin(), ix->res_off.end(), (int64_t)-1);
+        ix->res_blocks = 0;
+        DPH_CUDA(cudaMemcpy(ix->res_off_dev, ix->res_off.data(), ix->nlist * 8, cudaMemcpyHostToDevice));
+    }
     update_max_stream_blocks(ix);
     return 0;
 }
@@ -94,7 +105,9 @@ DPH_API int dph_index_set_code_residency(dph_index* ix, int on_host, int64_t str
         DPH_CUDA(cudaStreamSynchronize(ix->stream));
         cudaFree(ix->region);
         ix->region = r;
+        ix->region_blocks = ix->res_blocks + sb;
     }
+    if (!on_host) { ix->host_reserve = 0; ix->host_mutable = false; }
     ix->on_host = on_host != 0;
     ix->stream_blocks = sb;
     return 0;
@@ -136,6 +149,7 @@ DPH_API int dph_index_set_resident_lists(dph_index* ix, const int64_t* lists, in
     cudaFree(ix->region);
     ix->region = r;
     ix->res_blocks = nb;
+    ix->region_blocks = nb + ix->stream_blocks;
     ix->res_off = std::move(off);
     update_max_stream_blocks(ix);
     return 0;
@@ -143,7 +157,7 @@ DPH_API int dph_index_set_resident_lists(dph_index* ix, const int64_t* lists, in
 
 int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
     cudaStream_t st = ix->stream;
-    const int64_t lo = ix->list_lo, hi = ix->list_hi, np = n * ix->nprobe, sb = ix->stream_blocks;
+    const int64_t lo = ix->list_lo, hi = ix->list_hi, np = n * ix->nprobe, sb = ix->region_blocks - ix->res_blocks;
     if (ix->max_stream_blocks > sb) {
         dph_set_error("search: the stream region holds " + std::to_string(sb) + " blocks; the largest non-resident list of the shard needs " +
                       std::to_string(ix->max_stream_blocks) + " (raise stream_bytes or make that list resident)");
@@ -226,5 +240,5 @@ DPH_API int dph_index_last_fetch(const dph_index* ix, int64_t* counts, float* ms
 }
 
 DPH_API int64_t dph_index_host_bytes(const dph_index* ix) {
-    return ix->host_codes ? std::max<int64_t>(ix->blk_cap, 1) * DPH_BLK_BYTES : 0;
+    return ix->host_codes ? std::max<int64_t>(ix->host_blocks, 1) * DPH_BLK_BYTES : 0;
 }

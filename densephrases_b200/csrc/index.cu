@@ -164,7 +164,7 @@ DPH_API int64_t dph_index_device_bytes(const dph_index* ix) {
     if (ix->pq) b += sz(DPH_M * 256 * DPH_DSUB, 4);
     if (ix->list_len) b += sz(nlist, 4) + sz(nlist + 1, 8) + sz(nlist, 8);
     if (ix->codes && !ix->host_codes) b += sz(ix->blk_cap * DPH_BLK_BYTES, 1);
-    if (ix->region) b += sz((ix->res_blocks + ix->stream_blocks) * DPH_BLK_BYTES, 1);
+    if (ix->region) b += sz(ix->region_blocks * DPH_BLK_BYTES, 1);
     if (ix->res_off_dev) b += sz(nlist, 8);
     if (ix->ids) b += sz(ix->blk_cap * 32, 8);
     if (ix->dm_ids) b += 2 * sz(ix->dm_cap, 8);

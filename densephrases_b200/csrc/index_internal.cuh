@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include "../../include/dph_b200.h"
 #include <algorithm>
+#include <functional>
 #include <string.h>
 #include <vector>
 
@@ -106,11 +107,19 @@ struct dph_index {
     int64_t remove_tmp_peak = 0;       // last remove: largest total of its temporary device allocations (bytes)
 
     // Codes in host memory (host_codes.cu, DESIGN.md 3.5).  `codes` is then the device pointer of the mapped host array host_codes,
-    // and `region` holds in HBM the resident lists' blocks [0, res_blocks), then the stream region [res_blocks, + stream_blocks).
+    // and `region` [region_blocks] holds in HBM the resident lists' blocks [0, res_blocks), then the stream region (the rest).
+    // stream_blocks is the stream size the caller asked for; a mutation that empties the resident set leaves the whole region to the
+    // stream.
     bool on_host = false;
     uint8_t* host_codes = nullptr;
     uint8_t* region = nullptr;
-    int64_t res_blocks = 0, stream_blocks = 0;
+    int64_t res_blocks = 0, stream_blocks = 0, region_blocks = 0;
+    // A reserved host capacity (host_move.cu): host_blocks = blocks allocated in host_codes (max(host_reserve, the shard's blocks) at
+    // set_lists); host_mutable = reserve_host_codes was called, so add, remove, sync_list_len and merge run in place on host_codes.
+    int64_t host_blocks = 0, host_reserve = 0;
+    bool host_mutable = false;
+    int64_t move_counts[3] = {};       // last host mutation: blocks read from and written to the host array, staging chunks
+    float move_ms = 0.f;               // last host mutation: time of the in-place block mover
     std::vector<int64_t> res_off;      // [nlist] block of a resident list in `region`, else -1
     int64_t* res_off_dev = nullptr;    // [nlist] device copy
     int64_t max_stream_blocks = 0;     // the shard's largest non-resident list, in blocks
@@ -235,6 +244,33 @@ int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
 int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
 // Host mode after set_lists: the HBM region (stream only) and the resident table (empty).
 int dph_host_lists_ready(dph_index* ix);
+// Host mode after a committed mutation: when a list of the shard changed (its length, so its blocks), the resident set empties and
+// the whole region serves as the stream region; the largest non-resident list is recomputed either way.
+int dph_host_after_mutation(dph_index* ix, bool shard_changed);
+// ---- host_move.cu ----
+// The in-place re-layout of a host index's page-locked code array (DESIGN.md 3.5, "Mutable host indexes").  prepare() allocates the
+// two HBM staging buffers (through `tmp`), streams and events before the caller changes anything.  run() rewrites destination blocks
+// [d_first, nw.nblocks) of the new layout nw from the same list's blocks of the committed layout ix->lay (whole, zeros past a list's
+// old end), in chunks of whole blocks: descending when no list moves down (add, merge), ascending when none moves up (the remove's
+// block shift).  stage(buf, c0, c1, stream), when set, writes the new rows whose destination block is in [c0, c1) into the staged
+// chunk buf (block c0 at buf[0]) before it is written back.  Every host write is then a whole-block copy-engine transfer.
+struct DphHostMover {
+    using StageFn = std::function<int(uint8_t* buf, int64_t c0, int64_t c1, cudaStream_t st)>;
+    uint8_t* buf[2] = {};
+    cudaStream_t rs = nullptr, ws = nullptr;          // the gather (read) stream and the write-back stream
+    cudaEvent_t ev[6] = {};                           // start, end, read[2], write[2]
+    int64_t chunk_blocks = 0;
+    ~DphHostMover();
+    int prepare(dph_index* ix, DevTmp& tmp, int64_t blocks, const char* oom);
+    int run(dph_index* ix, const DphLayout& nw, int64_t d_first, const long long* boff_new, bool grow, const StageFn& stage);
+};
+// The first block of layout nw whose content differs from the committed layout's (nw.nblocks when none): a list's first block when
+// it moved, else its old tail block when its length changed.
+int64_t dph_first_changed_block(const DphLayout& old, const DphLayout& nw);
+// Host mode: rejects (the index unchanged) a layout that needs more blocks than the host array holds.
+int dph_host_capacity_check(const dph_index* ix, const DphLayout& nw, const char* what);
+// Whether a list of the shard has another length in nw than in the committed layout.
+bool dph_shard_changed(const dph_index* ix, const DphLayout& nw);
 // ---- lists.cu ----
 __global__ void fill_blocks_kernel(uint8_t* codes, long long nblocks, const long long* blk_off, const int* list_len, long long list_lo,
                                    long long list_hi, const uint8_t* raw, const long long* local_row_start, uint64_t seed, long long blk0,

@@ -1,6 +1,7 @@
 // lists.cu -- the resident lists: their layout, set_lists / set_lists_synthetic, add_with_ids, copy_lists (DESIGN.md 3, 3.1).
 // remove.cu holds remove_ids and sync_list_len; both commit their layout through dph_commit_layout below.
 #include "index_internal.cuh"
+#include <limits.h>
 #include <stdlib.h>
 #include <thrust/device_ptr.h>
 #include <thrust/execution_policy.h>
@@ -115,7 +116,7 @@ void dph_free_lists(dph_index* ix) {
                      (void**)&ix->dm_ids, (void**)&ix->dm_rows, (void**)&ix->region, (void**)&ix->res_off_dev};
     for (void** p : ptrs) { if (*p) cudaFree(*p); *p = nullptr; }
     ix->blk_cap = ix->dm_cap = ix->dm_n = 0;
-    ix->res_blocks = ix->max_stream_blocks = 0;
+    ix->res_blocks = ix->max_stream_blocks = ix->region_blocks = ix->host_blocks = 0;
     ix->res_off.clear();
 }
 
@@ -131,7 +132,8 @@ static int set_lists_common(dph_index* ix, const int64_t* list_len, const uint8_
     dph_free_lists(ix);
     auto alloc = [](auto** p, int64_t count) { return cudaMalloc((void**)p, std::max<int64_t>(count, 1) * sizeof(**p)); };
     if (ix->on_host) {      // page-locked and mapped: the scan's fetch, reconstruct and copy_lists read it through its device pointer
-        DPH_CUDA(cudaHostAlloc((void**)&ix->host_codes, (size_t)std::max<int64_t>(nb, 1) * DPH_BLK_BYTES, cudaHostAllocMapped));
+        ix->host_blocks = std::max(nb, ix->host_reserve);      // a reserved capacity: spare blocks at the array's end
+        DPH_CUDA(cudaHostAlloc((void**)&ix->host_codes, (size_t)std::max<int64_t>(ix->host_blocks, 1) * DPH_BLK_BYTES, cudaHostAllocMapped));
         DPH_CUDA(cudaHostGetDevicePointer((void**)&ix->codes, ix->host_codes, 0));
     } else DPH_CUDA(alloc(&ix->codes, nb * DPH_BLK_BYTES));
     if (labels) {
@@ -269,21 +271,30 @@ __global__ void remap_dm_kernel(const long long* dm_ids_old, const long long* dm
 }
 // new row of sorted position s (rows sorted stably by list: input order inside a list) -> j = old length + rank inside the batch.
 // Its direct-map pair goes to slot dm0 + (input row), so that equal labels keep insertion order through the stable sort; rows of
-// lists outside the shard get a sentinel label that sorts past the live entries.
+// lists outside the shard get a sentinel label that sorts past the live entries.  Codes go to the rows whose block is in [w0, w1),
+// block w0 at codes_new (the whole layout: 0, LLONG_MAX; a host index's staged chunk: its blocks); labels and direct-map pairs only
+// when ids_new is set.
 __global__ void add_scatter_kernel(long long n, const long long* sorted_list, const long long* perm, const long long* bstart, const int* len_old,
                                    const long long* boff_new, long long lo, long long hi, const uint8_t* codes_all, const long long* ids_all,
-                                   uint8_t* codes_new, long long* ids_new, long long* dm_ids, long long* dm_rows, long long dm0) {
+                                   uint8_t* codes_new, long long w0, long long w1, long long* ids_new, long long* dm_ids, long long* dm_rows,
+                                   long long dm0) {
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     const long long l = sorted_list[s], r = perm[s];
-    if (l < lo || l >= hi) { dm_ids[dm0 + r] = 0x7FFFFFFFFFFFFFFFll; dm_rows[dm0 + r] = -1; return; }
+    if (l < lo || l >= hi) {
+        if (ids_new) { dm_ids[dm0 + r] = 0x7FFFFFFFFFFFFFFFll; dm_rows[dm0 + r] = -1; }
+        return;
+    }
     const long long j = (long long)len_old[l] + (s - bstart[l]);
     const long long blk = boff_new[l] + (j >> 5);
     const int lane = (int)(j & 31);
-    uint4 row4[6];
+    if (blk >= w0 && blk < w1) {
+        uint4 row4[6];
 #pragma unroll
-    for (int c = 0; c < 6; c++) row4[c] = reinterpret_cast<const uint4*>(codes_all + r * DPH_CODE)[c];
-    dph_store_row(codes_new, blk, lane, reinterpret_cast<const unsigned char*>(row4));
+        for (int c = 0; c < 6; c++) row4[c] = reinterpret_cast<const uint4*>(codes_all + r * DPH_CODE)[c];
+        dph_store_row(codes_new, blk - w0, lane, reinterpret_cast<const unsigned char*>(row4));
+    }
+    if (!ids_new) return;
     const long long id = ids_all[r];
     ids_new[blk * 32 + lane] = id;
     dm_ids[dm0 + r] = id;
@@ -293,7 +304,8 @@ __global__ void add_scatter_kernel(long long n, const long long* sorted_list, co
 DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem) {
     DPH_TRY(check_ready(ix, 1));
     DPH_CHECK(n >= 0, "add_with_ids: n must be >= 0");
-    DPH_CHECK(!ix->on_host, "add_with_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
+    if (!ix->host_mutable)          // a host index without a reserved capacity (reserve_host_codes) stays read-only
+        DPH_CHECK(!ix->on_host, "add_with_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
     if (n == 0) return 0;
     cudaStream_t st = ix->stream;
@@ -338,17 +350,23 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     }
     DphLayout L;
     DPH_TRY(L.build(ix, len_new.data(), "add_with_ids: a list would exceed 2^31 - 1 rows; the index is unchanged"));
+    DPH_TRY(dph_host_capacity_check(ix, L, "add_with_ids"));
     const DphLayout& old = ix->lay;
     const int64_t nb = L.nblocks;
     const bool was_explicit = ix->ids != nullptr;
     const int64_t dm_old = was_explicit ? ix->dm_n : ix->ntotal_local;       // pairs carried over
     const int64_t dm_cap = dm_old + n, dm_n = dm_old + (L.rows - old.rows);
 
-    // 3. every new buffer before anything changes: a failed allocation leaves the index as it was
+    // 3. every new buffer before anything changes: a failed allocation leaves the index as it was.  A host index re-lays its code
+    //    array in place (host_move.cu) through two staging buffers instead of a new code buffer.
     const char* oom2 = "add_with_ids: not enough device memory for the re-layout (the old and the new code buffers of the shard are live "
                        "together); the index is unchanged";
-    uint8_t* codes_new; int64_t *ids_new, *dm_ids_new, *dm_rows_new, *d_boff_new, *d_bstart, *d_lrs, *perm;
-    DPH_TRY(tmp.alloc(&codes_new, (size_t)nb * DPH_BLK_BYTES, oom2)); DPH_TRY(tmp.alloc(&ids_new, (size_t)nb * 32, oom2));
+    uint8_t* codes_new = nullptr; int64_t *ids_new, *dm_ids_new, *dm_rows_new, *d_boff_new, *d_bstart, *d_lrs, *perm;
+    DphHostMover mover;
+    const int64_t d_first = ix->on_host ? dph_first_changed_block(old, L) : 0;
+    if (ix->on_host) DPH_TRY(mover.prepare(ix, tmp, nb - d_first, oom2));
+    else DPH_TRY(tmp.alloc(&codes_new, (size_t)nb * DPH_BLK_BYTES, oom2));
+    DPH_TRY(tmp.alloc(&ids_new, (size_t)nb * 32, oom2));
     DPH_TRY(tmp.alloc(&dm_ids_new, dm_cap, oom2)); DPH_TRY(tmp.alloc(&dm_rows_new, dm_cap, oom2));
     DPH_TRY(tmp.alloc(&d_boff_new, nlist, oom2)); DPH_TRY(tmp.alloc(&d_bstart, nlist, oom2));
     DPH_TRY(tmp.alloc(&d_lrs, old.row_start.size(), oom2)); DPH_TRY(tmp.alloc(&perm, n, oom2));
@@ -361,7 +379,7 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[4], st));
     const long long *bo_new = (const long long*)d_boff_new, *bo_old = (const long long*)ix->blk_off;
     if (nb > 0) {
-        relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, 0, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
+        if (!ix->on_host) relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, 0, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
         relayout_ids_kernel<<<(unsigned)nb, 32, 0, st>>>((long long*)ids_new, 0, bo_new, bo_old, ix->list_len, lo, hi, (const long long*)ix->ids,
                                                        (const long long*)ix->list_start, (const long long*)d_lrs, (long long*)dm_ids_new,
                                                        (long long*)dm_rows_new);
@@ -376,7 +394,8 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
         thrust::stable_sort_by_key(thrust::cuda::par.on(st), kp, kp + n, pp);
         add_scatter_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(n, (const long long*)list_all, (const long long*)perm, (const long long*)d_bstart,
                                                                        ix->list_len, bo_new, lo, hi, codes_all, (const long long*)ids_all, codes_new,
-                                                                       (long long*)ids_new, (long long*)dm_ids_new, (long long*)dm_rows_new, dm_old);
+                                                                       0, ix->on_host ? 0 : LLONG_MAX, (long long*)ids_new, (long long*)dm_ids_new,
+                                                                       (long long*)dm_rows_new, dm_old);
         DPH_CUDA(cudaGetLastError());
         thrust::device_ptr<long long> dk((long long*)dm_ids_new), dv((long long*)dm_rows_new);
         thrust::stable_sort_by_key(thrust::cuda::par.on(st), dk, dk + dm_cap, dv);       // equal labels keep insertion order
@@ -385,16 +404,27 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
         dph_set_error(std::string("add_with_ids: device sort failed; the index is unchanged: ") + e.what());
         return 1;
     }
+    if (ix->on_host)        // the old blocks move up in place; each staged chunk receives the new rows that land in it
+        DPH_TRY(mover.run(ix, L, d_first, bo_new, true, [&](uint8_t* buf, int64_t c0, int64_t c1, cudaStream_t rs) {
+            add_scatter_kernel<<<(unsigned)((n + 127) / 128), 128, 0, rs>>>(n, (const long long*)list_all, (const long long*)perm,
+                                                                            (const long long*)d_bstart, ix->list_len, bo_new, lo, hi, codes_all,
+                                                                            (const long long*)ids_all, buf, c0, c1, nullptr, nullptr, nullptr, 0);
+            DPH_CUDA(cudaGetLastError());
+            return 0;
+        }));
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[5], st));
     DPH_CUDA(cudaStreamSynchronize(st));
 
-    // 5. commit: tables, then the buffers
+    // 5. commit: tables, then the buffers (a host index keeps its code array)
+    const bool shard_changed = dph_shard_changed(ix, L);
     DPH_TRY(dph_commit_layout(ix, std::move(L)));
-    void* olds[] = {ix->codes, ix->ids, ix->dm_ids, ix->dm_rows};
+    void* olds[] = {ix->on_host ? nullptr : ix->codes, ix->ids, ix->dm_ids, ix->dm_rows};
     for (void* p : olds) if (p) cudaFree(p);
-    ix->codes = codes_new; ix->ids = ids_new; ix->dm_ids = dm_ids_new; ix->dm_rows = dm_rows_new;
+    if (!ix->on_host) ix->codes = codes_new;
+    ix->ids = ids_new; ix->dm_ids = dm_ids_new; ix->dm_rows = dm_rows_new;
     for (void* p : {(void*)codes_new, (void*)ids_new, (void*)dm_ids_new, (void*)dm_rows_new}) tmp.release(p);
     ix->dm_n = dm_n; ix->dm_cap = dm_cap; ix->blk_cap = nb;
+    if (ix->on_host) DPH_TRY(dph_host_after_mutation(ix, shard_changed));
     if (prof) DPH_CUDA(cudaEventElapsedTime(&ix->add_ms[3], ix->aev[4], ix->aev[5]));
     return 0;
 }

@@ -5,6 +5,7 @@
 // copies that source's rows into place, re-rotated for their new lane; the direct maps, each sorted by label, are merged, not
 // re-sorted.  The result is byte-identical to set_lists of the concatenated list-major arrays.
 #include "index_internal.cuh"
+#include <limits.h>
 #include <thrust/execution_policy.h>
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
@@ -19,22 +20,27 @@ __global__ void tables_differ_kernel(const uint32_t* a, const uint32_t* b, long 
 // One warp per block of a source's shard, lane = the row's lane there.  Row j of list l lands at j + base[l - lo] of the same list in
 // the new layout (base = this index's old length of l plus the earlier sources' lengths of l), re-rotated for its new lane; its label
 // is the stored one (sequential: list_start_src[l] + j) plus add_id.  A source with sequential labels also writes each row's
-// direct-map pair at the row's local position, which is label order; an explicit-label source's pairs come from its own map.
+// direct-map pair at the row's local position, which is label order; an explicit-label source's pairs come from its own map.  Codes
+// go to the rows whose new block is in [w0, w1), block w0 at codes_new (the whole layout: 0, LLONG_MAX; a host index's staged chunk:
+// its blocks); labels and direct-map pairs only when ids_new is set.
 __global__ void __launch_bounds__(256) merge_rows_kernel(long long nb_src, const long long* boff_src, const int* len_src, const uint8_t* codes_src,
                                                          const long long* ids_src, const long long* list_start_src, const long long* lrs_src,
                                                          long long lo, long long hi, const long long* base, const long long* boff_new,
-                                                         long long add_id, uint8_t* codes_new, long long* ids_new, long long* dm_ids,
-                                                         long long* dm_rows) {
+                                                         long long add_id, uint8_t* codes_new, long long w0, long long w1, long long* ids_new,
+                                                         long long* dm_ids, long long* dm_rows) {
     const long long b = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int lane = threadIdx.x & 31;
     if (b >= nb_src) return;
     const long long l = list_of_block(boff_src, lo, hi, b);
     const long long j = (b - boff_src[l]) * 32 + lane;
     if (j >= (long long)len_src[l]) return;
-    unsigned char row[DPH_CODE];
-    dph_load_row(codes_src, b, lane, row);
     const long long prow = boff_new[l] * 32 + base[l - lo] + j;          // the new list's blocks are consecutive
-    dph_store_row(codes_new, prow >> 5, (int)(prow & 31), row);
+    if ((prow >> 5) >= w0 && (prow >> 5) < w1) {
+        unsigned char row[DPH_CODE];
+        dph_load_row(codes_src, b, lane, row);
+        dph_store_row(codes_new, (prow >> 5) - w0, (int)(prow & 31), row);
+    }
+    if (!ids_new) return;
     const long long id = (ids_src ? ids_src[b * 32 + lane] : list_start_src[l] + j) + add_id;
     ids_new[prow] = id;
     if (!ids_src) {
@@ -88,7 +94,8 @@ static bool label_ok(int64_t v, int64_t add_id) {
 DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int n_src, int64_t add_id) {
     DPH_TRY(check_ready(ix, 1));
     DPH_CHECK(n_src >= 0 && (src != nullptr || n_src == 0), "merge_from: bad source list; the index is unchanged");
-    DPH_CHECK(!ix->on_host, "merge_from: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
+    if (!ix->host_mutable)          // a host index without a reserved capacity (reserve_host_codes) stays read-only
+        DPH_CHECK(!ix->on_host, "merge_from: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
     for (float& a : ix->merge_ms) a = 0.f;
     cudaStream_t st = ix->stream;
@@ -156,14 +163,20 @@ DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int
         }
     DphLayout L;
     DPH_TRY(L.build(ix, len_new.data(), "merge_from: a list would exceed 2^31 - 1 rows; the index is unchanged"));
+    DPH_TRY(dph_host_capacity_check(ix, L, "merge_from"));
     const int64_t nb = L.nblocks, nsb = std::max<int64_t>(ns, 1);
     const bool was_explicit = ix->ids != nullptr;
     const int64_t dm_dest = was_explicit ? ix->dm_n : ix->ntotal_local, dm_n = dm_dest + src_local;
 
-    // 3. every buffer before anything changes: a failed allocation leaves the index as it was
-    uint8_t* codes_new; int64_t *ids_new, *dm_ids_new, *dm_rows_new, *d_boff_new, *d_base, *d_lrs, *xk, *xv, *yk = nullptr, *yv = nullptr,
-                                *zk = nullptr, *zv = nullptr;
-    DPH_TRY(tmp.alloc(&codes_new, (size_t)nb * DPH_BLK_BYTES, oom)); DPH_TRY(tmp.alloc(&ids_new, (size_t)nb * 32, oom));
+    // 3. every buffer before anything changes: a failed allocation leaves the index as it was.  A host index re-lays its code array in
+    //    place (host_move.cu) through two staging buffers instead of a new code buffer.
+    uint8_t* codes_new = nullptr;
+    int64_t *ids_new, *dm_ids_new, *dm_rows_new, *d_boff_new, *d_base, *d_lrs, *xk, *xv, *yk = nullptr, *yv = nullptr, *zk = nullptr, *zv = nullptr;
+    DphHostMover mover;
+    const int64_t d_first = ix->on_host ? dph_first_changed_block(old, L) : 0;
+    if (ix->on_host) DPH_TRY(mover.prepare(ix, tmp, nb - d_first, oom));
+    else DPH_TRY(tmp.alloc(&codes_new, (size_t)nb * DPH_BLK_BYTES, oom));
+    DPH_TRY(tmp.alloc(&ids_new, (size_t)nb * 32, oom));
     DPH_TRY(tmp.alloc(&dm_ids_new, dm_n, oom)); DPH_TRY(tmp.alloc(&dm_rows_new, dm_n, oom));
     DPH_TRY(tmp.alloc(&d_boff_new, nlist, oom)); DPH_TRY(tmp.alloc(&d_base, base.size(), oom));
     DPH_TRY(tmp.alloc(&d_lrs, (size_t)(n_src + 1) * nsb, oom));        // [0]: this index's local row starts, [1 + s]: source s's
@@ -181,7 +194,7 @@ DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int
     // 4. this index's blocks move whole (zeros and label -1 past each list's old end)
     const long long *bo_new = (const long long*)d_boff_new, *bo_old = (const long long*)ix->blk_off;
     if (nb > 0) {
-        relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, 0, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
+        if (!ix->on_host) relayout_codes_kernel<<<(unsigned)nb, 192, 0, st>>>(codes_new, 0, bo_new, bo_old, ix->list_len, lo, hi, ix->codes);
         relayout_ids_kernel<<<(unsigned)nb, 32, 0, st>>>((long long*)ids_new, 0, bo_new, bo_old, ix->list_len, lo, hi, (const long long*)ix->ids,
                                                        (const long long*)ix->list_start, nullptr, nullptr, nullptr);
     }
@@ -197,7 +210,7 @@ DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int
         merge_rows_kernel<<<(unsigned)((o->nblocks_local * 32 + 255) / 256), 256, 0, st>>>(
             o->nblocks_local, (const long long*)o->blk_off, o->list_len, o->codes, (const long long*)o->ids, (const long long*)o->list_start,
             (const long long*)(d_lrs + (size_t)(s + 1) * nsb), lo, hi, (const long long*)(d_base + (size_t)s * nsb), bo_new, add_id, codes_new,
-            (long long*)ids_new, (long long*)(xk + xoff[s]), (long long*)(xv + xoff[s]));
+            0, ix->on_host ? 0 : LLONG_MAX, (long long*)ids_new, (long long*)(xk + xoff[s]), (long long*)(xv + xoff[s]));
     }
     DPH_CUDA(cudaGetLastError());
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[3], st));
@@ -235,16 +248,34 @@ DPH_API int dph_index_merge_from(dph_index* ix, const dph_index* const* src, int
         return 1;
     }
     DPH_CUDA(cudaGetLastError());
+    // 7. a host index: the old blocks move up in place, each staged chunk receiving every source's rows that land in it.  Last, after
+    //    the device merge that may still fail with the index unchanged (its time is in the direct-map stage and in last_host_move).
+    if (ix->on_host)
+        DPH_TRY(mover.run(ix, L, d_first, bo_new, true, [&](uint8_t* buf, int64_t c0, int64_t c1, cudaStream_t rs) {
+            for (int s = 0; s < n_src; s++) {
+                const dph_index* o = src[s];
+                if (o->nblocks_local == 0) continue;
+                merge_rows_kernel<<<(unsigned)((o->nblocks_local * 32 + 255) / 256), 256, 0, rs>>>(
+                    o->nblocks_local, (const long long*)o->blk_off, o->list_len, o->codes, (const long long*)o->ids, (const long long*)o->list_start,
+                    (const long long*)(d_lrs + (size_t)(s + 1) * nsb), lo, hi, (const long long*)(d_base + (size_t)s * nsb), bo_new, add_id, buf,
+                    c0, c1, nullptr, nullptr, nullptr);
+            }
+            DPH_CUDA(cudaGetLastError());
+            return 0;
+        }));
     if (prof) DPH_CUDA(cudaEventRecord(ix->aev[4], st));
     DPH_CUDA(cudaStreamSynchronize(st));
 
-    // 7. commit: the layout, then the buffers
+    // 8. commit: the layout, then the buffers (a host index keeps its code array)
+    const bool shard_changed = dph_shard_changed(ix, L);
     DPH_TRY(dph_commit_layout(ix, std::move(L)));
-    void* olds[] = {ix->codes, ix->ids, ix->dm_ids, ix->dm_rows};
+    void* olds[] = {ix->on_host ? nullptr : ix->codes, ix->ids, ix->dm_ids, ix->dm_rows};
     for (void* p : olds) if (p) cudaFree(p);
-    ix->codes = codes_new; ix->ids = ids_new; ix->dm_ids = dm_ids_new; ix->dm_rows = dm_rows_new;
+    if (!ix->on_host) ix->codes = codes_new;
+    ix->ids = ids_new; ix->dm_ids = dm_ids_new; ix->dm_rows = dm_rows_new;
     for (void* p : {(void*)codes_new, (void*)ids_new, (void*)dm_ids_new, (void*)dm_rows_new}) tmp.release(p);
     ix->dm_n = ix->dm_cap = dm_n; ix->blk_cap = nb;
+    if (ix->on_host) DPH_TRY(dph_host_after_mutation(ix, shard_changed));
     if (prof)
         for (int s = 0; s < 4; s++) DPH_CUDA(cudaEventElapsedTime(&ix->merge_ms[s], ix->aev[s], ix->aev[s + 1]));
     return 0;

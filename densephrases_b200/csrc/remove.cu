@@ -124,7 +124,8 @@ __global__ void rm_dm_gather_kernel(long long d0, long long n, const long long* 
 DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_ids, int64_t range_lo, int64_t range_hi, int mem,
                                  int64_t* n_removed_out, int64_t* removed_per_list_out) {
     DPH_CHECK(ix && ix->list_len, "remove_ids: lists are not set");
-    DPH_CHECK(!ix->on_host, "remove_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
+    if (!ix->host_mutable)          // a host index without a reserved capacity (reserve_host_codes) stays read-only
+        DPH_CHECK(!ix->on_host, "remove_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CHECK(n_ids >= 0, "remove_ids: n_ids must be >= 0; the index is unchanged");
     DPH_CHECK(!(ids && (range_lo != 0 || range_hi != 0)), "remove_ids: give a label set or a label range, not both; the index is unchanged");
     DPH_CHECK(ids || n_ids == 0, "remove_ids: n_ids > 0 without labels; the index is unchanged");
@@ -239,8 +240,10 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     const int64_t chunk_pairs = std::max<int64_t>(1, std::min(max_blocks * (DPH_BLK_BYTES + 256) / 16, dm_new));
     const int64_t stage_bytes = std::max(chunk_blocks * (DPH_BLK_BYTES + 256), chunk_pairs * 16);
     uint8_t* stage = nullptr;
+    DphHostMover mover;             // a host index shifts its code blocks through the mover's two buffers (host_move.cu)
     if (R > 0) {
         DPH_TRY(tmp.alloc(&stage, (size_t)stage_bytes, oom));
+        if (ix->on_host) DPH_TRY(mover.prepare(ix, tmp, nb_new - d_first, oom));
         DPH_CUDA(cudaMemcpyAsync(d_boff_new, L.blk_off.data(), nlist * 8, cudaMemcpyHostToDevice, st));
         DPH_CUDA(cudaMemcpyAsync(d_rm_off, rm_off.data(), nlist * 8, cudaMemcpyHostToDevice, st));
         rm_plan_moves_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(rm_prow, R, bo, ix->list_len, d_cnt, d_rm_off, lo, hi, mv_src, mv_dst);
@@ -258,22 +261,25 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     // Every allocation is done: from here on the index changes.
 
     if (R > 0) {
-        // 3. fill the holes, clear the tails (old layout)
+        // 3. fill the holes, clear the tails (old layout; on a host index row by row over mapped memory: R rows, not the array)
         rm_fill_holes_kernel<<<(unsigned)((R + 127) / 128), 128, 0, st>>>(mv_src, mv_dst, R, ix->codes, w_ids);
         rm_clear_tail_kernel<<<(unsigned)(hi - lo), 32, 0, st>>>(bo, ix->list_len, d_cnt, lo, ix->codes, w_ids);
         DPH_CUDA(cudaGetLastError());
         // 4. shift blocks [d_first, nb_new) down, ascending, one staged chunk at a time: every source is at or above its destination,
-        //    so a chunk's writes land below the sources of every later chunk
+        //    so a chunk's writes land below the sources of every later chunk.  A host index shifts its codes with the mover, its labels here.
         uint8_t* st_codes = stage;
         long long* st_ids = (long long*)(stage + chunk_blocks * DPH_BLK_BYTES);
         for (int64_t d0 = d_first; d0 < nb_new; d0 += chunk_blocks) {
             const int64_t m = std::min(chunk_blocks, nb_new - d0);
-            relayout_codes_kernel<<<(unsigned)m, 192, 0, st>>>(st_codes, d0, d_boff_new, bo, ix->list_len, lo, hi, ix->codes);
+            if (!ix->on_host)
+                relayout_codes_kernel<<<(unsigned)m, 192, 0, st>>>(st_codes, d0, d_boff_new, bo, ix->list_len, lo, hi, ix->codes);
             relayout_ids_kernel<<<(unsigned)m, 32, 0, st>>>(st_ids, d0, d_boff_new, bo, ix->list_len, lo, hi, w_ids, nullptr, nullptr, nullptr, nullptr);
             DPH_CUDA(cudaGetLastError());
-            DPH_CUDA(cudaMemcpyAsync(ix->codes + d0 * DPH_BLK_BYTES, st_codes, (size_t)m * DPH_BLK_BYTES, cudaMemcpyDeviceToDevice, st));
+            if (!ix->on_host)
+                DPH_CUDA(cudaMemcpyAsync(ix->codes + d0 * DPH_BLK_BYTES, st_codes, (size_t)m * DPH_BLK_BYTES, cudaMemcpyDeviceToDevice, st));
             DPH_CUDA(cudaMemcpyAsync(w_ids + d0 * 32, st_ids, (size_t)m * 256, cudaMemcpyDeviceToDevice, st));
         }
+        if (ix->on_host) DPH_TRY(mover.run(ix, L, d_first, d_boff_new, false, nullptr));
         if (prof) DPH_CUDA(cudaEventRecord(ix->aev[2], st));
         // 5. direct map: stable in-place compaction, rows remapped, through the same staging buffer
         long long *st_dm_ids = (long long*)stage, *st_dm_rows = (long long*)stage + chunk_pairs;
@@ -297,6 +303,7 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     }
     if (R > 0) DPH_TRY(dph_commit_layout(ix, std::move(L)));
     ix->dm_n = dm_new;
+    if (ix->on_host && R > 0) DPH_TRY(dph_host_after_mutation(ix, true));
     ix->remove_tmp_peak = tmp.peak;
     if (prof)
         for (int s = 0; s < 3; s++) DPH_CUDA(cudaEventElapsedTime(&ix->remove_ms[s], ix->aev[s], ix->aev[s + 1]));
@@ -307,7 +314,8 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
 
 DPH_API int dph_index_sync_list_len(dph_index* ix, const int64_t* list_len) {
     DPH_CHECK(ix && ix->list_len, "sync_list_len: lists are not set");
-    DPH_CHECK(!ix->on_host, "sync_list_len: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
+    if (!ix->host_mutable)          // a host index without a reserved capacity (reserve_host_codes) stays read-only
+        DPH_CHECK(!ix->on_host, "sync_list_len: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DphLayout L;
     DPH_TRY(L.build(ix, list_len, "sync_list_len: bad list length; the index is unchanged"));
     bool changed = false;

@@ -34,10 +34,14 @@ class IvfPqIndex:
             L._lib.dph_index_free(h)
 
     @classmethod
-    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, device=0, shard=None, codes_on_host=False, stream_bytes=None):
+    def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, device=0, shard=None, codes_on_host=False, stream_bytes=None,
+                    host_capacity_bytes=None):
         """Build from the arrays a faiss IndexPreTransform(OPQ)->IndexIVFPQ file holds (index.py:30).  codes_on_host: keep the codes in
         page-locked host memory and stream the probed lists through a device region of stream_bytes (None: default_stream_bytes);
-        see set_code_residency."""
+        see set_code_residency.  host_capacity_bytes (host mode only): reserve that much page-locked memory for the codes, which makes
+        the index mutable; see reserve_host_codes."""
+        if host_capacity_bytes is not None and not codes_on_host:
+            raise ValueError("host_capacity_bytes needs codes_on_host=True")
         ix = cls(len(list_len), device=device)
         ix.set_opq(A)
         ix.set_centroids(centroids)
@@ -46,6 +50,8 @@ class IvfPqIndex:
             ix.set_shard(*shard)
         if codes_on_host:
             ix.set_code_residency(True, default_stream_bytes(list_len, *(shard or (0, None))) if stream_bytes is None else stream_bytes)
+            if host_capacity_bytes is not None:
+                ix.reserve_host_codes(host_capacity_bytes)
         ix.set_lists(list_len, codes, ids)
         return ix
 
@@ -89,14 +95,17 @@ class IvfPqIndex:
     def set_code_residency(self, on_host, stream_bytes=0):
         """on_host=True (before set_lists): the codes live in page-locked host memory; every search copies the probed lists that are
         not resident into a device stream region of stream_bytes, slice by slice, with results bit-identical to a device-resident
-        index.  stream_bytes may be changed later.  The index is then read-only: add, remove and merge raise RuntimeError."""
+        index.  stream_bytes may be changed later.  The index is then read-only (add, remove, sync_list_len and merge raise
+        RuntimeError) unless a host capacity is reserved with reserve_host_codes; it is never a merge source."""
         L.check(L.lib().dph_index_set_code_residency(self._h, int(bool(on_host)), int(stream_bytes)))
 
     def set_resident_lists(self, lists):
         """Host mode: keep these lists of this shard in device memory (replaces the previous set; [] empties it).  To choose them,
         count the probes of a sample search: ``np.bincount(ix.last_probes(n).ravel() + 1, minlength=nlist + 1)[1:]`` after
         ``ix.search(sample, k)``, and take the most probed lists whose code bytes (ceil(len / 32) * 3072 each) fit the device memory
-        you can spare.  Raises RuntimeError, leaving the index unchanged, on a list outside the shard or too little device memory."""
+        you can spare.  Raises RuntimeError, leaving the index unchanged, on a list outside the shard or too little device memory.
+        An add, remove or merge that changes a list of this shard empties the resident set: the region keeps its device memory and
+        serves as the stream region (every list streams) until this is called again."""
         lists = np.ascontiguousarray(np.asarray(lists, dtype=np.int64).ravel())
         L.check(L.lib().dph_index_set_resident_lists(self._h, _np_ptr(lists), len(lists)))
 
@@ -113,6 +122,25 @@ class IvfPqIndex:
     def host_bytes(self):
         """Bytes of page-locked host memory holding the codes (0 unless the codes are in host memory)."""
         return L.lib().dph_index_host_bytes(self._h)
+
+    def reserve_host_codes(self, nbytes):
+        """Host mode: reserve a page-locked capacity of nbytes for the codes (rounded down to whole 3 KB blocks; it never shrinks) and
+        make the index mutable.  add_with_ids / add, remove_ids, sync_list_len and merge_from (from device-resident sources) then give
+        exactly what they give on a device-resident index, re-laying the host array in place through two device staging buffers of at
+        most ~256 MB; an add or merge that needs more than the capacity raises RuntimeError, the index unchanged.  Host memory stays
+        the capacity the caller chose.  Before set_lists, set_lists allocates max(capacity, what the lists need).  After it, a larger
+        capacity allocates a new array, copies the codes and frees the old one (the one time two host arrays exist; if the allocation
+        fails, RuntimeError and the index is unchanged); a capacity at or below host_bytes only makes the index mutable.  A mutation
+        that changes a list of this shard empties the resident set (see set_resident_lists)."""
+        L.check(L.lib().dph_index_reserve_host_codes(self._h, int(nbytes)))
+
+    def last_host_move(self):
+        """Host mode: the in-place block mover of the last add, remove or merge -> dict(blocks_read, blocks_written, chunks, ms): 3 KB
+        blocks gathered from and written back to the host array, staging chunks, and its time (first gather to last write-back)."""
+        counts = np.zeros(3, dtype=np.int64)
+        ms = C.c_float(0)
+        L.check(L.lib().dph_index_last_host_move(self._h, _np_ptr(counts), C.byref(ms)))
+        return dict(blocks_read=int(counts[0]), blocks_written=int(counts[1]), chunks=int(counts[2]), ms=ms.value)
 
     # ---- growing the index (faiss add_with_ids, build_phrase_index.py:145-150) --------------------
     def _rows(self, x):
@@ -142,7 +170,8 @@ class IvfPqIndex:
     def add_with_ids(self, x, ids):
         """== faiss index.add_with_ids(x, ids): append x [n,d] (numpy or torch cuda) with labels ids [n] (None: ntotal + arange(n))
         to their lists, in input order.  Raises RuntimeError, leaving the index unchanged, on a negative label, a non-finite value,
-        a shape mismatch or too little device memory for the re-layout."""
+        a shape mismatch or too little device memory for the re-layout.  A host-mode index needs a reserved host capacity
+        (reserve_host_codes) that holds the new layout."""
         if isinstance(x, np.ndarray):
             x = np.ascontiguousarray(x, dtype=np.float32)
             n = self._rows(x)
@@ -217,7 +246,8 @@ class IvfPqIndex:
 
     def remove_ids(self, sel):
         """== faiss index.remove_ids(IDSelectorBatch(sel)) for a label array, index.remove_ids(IDSelectorRange(lo, hi)) for
-        range(lo, hi) -> the number of rows removed (on a shard: from this shard)."""
+        range(lo, hi) -> the number of rows removed (on a shard: from this shard).  A host-mode index needs a reserved host capacity
+        (reserve_host_codes); the array is compacted in place."""
         return int(self.remove_ids_per_list(sel).sum())
 
     def list_len(self):
@@ -227,7 +257,8 @@ class IvfPqIndex:
         return out
 
     def sync_list_len(self, list_len):
-        """Sharded remove: set the lengths of the other shards' lists (this shard's entries must equal its own)."""
+        """Sharded remove: set the lengths of the other shards' lists (this shard's entries must equal its own).  A host-mode index
+        needs a reserved host capacity (reserve_host_codes)."""
         list_len = np.ascontiguousarray(list_len, dtype=np.int64)
         assert list_len.shape == (self.nlist,)
         L.check(L.lib().dph_index_sync_list_len(self._h, _np_ptr(list_len)))
@@ -248,7 +279,8 @@ class IvfPqIndex:
         of that list behind its own, labels shifted by add_id.  The sources are not modified (faiss empties `other`).  Raises
         RuntimeError, leaving the index unchanged, on an incompatible source (d, nlist, device, shard range, or any bit of the OPQ
         matrix, centroids or PQ codebooks), the index itself as a source, a label + add_id outside [0, 2^63) or too little device
-        memory.  Sources with no rows make it a no-op."""
+        memory.  Sources with no rows make it a no-op.  Into a host-mode index with a reserved host capacity (reserve_host_codes) from
+        device-resident sources: rejected, unchanged, when the merged layout exceeds the capacity; a host-mode source is rejected."""
         sources = [sources] if isinstance(sources, IvfPqIndex) else list(sources)
         for s in sources:
             if not isinstance(s, IvfPqIndex):

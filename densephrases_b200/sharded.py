@@ -112,11 +112,16 @@ class ShardedIvfPq:
         self._pinned_out = None
         self.query_split = None          # None: use_query_split() decides per batch; True / False force one protocol (tests, measurements)
 
-    def _residency(self, list_len, codes_on_host, stream_bytes):
+    def _residency(self, list_len, codes_on_host, stream_bytes, host_capacity_bytes):
+        if host_capacity_bytes is not None and not codes_on_host:
+            raise ValueError("host_capacity_bytes needs codes_on_host=True")
         if codes_on_host:
             self.local.set_code_residency(True, default_stream_bytes(list_len, *self.range) if stream_bytes is None else stream_bytes)
+            if host_capacity_bytes is not None:
+                self.local.reserve_host_codes(host_capacity_bytes)
 
-    def build_synthetic(self, A, list_len, seed, centroid_sigma=0.5, pq_sigma=0.25, codes_on_host=False, stream_bytes=None):
+    def build_synthetic(self, A, list_len, seed, centroid_sigma=0.5, pq_sigma=0.25, codes_on_host=False, stream_bytes=None,
+                        host_capacity_bytes=None):
         lo, hi = shard_ranges(list_len, self.world)[self.rank]
         self.range = (lo, hi)
         ix = self.local
@@ -125,15 +130,16 @@ class ShardedIvfPq:
         ix.gen_pq(seed, pq_sigma)
         if self.world > 1:
             ix.set_shard(lo, hi)
-        self._residency(list_len, codes_on_host, stream_bytes)
+        self._residency(list_len, codes_on_host, stream_bytes, host_capacity_bytes)
         ix.set_lists_synthetic(list_len, seed)
         return self
 
     @classmethod
     def from_arrays(cls, A, centroids, pq, list_len, codes, ids=None, rank=0, world=1, device=0, group=None, codes_on_host=False,
-                    stream_bytes=None):
+                    stream_bytes=None, host_capacity_bytes=None):
         """The arrays of a faiss IndexPreTransform(OPQ) -> IndexIVFPQ file (index.py:30), list-major rows of ALL lists; this rank
-        uploads only the rows of its own list range.  codes_on_host / stream_bytes: IvfPqIndex.from_arrays, per rank."""
+        uploads only the rows of its own list range.  codes_on_host / stream_bytes / host_capacity_bytes: IvfPqIndex.from_arrays, per
+        rank (host_capacity_bytes is this rank's capacity)."""
         list_len = np.asarray(list_len, dtype=np.int64)
         self = cls(len(list_len), rank=rank, world=world, device=device, group=group)
         lo, hi = shard_ranges(list_len, world)[rank]
@@ -145,7 +151,7 @@ class ShardedIvfPq:
         ix.set_pq(pq)
         if world > 1:
             ix.set_shard(lo, hi)
-        self._residency(list_len, codes_on_host, stream_bytes)
+        self._residency(list_len, codes_on_host, stream_bytes, host_capacity_bytes)
         ix.set_lists(list_len, codes[off[lo]:off[hi]], None if ids is None else ids[off[lo]:off[hi]])
         return self
 
@@ -179,6 +185,11 @@ class ShardedIvfPq:
             if (s.rank, s.world) != (self.rank, self.world) or getattr(s, "range", None) != getattr(self, "range", None):
                 raise RuntimeError("merge_from: a source is sharded differently (rank, world size or list range); the index is unchanged")
         self.local.merge_from([s.local for s in sources], add_id)
+
+    def reserve_host_codes(self, nbytes):
+        """Host mode: every rank reserves a host capacity of nbytes for its own shard (IvfPqIndex.reserve_host_codes), which makes
+        add_with_ids, remove_ids and merge_from run in place on its page-locked array."""
+        self.local.reserve_host_codes(nbytes)
 
     def set_resident_lists(self, lists):
         """Host mode: every rank keeps in device memory the given lists that fall in its own range (IvfPqIndex.set_resident_lists)."""

@@ -83,7 +83,8 @@ int dph_index_encode(dph_index* ix, const float* x, int64_t n, int64_t* list_no_
  * that adds the same batch reaches the same global state.  An index with sequential labels turns them into explicit ones.  A label
  * added twice is found at every row that carries it; reconstruct returns the most recent row (faiss' hashtable direct map), except
  * for a label repeated across shards, which reconstruct leaves undefined.  Rejected, with the index unchanged: a negative label, a
- * non-finite input value, too little device memory for the old and the new code buffers at once.  Synchronises the stream. */
+ * non-finite input value, too little device memory for the old and the new code buffers at once (a host index with a reserved
+ * capacity: for two staging buffers), a host index whose capacity the new layout exceeds.  Synchronises the stream. */
 int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem);
 /* This shard's lists as list-major host arrays: codes_out [ntotal_local,96], ids_out [ntotal_local] (may be NULL); the inverse of
  * set_lists, for writing a grown index back to a faiss file (artifacts.write_faiss_index). */
@@ -101,9 +102,10 @@ int dph_index_last_add_ms(const dph_index* ix, float* ms_out /* [4] */);
  * a slice's non-resident probed lists are copied into the stream region and scanned, and the slices' partial top-k are merged (score
  * desc, scan position asc).  Results are bit-identical to the same index in device memory.  A search is rejected when the stream region
  * is smaller than the shard's largest non-resident list.  Host mode costs one copy of the probes to the host and one synchronisation
- * per search chunk.  It is read-only after set_lists: add_with_ids, remove_ids, sync_list_len and merge_from (as destination or source)
- * are rejected with the index unchanged.  on_host must be chosen before set_lists (like set_shard); stream_bytes may be changed later
- * (the region is reallocated, resident lists kept); on_host = 0 needs stream_bytes = 0.  set_lists drops the resident set. */
+ * per search chunk.  Without a reserved host capacity (dph_index_reserve_host_codes) it is read-only after set_lists: add_with_ids,
+ * remove_ids, sync_list_len and merge_from are rejected with the index unchanged; it is never a merge source.  on_host must be chosen
+ * before set_lists (like set_shard); stream_bytes may be changed later (the region is reallocated, resident lists kept); on_host = 0
+ * needs stream_bytes = 0.  set_lists drops the resident set. */
 int dph_index_set_code_residency(dph_index* ix, int on_host, int64_t stream_bytes);
 /* Host mode, after set_lists: copy lists [n] (this shard's; any order, duplicates ignored) into an exact-size device region that replaces
  * the previous resident set (n = 0 empties it).  Rejected, with the index unchanged: a list outside [list_lo, list_hi), too little device
@@ -114,6 +116,18 @@ int dph_index_set_resident_lists(dph_index* ix, const int64_t* lists, int64_t n)
 int dph_index_last_fetch(const dph_index* ix, int64_t* counts, float* ms);
 /* Bytes of page-locked host memory holding the codes (0 unless host mode). */
 int64_t dph_index_host_bytes(const dph_index* ix);
+/* Host mode: reserve a host capacity of bytes (rounded down to whole 3 KB blocks), which makes the index mutable.  add_with_ids,
+ * remove_ids, sync_list_len and merge_from (from device-resident sources) then behave exactly as on a device-resident index, re-laying
+ * the page-locked array in place through two HBM staging buffers (DESIGN.md 3.5 "Mutable host indexes"); an add or merge whose layout
+ * needs more than the capacity is rejected with the index unchanged.  A mutation that changes a list of the shard empties the
+ * resident set: the region keeps its size and serves as the stream region until dph_index_set_resident_lists is called again.
+ * Before set_lists: set_lists allocates max(capacity, its blocks).  After: a larger capacity allocates a new page-locked array, copies
+ * the blocks and frees the old one (the only time two host arrays exist; rejected with the index unchanged if the allocation fails);
+ * a capacity at or below the allocation only makes the index mutable.  The capacity never shrinks.  Synchronises the stream. */
+int dph_index_reserve_host_codes(dph_index* ix, int64_t bytes);
+/* Host mode, measurement hook: the last add, remove or merge's in-place block mover: counts [3] = blocks read from the host array,
+ * blocks written to it, staging chunks; ms (may be NULL) = its time from the first gather to the last write-back. */
+int dph_index_last_host_move(const dph_index* ix, int64_t* counts, float* ms);
 
 /* ---- removing vectors (replaces index.remove_ids(faiss.IDSelectorBatch(ids)) / remove_ids(faiss.IDSelectorRange(lo, hi)) of faiss
  * 1.6.x IndexIVF; DESIGN.md 3.2 "Removing vectors") ----
