@@ -98,6 +98,12 @@ _SIGS = {
     "dph_index_get_centroids": (_i32, [_vp, _vp, _i32]),
     "dph_index_get_pq": (_i32, [_vp, _vp, _i32]),
     "dph_index_last_train_ms": (_i32, [_vp, _vp]),
+    "dph_filter_create": (_i32, [C.POINTER(_vp), _vp, _vp, _i64, _i64, _i64, _i32, _i32]),
+    "dph_filter_free": (None, [_vp]),
+    "dph_filter_rows": (_i64, [_vp]),
+    "dph_filter_bytes": (_i64, [_vp]),
+    "dph_filter_copy_mask": (_i32, [_vp, _vp]),
+    "dph_index_set_filter": (_i32, [_vp, _vp]),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -126,10 +126,25 @@ struct dph_index {
     int64_t fetch_counts[4] = {};      // last search: slices, lists fetched, blocks fetched, resident lists scanned
     float fetch_ms = 0.f;              // last search: time of its fetch kernels (profiling on)
     DevBuf view, fdesc, hs_D, hs_I, hs_G;   // per slice: block-offset view, fetch descriptors, the running top-k and the slice's
+
+    // Filtered search (filter.cu, DESIGN.md 3.6): the committed layout's serial (process-wide unique, set by dph_commit_layout) and
+    // the filter later searches apply (dph_index_set_filter; nullptr: none).
+    uint64_t layout_version = 0;
+    const dph_filter* filter = nullptr;
 };
 
-// Where the scan stage reads the codes of lists [lo, hi): the handle's own blocks, or in host mode the view of one slice.
-struct DphCodeSrc { const uint8_t* codes; const long long* blk_off; int64_t lo, hi; };
+// A row mask of one shard: mask[b] bit l = row l of the shard's code block b is selected.  Valid for ix while ix->layout_version ==
+// version.
+struct dph_filter {
+    dph_index* ix = nullptr;
+    uint64_t version = 0;
+    uint32_t* mask = nullptr;           // [nwords] device
+    int64_t nwords = 0, rows = 0;
+};
+
+// Where the scan stage reads the codes of lists [lo, hi): the handle's own blocks, or in host mode the view of one slice.  mask: the
+// active filter's row mask, indexed in the shard's own block numbering (ix->blk_off), or nullptr.
+struct DphCodeSrc { const uint8_t* codes; const long long* blk_off; int64_t lo, hi; const uint32_t* mask; };
 
 // Writes list_len / list_start / blk_off of `L` to the device and makes `L` the handle's layout, totals included; the only code
 // that does.
@@ -137,6 +152,11 @@ int dph_commit_layout(dph_index* ix, DphLayout L);
 void dph_free_lists(dph_index* ix);            // the handle's list arrays go; it then has no lists
 int check_ready(dph_index* ix, int k);
 
+__device__ __forceinline__ long long lower_bound_ll(const long long* a, long long n, long long key) {      // first i with a[i] >= key
+    long long lo = 0, hi = n;
+    while (lo < hi) { const long long mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
+    return lo;
+}
 // Block -> list lookup inside the shard: last l in [lo,hi) with blk_off[l] <= blk.
 __device__ __forceinline__ long long list_of_block(const long long* blk_off, long long lo, long long hi, long long blk) {
     while (hi - lo > 1) { long long mid = (lo + hi) >> 1; if (blk_off[mid] <= blk) lo = mid; else hi = mid; }
@@ -186,6 +206,9 @@ struct DevTmp {            // the device allocations of one call, freed on every
     void release(void* p) { for (void*& q : ps) if (q == p) q = nullptr; }
 };
 
+// A label-set selector on the device (remove.cu): ids [n] (mem: where they live) copied into a temporary of `tmp`, sorted and
+// de-duplicated on st -> *out [*nu].  `what` prefixes the error.
+int dph_label_set(DevTmp& tmp, const int64_t* ids, int64_t n, int mem, cudaStream_t st, long long** out, int64_t* nu, const char* what);
 // Rows per staging chunk of set_lists / copy_lists / remove (about 256 MB of code rows; DPH_UPLOAD_CHUNK_ROWS overrides it for tests).
 int64_t dph_chunk_rows();
 // Block re-layout of the add (lists.cu), also the remove's block shift: blocks [blk0, blk0 + gridDim.x) of the layout boff_new are
@@ -241,7 +264,7 @@ int dph_launch_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* 
 int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
 // ---- host_codes.cu ----
 // Host mode: the scan stage of one chunk, slice by slice (DESIGN.md 3.5).
-int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
+int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G, const uint32_t* mask);
 // Host mode after set_lists: the HBM region (stream only) and the resident table (empty).
 int dph_host_lists_ready(dph_index* ix);
 // Host mode after a committed mutation: when a list of the shard changed (its length, so its blocks), the resident set empties and

@@ -1,6 +1,7 @@
 // lists.cu -- the resident lists: their layout, set_lists / set_lists_synthetic, add_with_ids, copy_lists (DESIGN.md 3, 3.1).
 // remove.cu holds remove_ids and sync_list_len; both commit their layout through dph_commit_layout below.
 #include "index_internal.cuh"
+#include <atomic>
 #include <limits.h>
 #include <stdlib.h>
 #include <thrust/device_ptr.h>
@@ -52,6 +53,8 @@ int dph_commit_layout(dph_index* ix, DphLayout L) {
     DPH_CUDA(cudaMemcpy(ix->blk_off, L.blk_off.data(), nlist * 8, cudaMemcpyHostToDevice));
     ix->ntotal = L.start[nlist]; ix->ntotal_local = L.rows; ix->nblocks_local = L.nblocks;
     ix->lay = std::move(L);
+    static std::atomic<uint64_t> serial{0};          // unique across handles: a filter matches one handle's one layout
+    ix->layout_version = ++serial;
     return 0;
 }
 

@@ -14,11 +14,6 @@
 #include <thrust/sort.h>
 #include <thrust/unique.h>
 
-__device__ __forceinline__ long long lower_bound_ll(const long long* a, long long n, long long key) {      // first i with a[i] >= key
-    long long lo = 0, hi = n;
-    while (lo < hi) { const long long mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 __device__ __forceinline__ long long upper_bound_ll(const long long* a, long long n, long long key) {      // first i with a[i] > key
     long long lo = 0, hi = n;
     while (lo < hi) { const long long mid = (lo + hi) >> 1; if (a[mid] <= key) lo = mid + 1; else hi = mid; }
@@ -121,6 +116,24 @@ __global__ void rm_dm_gather_kernel(long long d0, long long n, const long long* 
     out_rows[k] = ((boff_new[l] + ob - boff_old[l]) << 5) | (row & 31);
 }
 
+int dph_label_set(DevTmp& tmp, const int64_t* ids, int64_t n, int mem, cudaStream_t st, long long** out, int64_t* nu, const char* what) {
+    const std::string oom = std::string(what) + ": not enough device memory for the temporary buffers; the index is unchanged";
+    long long* sel;
+    DPH_TRY(tmp.alloc(&sel, n, oom.c_str()));
+    DPH_CUDA(cudaMemcpyAsync(sel, ids, (size_t)n * 8, mem == DPH_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
+    try {
+        thrust::device_ptr<long long> sp(sel);
+        thrust::sort(thrust::cuda::par.on(st), sp, sp + n);
+        *nu = thrust::unique(thrust::cuda::par.on(st), sp, sp + n) - sp;
+    } catch (const std::exception& e) {
+        cudaGetLastError();
+        dph_set_error(std::string(what) + ": device sort failed; the index is unchanged: " + e.what());
+        return 1;
+    }
+    *out = sel;
+    return 0;
+}
+
 DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_ids, int64_t range_lo, int64_t range_hi, int mem,
                                  int64_t* n_removed_out, int64_t* removed_per_list_out) {
     DPH_CHECK(ix && ix->list_len, "remove_ids: lists are not set");
@@ -168,11 +181,8 @@ DPH_API int dph_index_remove_ids(dph_index* ix, const int64_t* ids, int64_t n_id
     try {
         if (ids) {
             long long *sel, *first, *cnt, *off;
-            DPH_TRY(tmp.alloc(&sel, n_ids, oom));
-            DPH_CUDA(cudaMemcpyAsync(sel, ids, (size_t)n_ids * 8, mem == DPH_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
-            thrust::device_ptr<long long> sp(sel);
-            thrust::sort(thrust::cuda::par.on(st), sp, sp + n_ids);
-            const int64_t nu = thrust::unique(thrust::cuda::par.on(st), sp, sp + n_ids) - sp;
+            int64_t nu = 0;
+            DPH_TRY(dph_label_set(tmp, ids, n_ids, mem, st, &sel, &nu, "remove_ids"));
             DPH_TRY(tmp.alloc(&first, nu, oom)); DPH_TRY(tmp.alloc(&cnt, nu, oom)); DPH_TRY(tmp.alloc(&off, nu, oom));
             rm_find_kernel<<<(unsigned)((nu + 255) / 256), 256, 0, st>>>(sel, nu, w_dm_ids, dm_n, first, cnt);
             DPH_CUDA(cudaGetLastError());

@@ -31,6 +31,7 @@ struct ScanArgs {
     const float* lut_canon;
     unsigned* gthr; unsigned long long* cand; const long long* cand_off; int* cand_cnt;
     long long n; int nprobe; int keep;
+    const unsigned* mask; const long long* mask_off;     // filtered variants: the row mask, and the shard's first block of each list
 };
 
 #define NT DPH_SCAN_THREADS
@@ -127,6 +128,22 @@ struct SegCursor {
     }
     __device__ __forceinline__ const uint4* ptr(unsigned b) const { return base + (size_t)(b - wrel) * (DPH_BLK_BYTES / 16); }
 };
+// The filtered scan's cursor: also the segment's row of the mask, mrow[b] = the mask word of work block b (the list's block b - wrel,
+// in the shard's block numbering).  The unfiltered scan keeps the plain SegCursor, so its code is what it was.
+struct SegCursorF : SegCursor {
+    const unsigned* mrow;
+    __device__ __forceinline__ void seek(const DphSeg* __restrict__ tab, unsigned b, const uint8_t* codes, const ScanArgs& a) {
+        if (b < wend) return;
+        SegCursor::seek(tab, b, codes);
+        mrow = a.mask + (a.mask_off[tab[seg].list] - (long long)wrel);
+    }
+};
+template <bool FILT> struct ScanCursor { using T = SegCursor; };
+template <> struct ScanCursor<true> { using T = SegCursorF; };
+__device__ __forceinline__ void cursor_seek(SegCursor& c, const DphSeg* tab, unsigned b, const uint8_t* codes, const ScanArgs&) { c.seek(tab, b, codes); }
+__device__ __forceinline__ void cursor_seek(SegCursorF& c, const DphSeg* tab, unsigned b, const uint8_t* codes, const ScanArgs& a) { c.seek(tab, b, codes, a); }
+__device__ __forceinline__ unsigned cursor_mask(const SegCursor&, unsigned) { return ~0u; }
+__device__ __forceinline__ unsigned cursor_mask(const SegCursorF& c, unsigned b) { return c.mrow[b]; }
 
 __device__ __forceinline__ void block_compact(ScanShared* sh, int keep, unsigned* gthr_q) {
     const int tid = threadIdx.x;
@@ -151,7 +168,8 @@ __device__ __forceinline__ void block_compact(ScanShared* sh, int keep, unsigned
     __syncthreads();
 }
 
-template <int MODE>
+// FILT: a row passes only when its mask bit is set; a block whose mask word is 0 is not prefetched, loaded or scored.
+template <int MODE, bool FILT>
 __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
     unsigned char* const smem = dph_smem;
     constexpr int LUT_BYTES = (MODE == DPH_SCAN_FAST) ? SMEM_LUT_FAST : SMEM_LUT_EXACT;
@@ -185,7 +203,7 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 
         // segment table of this query: shared memory when it fits (always for nprobe <= 256), else global
         const DphSeg* tab = (a.nseg[q] <= DPH_SEG_SMEM) ? sh->segtab : (a.segs + q * a.nprobe);
-        SegCursor cc, pc;                                 // consume / L2-prefetch cursors
+        typename ScanCursor<FILT>::T cc, pc;              // consume / L2-prefetch cursors
         cc.init(); pc.init();
         unsigned b = b0 + warp;                           // next block this warp consumes
         unsigned bp = b0 + warp;                          // next block this warp prefetches into L2
@@ -194,15 +212,19 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
         // the first code blocks are requested BEFORE the LUT is staged: their HBM latency overlaps the staging
 #pragma unroll 1
         for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < b1; r++, bp += NW) {
-            pc.seek(tab, bp, a.codes);
-            if (lane == 0) l2_prefetch_block(pc.ptr(bp));
+            cursor_seek(pc, tab, bp, a.codes, a);
+            if (lane == 0 && (!FILT || cursor_mask(pc, bp))) l2_prefetch_block(pc.ptr(bp));
         }
         bool more = b < b1;
+        unsigned n_mask = ~0u;                            // FILT: the mask word of the block in nxt
         if (more) {
-            cc.seek(tab, b, a.codes);
-            const uint4* p = cc.ptr(b) + lane;
+            cursor_seek(cc, tab, b, a.codes, a);
+            if (FILT) n_mask = cursor_mask(cc, b);
+            if (!FILT || n_mask) {
+                const uint4* p = cc.ptr(b) + lane;
 #pragma unroll
-            for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+            }
             n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = (b - cc.wrel) * 32u;
         }
         // ---- stage this query's LUT into shared memory (twelve 16-byte loads in flight per thread) ----
@@ -246,20 +268,25 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 #pragma unroll
                 for (int c6 = 0; c6 < 6; c6++) cur[c6] = nxt[c6];
                 const int c_len = n_len; const unsigned c_gstart = n_gstart, c_j0 = n_j0; const float c_dis0 = n_dis0;
+                const unsigned c_mask = n_mask;
                 if (bp < b1) {
-                    pc.seek(tab, bp, a.codes);
-                    if (lane == 0) l2_prefetch_block(pc.ptr(bp));
+                    cursor_seek(pc, tab, bp, a.codes, a);
+                    if (lane == 0 && (!FILT || cursor_mask(pc, bp))) l2_prefetch_block(pc.ptr(bp));
                     bp += NW;
                 }
                 b += NW;
                 more = b < b1;
                 if (more) {
-                    cc.seek(tab, b, a.codes);
-                    const uint4* p = cc.ptr(b) + lane;
+                    cursor_seek(cc, tab, b, a.codes, a);
+                    if (FILT) n_mask = cursor_mask(cc, b);
+                    if (!FILT || n_mask) {
+                        const uint4* p = cc.ptr(b) + lane;
 #pragma unroll
-                    for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                        for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                    }
                     n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = (b - cc.wrel) * 32u;
                 }
+                if (FILT && c_mask == 0) continue;                 // warp-uniform: no row of the block is selected
                 float score;
                 if (MODE == DPH_SCAN_FAST) {
                     float2 a01 = make_float2(c_dis0, 0.f), a23 = make_float2(0.f, 0.f);
@@ -284,7 +311,7 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
                 }
                 const unsigned j = c_j0 + lane;
                 const unsigned sk = dph_fkey(score);
-                const bool pass = ((int)j < c_len) && (sk >= *((volatile unsigned*)&sh->thr));
+                const bool pass = ((int)j < c_len) && (!FILT || ((c_mask >> lane) & 1u)) && (sk >= *((volatile unsigned*)&sh->thr));
                 const unsigned pm = __ballot_sync(0xffffffffu, pass);
                 if (pm) {
                     int basep = 0;
@@ -343,6 +370,7 @@ struct GroupScanArgs {     // both grouped kernels (scan_pair_kernel, scan_quad_
     long long list_lo, list_hi; int nprobe; int keep;
     const DphUnit* udesc;          // quad mode: resolved unit records (plan)
     unsigned one;                  // the constant 1, as a run-time value (imad_add)
+    const unsigned* mask; const long long* mask_off;     // filtered variants: the row mask, and the shard's first block of each list
 };
 #define PCAP 1536                  // PCAP - NT = DPH_PAIR_KEEP_MAX (each warp adds <= 32 per buffer after the latch is polled)
 static_assert(PCAP - NT == DPH_PAIR_KEEP_MAX, "pair latch margin");
@@ -401,6 +429,7 @@ __device__ __forceinline__ void warp_append(bool pass, unsigned long long key, u
     }
 }
 
+template <bool FILT>
 __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(GroupScanArgs a) {
     unsigned char* const smem = dph_smem;
     PairShared* sh = reinterpret_cast<PairShared*>(smem + SMEM_LUT_FAST);
@@ -455,17 +484,22 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(GroupScanArgs a) {
         const float base_a = a.cd[qa * a.nprobe + ra] + pa.y, base_b = a.cd[qb * a.nprobe + rb] + pb.y;
         const unsigned gs_a = a.gdense[qa * a.nprobe + ra], gs_b = a.gdense[qb * a.nprobe + rb];
         const uint4* lbase = reinterpret_cast<const uint4*>(a.codes + a.blk_off[l] * DPH_BLK_BYTES);
+        const unsigned* mrow = FILT ? a.mask + a.mask_off[l] : nullptr;      // FILT: mask word of the list's block b = mrow[b]
 
         unsigned b = bi0 + warp, bp = bi0 + warp;
         uint4 nxt[6];
 #pragma unroll 1
         for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += NW)
-            if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16));
+            if (lane == 0 && (!FILT || mrow[bp])) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16));
         bool more = b < bend;
+        unsigned n_mask = ~0u;
         if (more) {
-            const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+            if (FILT) n_mask = mrow[b];
+            if (!FILT || n_mask) {
+                const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
-            for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+            }
         }
         bool counted = false;
         while (true) {
@@ -474,15 +508,19 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(GroupScanArgs a) {
                 uint4 cur[6];
 #pragma unroll
                 for (int c6 = 0; c6 < 6; c6++) cur[c6] = nxt[c6];
-                const unsigned bcur = b;
-                if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16)); bp += NW; }
+                const unsigned bcur = b, c_mask = n_mask;
+                if (bp < bend) { if (lane == 0 && (!FILT || mrow[bp])) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16)); bp += NW; }
                 b += NW;
                 more = b < bend;
                 if (more) {
-                    const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+                    if (FILT) n_mask = mrow[b];
+                    if (!FILT || n_mask) {
+                        const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
-                    for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                        for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
+                    }
                 }
+                if (FILT && c_mask == 0) continue;                 // warp-uniform: no row of the block is selected
                 unsigned s0 = 0, s1 = 0, s2 = 0, s3 = 0;
                 pair_chunk<0>(cur[0], ywin, s0, s1, s2, s3);
                 pair_chunk<1>(cur[1], ywin, s0, s1, s2, s3);
@@ -494,7 +532,7 @@ __global__ void __launch_bounds__(NT, 1) scan_pair_kernel(GroupScanArgs a) {
                 const float sc_a = fmaf(pa.x, (float)(tot & 0xFFFFu), base_a);
                 const float sc_b = fmaf(pb.x, (float)(tot >> 16), base_b);
                 const unsigned j = bcur * 32u + lane;
-                const bool valid = (int)j < len;
+                const bool valid = (int)j < len && (!FILT || ((c_mask >> lane) & 1u));
                 const unsigned ka = dph_fkey(sc_a), kb = dph_fkey(sc_b);
                 warp_append(valid && ka >= *((volatile unsigned*)&sh->thr[0]), ((unsigned long long)ka << 32) | (unsigned long long)(0xFFFFFFFFu - (gs_a + j)),
                             sh->cbuf[0], &sh->cnt[0], PCAP, lane);
@@ -657,6 +695,7 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() { unsigned long l
 // A warp that runs out of blocks starts the next item's stream: it waits for its copy of the next record's head (requested with
 // cp.async after this item's table build; warp 0 also waits for the whole record here) and issues the L2 prefetch of its first
 // DPH_L2_PREFETCH_ROUNDS blocks of the next item, so HBM keeps streaming while the other warps finish, compact and publish.
+template <bool FILT>
 __device__ __forceinline__ void quad_prefetch_next(const GroupScanArgs& a, const QuadShared* sh, int total_units, unsigned long long pol) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     asm volatile("cp.async.wait_all;" ::: "memory");
@@ -664,19 +703,23 @@ __device__ __forceinline__ void quad_prefetch_next(const GroupScanArgs& a, const
         const DphUnit* nd = reinterpret_cast<const DphUnit*>(sh->head[warp]);
         const uint4* lb = reinterpret_cast<const uint4*>(a.codes + nd->blk * DPH_BLK_BYTES);
         const unsigned bend = nd->bend;
+        const unsigned* mrow = FILT ? a.mask + a.mask_off[nd->list] : nullptr;
         unsigned bp = nd->bi0 + warp;
 #pragma unroll 1
-        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += QNW) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol);
+        for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < bend; r++, bp += QNW)
+            if (!FILT || mrow[bp]) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol);
     }
 }
 
 // The scan of one item over its block range with NTAB packed tables: rounds until a candidate buffer may overflow or the warp is out
 // of blocks, then a barrier, the compaction of the buffers over keep and the refresh of the thresholds; until every warp is done.
 // The code stream is loaded with the evict_first policy `pol`: each block is read once per batch.
-template <int NTAB, int IMADL>
+// FILT: nmask is the mask word of the block in nxt (in and out), mrow[b] the mask word of the item's list's block b.
+template <int NTAB, int IMADL, bool FILT>
 __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
                                                  unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, int total_units,
-                                                 unsigned long long pol, unsigned long long* ph, unsigned long long& ph_t) {
+                                                 unsigned long long pol, unsigned long long* ph, unsigned long long& ph_t, unsigned& nmask,
+                                                 const unsigned* mrow) {
     (void)ph; (void)ph_t;
     const int lane = threadIdx.x & 31;
     const int len = dsc->len, nq = dsc->nq;
@@ -692,15 +735,19 @@ __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadSha
             uint4 cur6[6];
 #pragma unroll
             for (int c6 = 0; c6 < 6; c6++) cur6[c6] = nxt[c6];
-            const unsigned bcur = b;
-            if (bp < bend) { if (lane == 0) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16), pol); bp += QNW; }
+            const unsigned bcur = b, cmask = nmask;
+            if (bp < bend) { if (lane == 0 && (!FILT || mrow[bp])) l2_prefetch_block(lbase + (size_t)bp * (DPH_BLK_BYTES / 16), pol); bp += QNW; }
             b += QNW;
             more = b < bend;
             if (more) {
-                const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+                if (FILT) nmask = mrow[b];
+                if (!FILT || nmask) {
+                    const uint4* p = lbase + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
-                for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
+                    for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
+                }
             }
+            if (FILT && cmask == 0) continue;                      // warp-uniform: no row of the block is selected
             unsigned sr[2][4] = {}, ab[2][4] = {};
             quad_chunk<0, NTAB, IMADL>(cur6[0], rot, one, sr, ab);
             quad_chunk<1, NTAB, IMADL>(cur6[1], rot, one, sr, ab);
@@ -709,7 +756,7 @@ __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadSha
             quad_chunk<4, NTAB, IMADL>(cur6[4], rot, one, sr, ab);
             quad_chunk<5, NTAB, IMADL>(cur6[5], rot, one, sr, ab);
             const unsigned j = bcur * 32u + lane;
-            const bool valid = (int)j < len;
+            const bool valid = (int)j < len && (!FILT || ((cmask >> lane) & 1u));
             // thresholds are compared in the float domain (one FSETP per query); the order-preserving integer key is built only for
             // the rare vector that passes.  (float)(unsigned short) converts a 16-bit half of the register without a mask / shift.
             float f[NS]; bool p[NS]; bool any = false;
@@ -736,7 +783,7 @@ __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadSha
         }
         if (!more && !counted) {
             counted = true;
-            quad_prefetch_next(a, sh, total_units, pol);
+            quad_prefetch_next<FILT>(a, sh, total_units, pol);
             if (lane == 0) atomicAdd(&sh->ndone, 1);
         }
         __syncthreads();
@@ -763,14 +810,19 @@ __device__ __forceinline__ uint4 quad_pack(unsigned a, unsigned b, unsigned c, u
     const unsigned u0 = __byte_perm(c, d, 0x5140), u1 = __byte_perm(c, d, 0x7362);
     return make_uint4(__byte_perm(t0, u0, 0x5410), __byte_perm(t0, u0, 0x7632), __byte_perm(t1, u1, 0x5410), __byte_perm(t1, u1, 0x7632));
 }
-// This warp's first code block of an item into registers.
-__device__ __forceinline__ void quad_first_block(const GroupScanArgs& a, const DphUnit* d, uint4 (&nxt)[6], unsigned long long pol) {
+// This warp's first code block of an item into registers (FILT: with its mask word in nmask; not loaded when that is 0).
+template <bool FILT>
+__device__ __forceinline__ void quad_first_block(const GroupScanArgs& a, const DphUnit* d, uint4 (&nxt)[6], unsigned long long pol,
+                                                 unsigned& nmask) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned b = d->bi0 + warp;
     if (b < d->bend) {
-        const uint4* p = reinterpret_cast<const uint4*>(a.codes + d->blk * DPH_BLK_BYTES) + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
+        if (FILT) nmask = a.mask[a.mask_off[d->list] + b];
+        if (!FILT || nmask) {
+            const uint4* p = reinterpret_cast<const uint4*>(a.codes + d->blk * DPH_BLK_BYTES) + (size_t)b * (DPH_BLK_BYTES / 16) + lane;
 #pragma unroll
-        for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
+            for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32, pol);
+        }
     }
 }
 
@@ -780,7 +832,7 @@ __device__ __forceinline__ void quad_first_block(const GroupScanArgs& a, const D
 // out of blocks prefetches its first blocks of the next item into L2 (quad_prefetch_next), and every warp loads its first block of the
 // next item into registers before the candidates are published, so those are in flight during the publish and the next table build.
 // The table sources (a few MB per batch, re-read at every item) are loaded evict_last, the code stream evict_first.
-template <int IMADL>
+template <int IMADL, bool FILT>
 __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
     unsigned char* const smem = dph_smem;
     QuadShared* sh = reinterpret_cast<QuadShared*>(smem + SMEM_QUAD_TABLES);
@@ -811,14 +863,16 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
         reinterpret_cast<uint4*>(&sh->desc[0])[tid] = __ldg(reinterpret_cast<const uint4*>(a.udesc + sh->unit) + tid);
     __syncthreads();
     uint4 nxt[6];
+    unsigned nmask = ~0u;
     if (any_unit) {      // the first item's first blocks; later items get theirs at the end of the previous item
         const DphUnit* d = &sh->desc[0];
         const uint4* lb = reinterpret_cast<const uint4*>(a.codes + d->blk * DPH_BLK_BYTES);
+        const unsigned* mrow = FILT ? a.mask + a.mask_off[d->list] : nullptr;
         unsigned bp = d->bi0 + warp;
 #pragma unroll 1
         for (int r = 0; r < DPH_L2_PREFETCH_ROUNDS && bp < d->bend; r++, bp += QNW)
-            if (lane == 0) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol_stream);
-        quad_first_block(a, d, nxt, pol_stream);
+            if (lane == 0 && (!FILT || mrow[bp])) l2_prefetch_block(lb + (size_t)bp * (DPH_BLK_BYTES / 16), pol_stream);
+        quad_first_block<FILT>(a, d, nxt, pol_stream, nmask);
     }
     while (any_unit) {
         int next_u = 0;
@@ -880,11 +934,12 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
             if (warp == 0 && lane < (int)(sizeof(DphUnit) / 16)) cp_async16(reinterpret_cast<unsigned char*>(&sh->desc[cur ^ 1]) + lane * 16, rec + lane * 16);
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
-        if (ntab == 2) quad_item_rounds<2, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t);
-        else quad_item_rounds<1, IMADL>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t);
+        const unsigned* mrow = FILT ? a.mask + a.mask_off[dsc->list] : nullptr;
+        if (ntab == 2) quad_item_rounds<2, IMADL, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
+        else quad_item_rounds<1, IMADL, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
         // every warp waited for its copies before the rounds' last barrier: the next record is visible
         any_unit = nu < total_units;
-        if (any_unit) quad_first_block(a, &sh->desc[cur ^ 1], nxt, pol_stream);
+        if (any_unit) quad_first_block<FILT>(a, &sh->desc[cur ^ 1], nxt, pol_stream, nmask);
         // ---- publish the candidate sets: the (up to) eight region reservations go out together, one barrier ----
         if (tid < nq) sh->base[tid] = atomicAdd(a.cand_cnt + sh->qs[tid], sh->cnt[tid]);
         __syncthreads();
@@ -919,8 +974,10 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
 #undef QPH_MARK
 
 __global__ void smem_base_probe_kernel(unsigned* out) { *out = (unsigned)__cvta_generic_to_shared(dph_smem); }
-// scan_quad_kernel by IMAD level, knob 0 of dph_set_tuning (out of range: the default, 1)
-static void (*const quad_kernels[4])(GroupScanArgs) = {scan_quad_kernel<0>, scan_quad_kernel<1>, scan_quad_kernel<2>, scan_quad_kernel<3>};
+// scan_quad_kernel by filter (unfiltered, filtered) and IMAD level, knob 0 of dph_set_tuning (out of range: the default, 1)
+static void (*const quad_kernels[2][4])(GroupScanArgs) = {
+    {scan_quad_kernel<0, false>, scan_quad_kernel<1, false>, scan_quad_kernel<2, false>, scan_quad_kernel<3, false>},
+    {scan_quad_kernel<0, true>, scan_quad_kernel<1, true>, scan_quad_kernel<2, true>, scan_quad_kernel<3, true>}};
 
 static int dph_scan_setup_attrs() {
     static DphPerDeviceOnce once;
@@ -934,10 +991,14 @@ static int dph_scan_setup_attrs() {
         // the quad scan also needs the window's top address byte to be 0 (its gather addresses are built without it)
         DPH_CHECK(h == DPH_DYN_SMEM_BASE, "dynamic shared memory window does not start at 0x400 on this driver; rebuild with the probed value");
     }
-    DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(ScanShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_kernel<DPH_SCAN_EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
-    DPH_CUDA(cudaFuncSetAttribute(scan_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
-    for (auto f : quad_kernels) DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    for (auto f : {scan_kernel<DPH_SCAN_FAST, false>, scan_kernel<DPH_SCAN_FAST, true>})
+        DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(ScanShared)));
+    for (auto f : {scan_kernel<DPH_SCAN_EXACT, false>, scan_kernel<DPH_SCAN_EXACT, true>})
+        DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
+    for (auto f : {scan_pair_kernel<false>, scan_pair_kernel<true>})
+        DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
+    for (auto& row : quad_kernels)
+        for (auto f : row) DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
     return 0;
 }
 
@@ -945,14 +1006,18 @@ int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
     if (n == 0) return 0;
     DPH_TRY(dph_scan_setup_attrs());
     const int grid = p.grid, group = p.pass_group(exact), keep = p.pass_keep(exact);
+    const bool filt = src.mask != nullptr;          // the row mask is indexed in the shard's own block numbering (ix->blk_off)
     if (group == 1) {
         ScanArgs a;
         a.codes = src.codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
         a.lut_canon = ix->lut_canon.as<float>(); a.gthr = ix->gthr.as<unsigned>();
         a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
         a.n = n; a.nprobe = ix->nprobe; a.keep = keep;
-        if (exact) scan_kernel<DPH_SCAN_EXACT><<<grid, NT, SMEM_LUT_EXACT + sizeof(ScanShared), st>>>(a);
-        else scan_kernel<DPH_SCAN_FAST><<<grid, NT, SMEM_LUT_FAST + sizeof(ScanShared), st>>>(a);
+        a.mask = src.mask; a.mask_off = (const long long*)ix->blk_off;
+        const size_t smem = (exact ? SMEM_LUT_EXACT : SMEM_LUT_FAST) + sizeof(ScanShared);
+        auto f = exact ? (filt ? scan_kernel<DPH_SCAN_EXACT, true> : scan_kernel<DPH_SCAN_EXACT, false>)
+                       : (filt ? scan_kernel<DPH_SCAN_FAST, true> : scan_kernel<DPH_SCAN_FAST, false>);
+        f<<<grid, NT, smem, st>>>(a);
     } else {
         GroupScanArgs a;
         a.codes = src.codes; a.blk_off = src.blk_off; a.list_len = ix->list_len; a.grp_cnt = ix->grp_cnt.as<int>();
@@ -962,9 +1027,10 @@ int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
         a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
         a.list_lo = src.lo; a.list_hi = src.hi; a.nprobe = ix->nprobe; a.keep = keep;
         a.udesc = ix->grp_udesc.as<DphUnit>(); a.one = 1u;
+        a.mask = src.mask; a.mask_off = (const long long*)ix->blk_off;
         const int lv = g_dph_tune[0] >= 0 && g_dph_tune[0] <= 3 ? g_dph_tune[0] : 1;
-        if (group == 4) quad_kernels[lv]<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
-        else scan_pair_kernel<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
+        if (group == 4) quad_kernels[filt][lv]<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
+        else (filt ? scan_pair_kernel<true> : scan_pair_kernel<false>)<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
     }
     DPH_CUDA(cudaGetLastError());
     return 0;

@@ -115,18 +115,33 @@ int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
     return 0;
 }
 
+// The row mask of the filter set on ix (nullptr: none).  Rejects a filter of another handle or of an earlier layout of this one.
+static int active_mask(const dph_index* ix, const uint32_t** mask) {
+    const dph_filter* f = ix->filter;
+    *mask = nullptr;
+    if (!f) return 0;
+    DPH_CHECK(f->ix == ix, "search: the filter was built for another index; build it with this index's make_filter");
+    DPH_CHECK(f->version == ix->layout_version,
+              "search: the filter is stale (the index's lists changed since it was built: set_lists, add, remove, merge or sync_list_len); "
+              "rebuild the filter");
+    *mask = f->mask;
+    return 0;
+}
+
 // Scan stage, from the rotated queries in xr and the probes in (key, cd): the tables, then the passes over the shard's codes -- in
-// host mode slice by slice, the tables built once for all slices.
+// host mode slice by slice, the tables built once for all slices.  Every search path passes here, so the active filter applies here.
 static int scan_stage(dph_index* ix, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
     cudaStream_t st = ix->stream;
+    const uint32_t* mask;
+    DPH_TRY(active_mask(ix, &mask));
     const DphSearchPlan p = search_plan(ix, n, k);
     DPH_TRY(size_scan(ix, p, n));
     ix->last_group = p.group;
     DPH_TRY(dph_launch_lut(ix->xr.as<float>(), n, ix->pq, ix->lut_canon.as<float>(), ix->lutmax.as<float>(),
                            ix->lutmin.as<float>(), ix->lutmaxv.as<float>(), p.grouped() ? ix->lutq.p : nullptr,
                            p.grouped() ? ix->qparams.as<float2>() : nullptr, st, p.group));
-    if (ix->on_host) return dph_host_scan(ix, p, n, k, D, I, G);
-    const DphCodeSrc src{ix->codes, (const long long*)ix->blk_off, ix->list_lo, ix->list_hi};
+    if (ix->on_host) return dph_host_scan(ix, p, n, k, D, I, G, mask);
+    const DphCodeSrc src{ix->codes, (const long long*)ix->blk_off, ix->list_lo, ix->list_hi, mask};
     return dph_scan_passes(ix, p, src, n, k, D, I, G);
 }
 

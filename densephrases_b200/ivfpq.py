@@ -4,6 +4,7 @@ Mirrors the slice of the faiss Python API that reference densephrases/index.py u
 ``search(x, k) -> (D, I)`` (index.py:200), ``reconstruct`` (index.py:31,286,296), ``ntotal``, ``d``, ``nprobe``
 (index.py:33,53,62), the OPQ matrix (index.py:32).  numpy in -> numpy out through the C ABI with host buffers;
 torch CUDA tensors in -> torch CUDA tensors out (device pointers, asynchronous on the current stream)."""
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -213,36 +214,66 @@ class IvfPqIndex:
         return out
 
     # ---- removing vectors (faiss index.remove_ids with IDSelectorBatch / IDSelectorRange) ----------
+    def _selector(self, sel, what):
+        """A label selector (remove_ids, make_filter) -> the C arguments (ids, n_ids, range_lo, range_hi, mem) and the array they point
+        into (keep it alive for the call).  sel: a numpy or torch int64 array of labels or a step-1 range of labels."""
+        if isinstance(sel, range):
+            if sel.step != 1:
+                raise ValueError(f"{what}: a range selector must have step 1")
+            # ctypes would wrap bounds past the int64 range: clamp them (a stop past it then reaches every label up to 2^63 - 2)
+            lo, hi = (min(max(v, -2**63), 2**63 - 1) for v in (sel.start, sel.stop))
+            return (None, 0, lo, hi, L.MEM_HOST), None
+        if isinstance(sel, np.ndarray):
+            if sel.dtype != np.int64:
+                raise TypeError(f"{what}: labels must be int64, got {sel.dtype}")
+            ids = np.ascontiguousarray(sel).ravel()
+            return (_np_ptr(ids), len(ids), 0, 0, L.MEM_HOST), ids
+        import torch
+        if not isinstance(sel, torch.Tensor) or sel.dtype != torch.int64:
+            raise TypeError(f"{what}: expected an int64 numpy array, an int64 torch tensor or a step-1 range, got %r" % type(sel))
+        ids = sel.contiguous().view(-1)
+        if ids.is_cuda:
+            self.set_stream(torch.cuda.current_stream(ids.device).cuda_stream)
+            return (ids.data_ptr(), ids.numel(), 0, 0, L.MEM_DEVICE), ids
+        ids = ids.numpy()
+        return (_np_ptr(ids), len(ids), 0, 0, L.MEM_HOST), ids
+
     def remove_ids_per_list(self, sel):
         """Remove every row whose label is selected -> rows removed per list [nlist] i64 (this shard's lists only).  sel: a numpy or
         torch int64 array of labels (any order, duplicates allowed, absent or negative labels match nothing) or a step-1 range of
         labels.  Survivor order and the rejected cases: DESIGN.md 3.2 / dph_index_remove_ids."""
         per = np.zeros(self.nlist, dtype=np.int64)
         n = C.c_int64(0)
-        if isinstance(sel, range):
-            if sel.step != 1:
-                raise ValueError("remove_ids: a range selector must have step 1")
-            # ctypes would wrap bounds past the int64 range: clamp them (a stop past it then reaches every label up to 2^63 - 2)
-            lo, hi = (min(max(v, -2**63), 2**63 - 1) for v in (sel.start, sel.stop))
-            L.check(L.lib().dph_index_remove_ids(self._h, None, 0, lo, hi, L.MEM_HOST, C.byref(n), _np_ptr(per)))
-            return per
-        if isinstance(sel, np.ndarray):
-            if sel.dtype != np.int64:
-                raise TypeError(f"remove_ids: labels must be int64, got {sel.dtype}")
-            ids = np.ascontiguousarray(sel).ravel()
-            L.check(L.lib().dph_index_remove_ids(self._h, _np_ptr(ids), len(ids), 0, 0, L.MEM_HOST, C.byref(n), _np_ptr(per)))
-            return per
-        import torch
-        if not isinstance(sel, torch.Tensor) or sel.dtype != torch.int64:
-            raise TypeError("remove_ids: expected an int64 numpy array, an int64 torch tensor or a step-1 range, got %r" % type(sel))
-        ids = sel.contiguous().view(-1)
-        if ids.is_cuda:
-            self.set_stream(torch.cuda.current_stream(ids.device).cuda_stream)
-            L.check(L.lib().dph_index_remove_ids(self._h, ids.data_ptr(), ids.numel(), 0, 0, L.MEM_DEVICE, C.byref(n), _np_ptr(per)))
-        else:
-            ids = ids.numpy()
-            L.check(L.lib().dph_index_remove_ids(self._h, _np_ptr(ids), len(ids), 0, 0, L.MEM_HOST, C.byref(n), _np_ptr(per)))
+        args, keep = self._selector(sel, "remove_ids")
+        L.check(L.lib().dph_index_remove_ids(self._h, *args, C.byref(n), _np_ptr(per)))
+        del keep
         return per
+
+    # ---- filtered search (faiss SearchParametersIVF(sel=IDSelector...); DESIGN.md 3.6) ----------------------------------------
+    def make_filter(self, sel, exclude=False):
+        """A row filter of this index for search(..., filter=) -> IndexFilter.  sel: the selectors of remove_ids (an int64 numpy or
+        torch label array, or a step-1 range); exclude=True selects every row whose label is NOT selected.  The index is not changed.
+        The filter holds one 4-byte mask word per 32-row code block of this shard, in device memory of its own; it is valid until the
+        index's lists change (set_lists, add, remove, merge, sync_list_len), after which a search with it raises RuntimeError."""
+        h = C.c_void_p()
+        args, keep = self._selector(sel, "make_filter")
+        L.check(L.lib().dph_filter_create(C.byref(h), self._h, *args[:4], int(bool(exclude)), args[4]))
+        del keep
+        return IndexFilter(self, h)
+
+    @contextlib.contextmanager
+    def _filtered(self, filter):
+        """The filter applies to the searches inside the block, and to no other."""
+        if filter is None:
+            yield
+            return
+        if not isinstance(filter, IndexFilter):
+            raise TypeError(f"filter: expected an IndexFilter from make_filter, got {type(filter)!r}")
+        L.check(L.lib().dph_index_set_filter(self._h, filter._h))
+        try:
+            yield
+        finally:
+            L.lib().dph_index_set_filter(self._h, None)
 
     def remove_ids(self, sel):
         """== faiss index.remove_ids(IDSelectorBatch(sel)) for a label array, index.remove_ids(IDSelectorRange(lo, hi)) for
@@ -465,8 +496,14 @@ class IvfPqIndex:
         return L.lib().dph_index_device_bytes(self._h)
 
     # ---- search -------------------------------------------------------------------------------
-    def search(self, x, k):
-        """numpy [n,d] -> (D [n,k] f32, I [n,k] i64) numpy   |   torch cuda [n,d] -> torch cuda (D, I)."""
+    def search(self, x, k, filter=None):
+        """numpy [n,d] -> (D [n,k] f32, I [n,k] i64) numpy   |   torch cuda [n,d] -> torch cuda (D, I).  filter (make_filter): the
+        same probes, and only selected rows can be results -- the unfiltered ranking of the probed rows restricted to the selected ones,
+        cut at k; short results are padded with (-FLT_MAX, -1)."""
+        with self._filtered(filter):
+            return self._search(x, k)
+
+    def _search(self, x, k):
         if isinstance(x, np.ndarray):
             x = np.ascontiguousarray(x, dtype=np.float32)
             n = x.shape[0]
@@ -483,8 +520,12 @@ class IvfPqIndex:
         L.check(L.lib().dph_index_search(self._h, x.data_ptr(), n, k, D.data_ptr(), I.data_ptr(), L.MEM_DEVICE))
         return D, I
 
-    def search_partial(self, x, k):
-        """torch cuda [n,d] -> per-shard (D, I, G) torch cuda; G = canonical scan position (tie-break)."""
+    def search_partial(self, x, k, filter=None):
+        """torch cuda [n,d] -> per-shard (D, I, G) torch cuda; G = canonical scan position (tie-break).  filter: as in search."""
+        with self._filtered(filter):
+            return self._search_partial(x, k)
+
+    def _search_partial(self, x, k):
         import torch
         assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
         n = x.shape[0]
@@ -504,8 +545,13 @@ class IvfPqIndex:
         L.check(L.lib().dph_index_coarse_local(self._h, x.data_ptr(), n, keys.data_ptr()))
         return keys
 
-    def search_preassigned(self, keys_gathered, k):
-        """all-gathered keys [nshards,n,nprobe] -> this shard's partial (D, I, G) for the batch passed to coarse_local."""
+    def search_preassigned(self, keys_gathered, k, filter=None):
+        """all-gathered keys [nshards,n,nprobe] -> this shard's partial (D, I, G) for the batch passed to coarse_local.  filter: as in
+        search, this shard's own."""
+        with self._filtered(filter):
+            return self._search_preassigned(keys_gathered, k)
+
+    def _search_preassigned(self, keys_gathered, k):
         import torch
         W, n, _ = keys_gathered.shape
         D = torch.empty((n, k), dtype=torch.float32, device=keys_gathered.device)
@@ -525,8 +571,13 @@ class IvfPqIndex:
         L.check(L.lib().dph_index_coarse_split(self._h, x_local.data_ptr(), n, rec.data_ptr()))
         return rec
 
-    def search_assigned(self, rec, k):
-        """all-gathered records [n, 768 + 2 nprobe] (batch order) -> this shard's partial (D, I, G)."""
+    def search_assigned(self, rec, k, filter=None):
+        """all-gathered records [n, 768 + 2 nprobe] (batch order) -> this shard's partial (D, I, G).  filter: as in search, this
+        shard's own."""
+        with self._filtered(filter):
+            return self._search_assigned(rec, k)
+
+    def _search_assigned(self, rec, k):
         import torch
         assert rec.is_cuda and rec.dtype == torch.float32 and rec.is_contiguous()
         n = rec.shape[0]
@@ -570,6 +621,36 @@ class IvfPqIndex:
         self.set_stream(torch.cuda.current_stream(ids.device).cuda_stream)
         L.check(L.lib().dph_index_reconstruct_batch(self._h, ids.data_ptr(), ids.numel(), out.data_ptr(), found.data_ptr(), L.MEM_DEVICE))
         return out, found
+
+
+class IndexFilter:
+    """A row filter of one IvfPqIndex (make_filter): a device mask of one bit per row of the index's shard."""
+
+    def __init__(self, index, h):
+        self.index = index          # the mask belongs to this handle; keeping it alive keeps the handle alive
+        self._h = h
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        index = getattr(self, "index", None)
+        if h and getattr(index, "_h", None) and L is not None and getattr(L, "_lib", None) is not None:   # the handle outlives the filter
+            L._lib.dph_filter_free(h)
+
+    @property
+    def rows(self):
+        """Selected rows of the shard."""
+        return int(L.lib().dph_filter_rows(self._h))
+
+    @property
+    def nbytes(self):
+        """Device bytes of the mask (4 per 32-row code block of the shard)."""
+        return int(L.lib().dph_filter_bytes(self._h))
+
+    def mask(self):
+        """-> uint32 [code blocks of the shard]: bit l of word b = row l of block b is selected (blocks in the shard's list order)."""
+        out = np.empty(self.nbytes // 4, dtype=np.uint32)
+        L.check(L.lib().dph_filter_copy_mask(self._h, _np_ptr(out)))
+        return out
 
 
 def _window_scores(self, q, first_ids, L):

@@ -232,28 +232,43 @@ class MIPS(object):
             word[sel] = self.idx_f[str(g)]['word'][row[sel]]
         return doc, word
 
-    def search_dense(self, query, q_texts, nprobe=256, top_k=10):
+    def doc_filter(self, doc_ids, exclude=False):
+        """A filter of the index (make_filter) that selects the phrases of the documents doc_ids (exclude=True: of every other
+        document), for search / search_dense(doc_filter=...).  A phrase's label is its offset group plus its row in that group's
+        idx2id arrays (the inverse of get_idxs)."""
+        docs = np.unique(np.asarray(doc_ids, dtype=np.int64))
+        labels = [int(g) + np.flatnonzero(np.isin(t['doc'], docs)) for g, t in self.idx_f.items()]
+        return self.index.make_filter(np.concatenate(labels + [np.zeros(0, np.int64)]).astype(np.int64), exclude=exclude)
+
+    def search_dense(self, query, q_texts, nprobe=256, top_k=10, doc_filter=None):
         """Start and end halves of `query [B, 2d]` are stacked into one [2B, d] search (index.py:195-202).
-        `nprobe` is accepted and ignored, like the reference (its assignment is commented out at index.py:191)."""
+        `nprobe` is accepted and ignored, like the reference (its assignment is commented out at index.py:191).
+        doc_filter (doc_filter()): only phrases of the selected documents are hits; a query may then get fewer than top_k, and the
+        padded slots (label -1) get document and word -1, which the phrase stage drops."""
         B = query.shape[0]
         tic = time()
+        kw = {} if doc_filter is None else {'filter': doc_filter}
         if isinstance(query, torch.Tensor) and query.is_cuda and hasattr(self.index, 'search_device'):
             # device-resident queries (DensePhrases.search hands over the encoder's output): no host round trip before the index
             d = query.shape[1] // 2
             x = torch.cat([query[:, :d], query[:, d:]], 0).float().contiguous()
-            Dd, Id = self.index.search_device(x, top_k)
+            Dd, Id = self.index.search_device(x, top_k, **kw)
             scores, labels = Dd.cpu().numpy(), Id.cpu().numpy()
         else:
             if isinstance(query, torch.Tensor):
                 query = query.detach().cpu().numpy()
             halves = np.split(query.astype(np.float32), 2, axis=1)
-            scores, labels = self.index.search(np.concatenate(halves, axis=0), top_k)
+            scores, labels = self.index.search(np.concatenate(halves, axis=0), top_k, **kw)
         self.stage_seconds['mips'] += time() - tic
         self.stage_seconds['batches'] += 1
         logger.debug(f'1) {time()-tic:.3f}s: MIPS')
         tic = time()
         s_doc, s_word = self.get_idxs(labels[:B])
         e_doc, e_word = self.get_idxs(labels[B:])
+        if doc_filter is not None:      # get_idxs maps a padded slot to label 0, whose document may be outside the filter
+            for doc, word, lab in ((s_doc, s_word, labels[:B]), (e_doc, e_word, labels[B:])):
+                doc[lab < 0] = -1
+                word[lab < 0] = -1
         self.num_docs_list.append(sum(len(set(a.tolist()) | set(b.tolist())) for a, b in zip(s_doc, e_doc)) / B)
         self.stage_seconds['get_idxs'] += time() - tic
         logger.debug(f'2) {time()-tic:.3f}s: get index')
@@ -448,10 +463,11 @@ class MIPS(object):
     def search(self, query, q_texts=None,
                nprobe=256, top_k=10,
                aggregate=False, return_idxs=False,
-               max_answer_length=10, agg_strat='opt1', return_sent=False):
-        """query [B, 2*768] (start || end) -> list[B] of result dicts sorted by score (index.py:450-482)."""
+               max_answer_length=10, agg_strat='opt1', return_sent=False, doc_filter=None):
+        """query [B, 2*768] (start || end) -> list[B] of result dicts sorted by score (index.py:450-482).  doc_filter (doc_filter()):
+        only phrases of the selected documents are hits (search_dense); the phrase windows around a hit are not filtered."""
         tic = time()
-        dense = self.search_dense(query, q_texts=q_texts, nprobe=nprobe, top_k=top_k)
+        dense = self.search_dense(query, q_texts=q_texts, nprobe=nprobe, top_k=top_k, doc_filter=doc_filter)
         s_doc, s_word, s_lab, e_doc, e_word, e_lab, s_sc, e_sc = dense
         if isinstance(query, torch.Tensor):          # the phrase stage and the result dicts work on host arrays
             query = query.detach().cpu().numpy()

@@ -191,6 +191,12 @@ class ShardedIvfPq:
         add_with_ids, remove_ids and merge_from run in place on its page-locked array."""
         self.local.reserve_host_codes(nbytes)
 
+    def make_filter(self, sel, exclude=False):
+        """A row filter for search / search_device (IvfPqIndex.make_filter): every rank builds the mask of its own shard from the same
+        selector, with no exchange (labels are looked up where the rows live).  A collective by convention: every rank passes the same
+        selector."""
+        return self.local.make_filter(sel, exclude)
+
     def set_resident_lists(self, lists):
         """Host mode: every rank keeps in device memory the given lists that fall in its own range (IvfPqIndex.set_resident_lists)."""
         lists = np.asarray(lists, dtype=np.int64).ravel()
@@ -246,32 +252,41 @@ class ShardedIvfPq:
     def _qsplit(self, n):
         return self.world > 1 and (self.query_split is True or (self.query_split is None and use_query_split(n, self.world, self.local.nlist)))
 
-    def search_device(self, x, k):
-        """x torch cuda [n,d] (same on every rank) -> (D, I) torch cuda [n,k] (same on every rank)."""
+    def _local_steps(self, filter):
+        """This rank's search steps of both protocols, with `filter` (make_filter) applied to each."""
+        if filter is None:
+            return self.local.search_assigned, self.local.search_preassigned
+        return (lambda rec, k: self.local.search_assigned(rec, k, filter=filter),
+                lambda keys, k: self.local.search_preassigned(keys, k, filter=filter))
+
+    def search_device(self, x, k, filter=None):
+        """x torch cuda [n,d] (same on every rank) -> (D, I) torch cuda [n,k] (same on every rank).  filter (make_filter): only
+        selected rows can be results (IvfPqIndex.search)."""
         if self.world == 1:
-            return self.local.search(x, k)
+            return self.local.search(x, k, filter=filter)
         n = x.shape[0]
         if n > 4096:        # one chunk per collective round
-            parts = [self.search_device(x[i:i + 4096], k) for i in range(0, n, 4096)]
+            parts = [self.search_device(x[i:i + 4096], k, filter) for i in range(0, n, 4096)]
             return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
+        assigned, preassigned = self._local_steps(filter)
         if self._qsplit(n):
-            return sharded_search_qsplit(x, k, self.world, self.rank, self.group, self.local.coarse_split, self.local.search_assigned, pack_topk,
-                                         merge_shards_packed)
-        return sharded_search(x, k, self.world, self.group, self.local.coarse_local, self.local.search_preassigned, pack_topk, merge_shards_packed)
+            return sharded_search_qsplit(x, k, self.world, self.rank, self.group, self.local.coarse_split, assigned, pack_topk, merge_shards_packed)
+        return sharded_search(x, k, self.world, self.group, self.local.coarse_local, preassigned, pack_topk, merge_shards_packed)
 
-    def search(self, x, k):
-        """Host API == faiss index.search (index.py:200): numpy / pinned CPU tensor [n,d] -> numpy (D, I)."""
+    def search(self, x, k, filter=None):
+        """Host API == faiss index.search (index.py:200): numpy / pinned CPU tensor [n,d] -> numpy (D, I).  filter: as in
+        search_device."""
         if self.world == 1 and isinstance(x, np.ndarray):
-            return self.local.search(x, k)
+            return self.local.search(x, k, filter=filter)
         xt = torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)) if isinstance(x, np.ndarray) else x
         n = xt.shape[0]
         dev = torch.device("cuda", self.device)
         if n <= 4096 and self._qsplit(n):        # query-split: only this rank's slice of the batch crosses PCIe
             xl = query_slice(xt, self.rank, self.world).to(dev, non_blocking=True)
-            D, I = sharded_search_qsplit(None, k, self.world, self.rank, self.group, self.local.coarse_split, self.local.search_assigned, pack_topk,
-                                         merge_shards_packed, x_local=xl, n=n)
+            D, I = sharded_search_qsplit(None, k, self.world, self.rank, self.group, self.local.coarse_split, self._local_steps(filter)[0],
+                                         pack_topk, merge_shards_packed, x_local=xl, n=n)
         else:
-            D, I = self.search_device(xt.to(dev, non_blocking=True), k)
+            D, I = self.search_device(xt.to(dev, non_blocking=True), k, filter)
         if self._pinned_out is None or self._pinned_out[0].shape != (n, k):
             self._pinned_out = (torch.empty((n, k), dtype=torch.float32).pin_memory(), torch.empty((n, k), dtype=torch.int64).pin_memory())
         Dh, Ih = self._pinned_out

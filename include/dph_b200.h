@@ -15,6 +15,7 @@
  *   dph_index_encode            <- the assignment + PQ encoding inside add_with_ids (IndexIVFPQ::encode_vectors)
  *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
  *   dph_index_remove_ids        <- index.remove_ids(IDSelectorBatch(ids) | IDSelectorRange(lo, hi)) (faiss 1.6.x IndexIVF)
+ *   dph_filter_create           <- faiss.SearchParametersIVF(sel=IDSelectorBatch | IDSelectorRange | IDSelectorNot) (faiss >= 1.7.3)
  *   dph_index_sync_list_len     <- (sharded remove) the list lengths faiss keeps in one process, exchanged between shards
  *   dph_index_merge_from        <- invlists.merge_from(sub_index.invlists, offset)            build_phrase_index.py:282-338
  *   dph_index_train_coarse      <- the coarse quantizer's k-means inside index.train(x)   build_phrase_index.py:96-142
@@ -255,6 +256,32 @@ int dph_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* Gg, int
  * all-gather P; merge Pg [nshards,n,k,2] -> D/I [n,k]. */
 int dph_pack_topk(const float* D, const int64_t* I, const uint32_t* G, int64_t n, int k, int64_t* P, void* cuda_stream);
 int dph_merge_shards_packed(const int64_t* Pg, int nshards, int64_t n, int k, float* D, int64_t* I, void* cuda_stream);
+
+/* ---- filtered search (replaces index.search(x, k, params=faiss.SearchParametersIVF(sel=IDSelectorBatch(ids) |
+ * IDSelectorRange(lo, hi) | IDSelectorNot(...))), faiss >= 1.7.3; DESIGN.md 3.6 "Filtered search") ----
+ * A filter is a row mask of one shard: one uint32 per 32-row code block, bit l = lane l's row is selected.  A search with a filter set
+ * (dph_index_set_filter) has the same probes as without it; every probed row whose label is not selected is skipped before it can
+ * become a candidate, so its result is the unfiltered canonical ranking of the probed rows restricted to the selected ones, cut at k
+ * (short results padded with (-FLT_MAX, -1)).  A row is selected exactly when its label is. */
+typedef struct dph_filter dph_filter;
+/* Selector forms and rejections as dph_index_remove_ids: the label set ids [n_ids] (mem says where it lives; any order, duplicates
+ * allowed, absent or negative labels match nothing) with range_lo = range_hi = 0, or the label range [range_lo, range_hi) with ids =
+ * NULL and n_ids = 0.  exclude != 0 selects every real row whose label is NOT in the selector (padding rows never).  The index is not
+ * changed (sequential labels stay sequential).  The mask is built on the device and owned by the filter (dph_index_device_bytes does
+ * not count it).  It belongs to ix and to ix's current list layout: after set_lists, add, remove, merge or sync_list_len on ix a
+ * search with it is rejected until it is rebuilt.  Synchronises the stream. */
+int dph_filter_create(dph_filter** out, dph_index* ix, const int64_t* ids, int64_t n_ids, int64_t range_lo, int64_t range_hi, int exclude,
+                      int mem);
+/* Frees the mask; a filter set on its index is cleared there.  Free a filter before its index. */
+void dph_filter_free(dph_filter* f);
+int64_t dph_filter_rows(const dph_filter* f);            /* selected rows of the shard */
+int64_t dph_filter_bytes(const dph_filter* f);           /* device bytes of the mask */
+/* The mask [nblocks of the shard] uint32 into host memory (block order of the shard's code array). */
+int dph_filter_copy_mask(const dph_filter* f, uint32_t* out_host);
+/* Applies f (NULL clears) to every later search of ix -- dph_index_search, search_partial, search_preassigned, search_assigned -- like
+ * dph_index_set_nprobe.  Rejected when f was built for another index.  A search with a stale filter is rejected. */
+int dph_index_set_filter(dph_index* ix, const dph_filter* f);
+
 /* Per-query flags of the last search (device pointer, int32 [n]): bit0 = fast filter could not prove
  * exactness and the query was re-run through the exact kernel. */
 const int32_t* dph_index_last_flags(const dph_index* ix);
