@@ -104,6 +104,13 @@ _SIGS = {
     "dph_filter_bytes": (_i64, [_vp]),
     "dph_filter_copy_mask": (_i32, [_vp, _vp]),
     "dph_index_set_filter": (_i32, [_vp, _vp]),
+    "dph_query_filter_create": (_i32, [C.POINTER(_vp), _vp, _vp, _vp, _vp, _i64, _vp, _i64, _i32]),
+    "dph_query_filter_free": (None, [_vp]),
+    "dph_query_filter_bytes": (_i64, [_vp]),
+    "dph_query_filter_rows": (_i64, [_vp, _i64]),
+    "dph_query_filter_blocks": (_i64, [_vp, _i64]),
+    "dph_query_filter_copy_selector": (_i32, [_vp, _i64, _vp, _vp, _vp]),
+    "dph_index_set_query_filter": (_i32, [_vp, _vp]),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -87,5 +87,6 @@ DPH_API int dph_index_set_filter(dph_index* ix, const dph_filter* f) {
     DPH_CHECK(ix != nullptr, "null index");
     DPH_CHECK(f == nullptr || f->ix == ix, "set_filter: the filter was built for another index; build it with this index's make_filter");
     ix->filter = f;
+    if (f) ix->qfilter = nullptr;         // one active filter per handle
     return 0;
 }

@@ -155,7 +155,8 @@ DPH_API int dph_index_set_resident_lists(dph_index* ix, const int64_t* lists, in
     return 0;
 }
 
-int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G, const uint32_t* mask) {
+int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G, const uint32_t* mask,
+                  const DphQfView* qf) {
     cudaStream_t st = ix->stream;
     const int64_t lo = ix->list_lo, hi = ix->list_hi, np = n * ix->nprobe, sb = ix->region_blocks - ix->res_blocks;
     if (ix->max_stream_blocks > sb) {
@@ -219,7 +220,7 @@ int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float
             view_kernel<<<(unsigned)((shi - slo + 255) / 256), 256, 0, st>>>(view, slo, shi, (const long long*)ix->res_off_dev, lists, spre,
                                                                            (int)nf, ix->res_blocks);
         DPH_CUDA(cudaGetLastError());
-        const DphCodeSrc src{ix->region, view, slo, shi, mask};     // the mask is indexed by the shard's blocks, not the view's
+        const DphCodeSrc src{ix->region, view, slo, shi, mask, qf};     // the filters are indexed by the shard's blocks / lists, not the view's
         if (s == 0) { DPH_TRY(dph_scan_passes(ix, p, src, n, k, D, I, G)); continue; }
         float* hD = ix->hs_D.as<float>(); int64_t* hI = ix->hs_I.as<int64_t>(); uint32_t* hG = ix->hs_G.as<uint32_t>();
         DPH_CUDA(cudaMemcpyAsync(hD, D, nk * 4, cudaMemcpyDeviceToDevice, st));

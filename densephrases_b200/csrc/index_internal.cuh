@@ -91,7 +91,8 @@ struct dph_index {
         grp_cnt, grp_fill, grp_off, grp_blockpre, grp_entries, grp_unitpre, grp_units, grp_udesc, groupwork,   // grouped plan (prep.cu)
         csplit, xsplit, candkeys, cflags, selkeys,
         rb_ids, rb_out, rb_found, ws_q, ws_id, ws_out, ws_xq,        // reconstruct_batch / window_scores staging (host-buffer calls)
-        enc_key, enc_cd, enc_list, enc_codes;                        // encode / add: top-1 coarse result, host-call output staging
+        enc_key, enc_cd, enc_list, enc_codes,                        // encode / add: top-1 coarse result, host-call output staging
+        qfview;                                                      // the search chunk's DphQfView (per-query filter)
     int64_t csplit_lo = -1, csplit_nl = -1;
     int coarse_tc = 1;                 // tensor-core coarse quantizer with exact re-rank (0: always the SIMT sequential-k GEMM)
     int last_group = 1;                // queries per gather used by the last search (1, 2 or 4)
@@ -131,6 +132,9 @@ struct dph_index {
     // the filter later searches apply (dph_index_set_filter; nullptr: none).
     uint64_t layout_version = 0;
     const dph_filter* filter = nullptr;
+    // Per-query filtered search (query_filter.cu, DESIGN.md 3.7): the query filter later searches apply (dph_index_set_query_filter).
+    // At most one of filter and qfilter is set.
+    const dph_query_filter* qfilter = nullptr;
 };
 
 // A row mask of one shard: mask[b] bit l = row l of the shard's code block b is selected.  Valid for ix while ix->layout_version ==
@@ -142,9 +146,33 @@ struct dph_filter {
     int64_t nwords = 0, rows = 0;
 };
 
+// Per-query selectors of one search chunk, on the device (dph_query_filter): assign[q] = query q's selector, -1 = none.  Selector f's
+// blocks of shard list lo + i are entries base[f] + [off[f * stride + i], off[f * stride + i + 1]) of blk (the list's block numbers,
+// ascending) and word (their mask words: bit l = lane l's row is selected).
+struct DphQfView {
+    const int32_t* assign; const uint32_t* off; const long long* base; const uint32_t* blk; const uint32_t* word;
+    long long lo, stride;
+};
+// A per-query filter of one shard (query_filter.cu): F selectors in the CSR of DphQfView, and the selector of each of n queries.
+// Valid for ix while ix->layout_version == version.
+struct dph_query_filter {
+    dph_index* ix = nullptr;
+    uint64_t version = 0;
+    int64_t nsel = 0, n = 0, lo = 0, nl = 0;     // selectors, queries, the shard's first list and its list count
+    int32_t* assign = nullptr;                   // [n] device
+    uint32_t* off = nullptr;                     // [nsel * (nl + 1)] device
+    int64_t* base = nullptr;                     // [nsel + 1] device
+    uint32_t *blk = nullptr, *word = nullptr;    // [nblk] device
+    int64_t nblk = 0;
+    std::vector<int64_t> h_base, rows;           // host copies: base [nsel + 1], selected rows per selector [nsel]
+    DphQfView view(int64_t q0) const { return {assign + q0, off, (const long long*)base, blk, word, (long long)lo, (long long)nl + 1}; }
+};
+
 // Where the scan stage reads the codes of lists [lo, hi): the handle's own blocks, or in host mode the view of one slice.  mask: the
-// active filter's row mask, indexed in the shard's own block numbering (ix->blk_off), or nullptr.
-struct DphCodeSrc { const uint8_t* codes; const long long* blk_off; int64_t lo, hi; const uint32_t* mask; };
+// active filter's row mask, indexed in the shard's own block numbering (ix->blk_off), or nullptr.  qf: the active per-query filter's
+// selectors for the chunk's queries, indexed by list (a device copy of the view: the scan kernel's arguments gain one pointer only), or
+// nullptr.
+struct DphCodeSrc { const uint8_t* codes; const long long* blk_off; int64_t lo, hi; const uint32_t* mask; const DphQfView* qf; };
 
 // Writes list_len / list_start / blk_off of `L` to the device and makes `L` the handle's layout, totals included; the only code
 // that does.
@@ -264,7 +292,8 @@ int dph_launch_merge_shards(const float* Dg, const int64_t* Ig, const uint32_t* 
 int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, int k, float* D, int64_t* I, uint32_t* G);
 // ---- host_codes.cu ----
 // Host mode: the scan stage of one chunk, slice by slice (DESIGN.md 3.5).
-int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G, const uint32_t* mask);
+int dph_host_scan(dph_index* ix, const DphSearchPlan& p, int64_t n, int k, float* D, int64_t* I, uint32_t* G, const uint32_t* mask,
+                  const DphQfView* qf);
 // Host mode after set_lists: the HBM region (stream only) and the resident table (empty).
 int dph_host_lists_ready(dph_index* ix);
 // Host mode after a committed mutation: when a list of the shard changed (its length, so its blocks), the resident set empties and

@@ -693,13 +693,19 @@ struct PlanArgs {
     DphSeg* segs; unsigned* qblocks; int* nseg; float* eps;
     unsigned* gdense;              // nullable: canonical scan position of every (query, probe), dense [n, nprobe] (grouped modes)
     const float2* qparams;         // nullable: quantisation (step, base) -> the grouped filter's extra error term
+    const DphQfView* qf;           // QF: the per-query filter's selectors (device memory)
 };
 // One warp per query.  Writes the COMPACTED list of in-shard, non-empty segments (probe-rank order) to
 // segs[q][0..nseg[q]); gstart stays the canonical scan position over ALL probed lists (tie-break key across shards).
+// QF (per-query filter, DESIGN.md 3.7): a query with a selector has as much work in a list as its selector has blocks there; a list
+// with none is no segment, but its rows still count in the scan positions of the lists after it.
+template <bool QF>
 __global__ void __launch_bounds__(256) plan_segs_kernel(PlanArgs a) {
     const int lane = threadIdx.x & 31;
     const long long q = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     if (q >= a.n) return;
+    int f = -1;
+    if (QF) f = a.qf->assign[q];
     const bool active = a.only_flagged ? (a.only_flagged[q] != 0) : true;
     if (!active) {                                   // fallback plan: nothing to do for queries whose fast filter was proven exact
         if (lane == 0) { a.qblocks[q] = 0u; a.nseg[q] = 0; }
@@ -718,6 +724,7 @@ __global__ void __launch_bounds__(256) plan_segs_kernel(PlanArgs a) {
                 len = a.list_len[l];
                 dmax = fmaxf(dmax, fabsf(d0));
                 if (active && len > 0 && l >= a.list_lo && l < a.list_hi) { nb = (unsigned)((len + 31) >> 5); blk = a.blk_off[l]; }
+                if (QF && nb > 0 && f >= 0) { const uint32_t* o = a.qf->off + (long long)f * a.qf->stride + (l - a.qf->lo); nb = o[1] - o[0]; }
             }
         }
         // warp inclusive scans of len and nb
@@ -983,7 +990,9 @@ int dph_launch_plan(dph_index* ix, const DphSearchPlan& sp, const DphCodeSrc& sr
     a.list_lo = src.lo; a.list_hi = src.hi; a.nprobe = ix->nprobe; a.n = n; a.only_flagged = only_flagged;
     a.lutmax = ix->lutmax.as<float>(); a.segs = ix->segs.as<DphSeg>(); a.qblocks = ix->qinfo.as<unsigned>(); a.nseg = ix->nseg.as<int>(); a.eps = ix->eps.as<float>();
     a.gdense = grouped ? ix->gdense.as<unsigned>() : nullptr; a.qparams = grouped ? ix->qparams.as<float2>() : nullptr;
-    plan_segs_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(a);
+    a.qf = src.qf;
+    if (src.qf) plan_segs_kernel<true><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(a);
+    else plan_segs_kernel<false><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(a);
     DPH_CUDA(cudaGetLastError());
     if (grouped) {
         GroupPlanArgs p;

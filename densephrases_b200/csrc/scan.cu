@@ -32,6 +32,7 @@ struct ScanArgs {
     unsigned* gthr; unsigned long long* cand; const long long* cand_off; int* cand_cnt;
     long long n; int nprobe; int keep;
     const unsigned* mask; const long long* mask_off;     // filtered variants: the row mask, and the shard's first block of each list
+    const DphQfView* qf;                                 // per-query filtered variant: the chunk's selectors (device memory, DESIGN.md 3.7)
 };
 
 #define NT DPH_SCAN_THREADS
@@ -127,6 +128,7 @@ struct SegCursor {
         len = (int)u0.z; gstart = u0.w; dis0 = __uint_as_float(u1.x); wrel = u1.y; wend = u1.z;
     }
     __device__ __forceinline__ const uint4* ptr(unsigned b) const { return base + (size_t)(b - wrel) * (DPH_BLK_BYTES / 16); }
+    __device__ __forceinline__ unsigned j0(unsigned b) const { return (b - wrel) * 32u; }       // the list row of lane 0 of work block b
 };
 // The filtered scan's cursor: also the segment's row of the mask, mrow[b] = the mask word of work block b (the list's block b - wrel,
 // in the shard's block numbering).  The unfiltered scan keeps the plain SegCursor, so its code is what it was.
@@ -138,12 +140,39 @@ struct SegCursorF : SegCursor {
         mrow = a.mask + (a.mask_off[tab[seg].list] - (long long)wrel);
     }
 };
-template <bool FILT> struct ScanCursor { using T = SegCursor; };
-template <> struct ScanCursor<true> { using T = SegCursorF; };
+// The per-query filtered scan's cursor (DESIGN.md 3.7).  A query with a selector (f >= 0) has as many work blocks in a segment as its
+// selector has blocks in the segment's list: work block b is the list's block qblk[b] with the mask word qword[b] (the selector's CSR
+// entries of the list, shifted by wrel).  A query without one (f = -1) walks every block of the list with the word ~0u.  The code
+// address and the row numbers come from the list's block, so the scan positions are those of the unfiltered scan.
+struct SegCursorQ : SegCursor {
+    const unsigned* qblk; const unsigned* qword; int f;
+    __device__ __forceinline__ void seek(const DphSeg* __restrict__ tab, unsigned b, const uint8_t* codes, const ScanArgs& a) {
+        if (b < wend) return;
+        SegCursor::seek(tab, b, codes);
+        if (f >= 0) {
+            const DphQfView& v = *a.qf;
+            const long long e = v.base[f] + (long long)v.off[(long long)f * v.stride + (tab[seg].list - v.lo)] - (long long)wrel;
+            qblk = v.blk + e; qword = v.word + e;
+        }
+    }
+    __device__ __forceinline__ unsigned blk(unsigned b) const { return f >= 0 ? __ldg(qblk + b) : b - wrel; }
+    __device__ __forceinline__ const uint4* ptr(unsigned b) const { return base + (size_t)blk(b) * (DPH_BLK_BYTES / 16); }
+    __device__ __forceinline__ unsigned j0(unsigned b) const { return blk(b) * 32u; }
+};
+// The scan kernel's row filter: none, the batch-wide row mask (3.6) or per-query selectors (3.7).
+enum { DPH_FILT_NONE = 0, DPH_FILT_MASK = 1, DPH_FILT_QUERY = 2 };
+template <int FK> struct ScanCursor { using T = SegCursor; };
+template <> struct ScanCursor<DPH_FILT_MASK> { using T = SegCursorF; };
+template <> struct ScanCursor<DPH_FILT_QUERY> { using T = SegCursorQ; };
 __device__ __forceinline__ void cursor_seek(SegCursor& c, const DphSeg* tab, unsigned b, const uint8_t* codes, const ScanArgs&) { c.seek(tab, b, codes); }
 __device__ __forceinline__ void cursor_seek(SegCursorF& c, const DphSeg* tab, unsigned b, const uint8_t* codes, const ScanArgs& a) { c.seek(tab, b, codes, a); }
+__device__ __forceinline__ void cursor_seek(SegCursorQ& c, const DphSeg* tab, unsigned b, const uint8_t* codes, const ScanArgs& a) { c.seek(tab, b, codes, a); }
 __device__ __forceinline__ unsigned cursor_mask(const SegCursor&, unsigned) { return ~0u; }
 __device__ __forceinline__ unsigned cursor_mask(const SegCursorF& c, unsigned b) { return c.mrow[b]; }
+__device__ __forceinline__ unsigned cursor_mask(const SegCursorQ& c, unsigned b) { return c.f >= 0 ? __ldg(c.qword + b) : ~0u; }
+// Start of query q's range: only the per-query cursor depends on the query (its selector).
+__device__ __forceinline__ void cursor_query(SegCursor&, const ScanArgs&, long long) {}
+__device__ __forceinline__ void cursor_query(SegCursorQ& c, const ScanArgs& a, long long q) { c.f = a.qf->assign[q]; }
 
 __device__ __forceinline__ void block_compact(ScanShared* sh, int keep, unsigned* gthr_q) {
     const int tid = threadIdx.x;
@@ -168,9 +197,11 @@ __device__ __forceinline__ void block_compact(ScanShared* sh, int keep, unsigned
     __syncthreads();
 }
 
-// FILT: a row passes only when its mask bit is set; a block whose mask word is 0 is not prefetched, loaded or scored.
-template <int MODE, bool FILT>
+// FK (DPH_FILT_*): with a filter, a row passes only when its mask bit is set; a block whose mask word is 0 is not prefetched, loaded
+// or scored.  The per-query filter's work blocks are only the selected blocks, so its mask words are never 0.
+template <int MODE, int FK>
 __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
+    constexpr bool FILT = FK != DPH_FILT_NONE;
     unsigned char* const smem = dph_smem;
     constexpr int LUT_BYTES = (MODE == DPH_SCAN_FAST) ? SMEM_LUT_FAST : SMEM_LUT_EXACT;
     ScanShared* sh = reinterpret_cast<ScanShared*>(smem + LUT_BYTES);
@@ -203,8 +234,9 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 
         // segment table of this query: shared memory when it fits (always for nprobe <= 256), else global
         const DphSeg* tab = (a.nseg[q] <= DPH_SEG_SMEM) ? sh->segtab : (a.segs + q * a.nprobe);
-        typename ScanCursor<FILT>::T cc, pc;              // consume / L2-prefetch cursors
+        typename ScanCursor<FK>::T cc, pc;                // consume / L2-prefetch cursors
         cc.init(); pc.init();
+        cursor_query(cc, a, q); cursor_query(pc, a, q);
         unsigned b = b0 + warp;                           // next block this warp consumes
         unsigned bp = b0 + warp;                          // next block this warp prefetches into L2
         uint4 nxt[6];
@@ -225,7 +257,7 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 #pragma unroll
                 for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
             }
-            n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = (b - cc.wrel) * 32u;
+            n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = cc.j0(b);
         }
         // ---- stage this query's LUT into shared memory (twelve 16-byte loads in flight per thread) ----
         {
@@ -284,7 +316,7 @@ __global__ void __launch_bounds__(NT, 1) scan_kernel(ScanArgs a) {
 #pragma unroll
                         for (int c6 = 0; c6 < 6; c6++) nxt[c6] = ldg_stream(p + c6 * 32);
                     }
-                    n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = (b - cc.wrel) * 32u;
+                    n_len = cc.len; n_gstart = cc.gstart; n_dis0 = cc.dis0; n_j0 = cc.j0(b);
                 }
                 if (FILT && c_mask == 0) continue;                 // warp-uniform: no row of the block is selected
                 float score;
@@ -991,9 +1023,9 @@ static int dph_scan_setup_attrs() {
         // the quad scan also needs the window's top address byte to be 0 (its gather addresses are built without it)
         DPH_CHECK(h == DPH_DYN_SMEM_BASE, "dynamic shared memory window does not start at 0x400 on this driver; rebuild with the probed value");
     }
-    for (auto f : {scan_kernel<DPH_SCAN_FAST, false>, scan_kernel<DPH_SCAN_FAST, true>})
+    for (auto f : {scan_kernel<DPH_SCAN_FAST, DPH_FILT_NONE>, scan_kernel<DPH_SCAN_FAST, DPH_FILT_MASK>, scan_kernel<DPH_SCAN_FAST, DPH_FILT_QUERY>})
         DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(ScanShared)));
-    for (auto f : {scan_kernel<DPH_SCAN_EXACT, false>, scan_kernel<DPH_SCAN_EXACT, true>})
+    for (auto f : {scan_kernel<DPH_SCAN_EXACT, DPH_FILT_NONE>, scan_kernel<DPH_SCAN_EXACT, DPH_FILT_MASK>, scan_kernel<DPH_SCAN_EXACT, DPH_FILT_QUERY>})
         DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
     for (auto f : {scan_pair_kernel<false>, scan_pair_kernel<true>})
         DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
@@ -1007,16 +1039,18 @@ int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
     DPH_TRY(dph_scan_setup_attrs());
     const int grid = p.grid, group = p.pass_group(exact), keep = p.pass_keep(exact);
     const bool filt = src.mask != nullptr;          // the row mask is indexed in the shard's own block numbering (ix->blk_off)
+    const bool qfilt = src.qf != nullptr;           // per-query selectors: the one-query scan only (search_plan)
+    DPH_CHECK(group == 1 || !qfilt, "scan: a per-query filter runs the one-query scan only");
     if (group == 1) {
         ScanArgs a;
         a.codes = src.codes; a.qpre = ix->wpre.as<long long>(); a.segs = ix->segs.as<DphSeg>(); a.nseg = ix->nseg.as<int>(); a.work = ix->work.as<DphWork>();
         a.lut_canon = ix->lut_canon.as<float>(); a.gthr = ix->gthr.as<unsigned>();
         a.cand = ix->cand.as<unsigned long long>(); a.cand_off = ix->cand_off.as<long long>(); a.cand_cnt = ix->cand_cnt.as<int>();
         a.n = n; a.nprobe = ix->nprobe; a.keep = keep;
-        a.mask = src.mask; a.mask_off = (const long long*)ix->blk_off;
+        a.mask = src.mask; a.mask_off = (const long long*)ix->blk_off; a.qf = src.qf;
         const size_t smem = (exact ? SMEM_LUT_EXACT : SMEM_LUT_FAST) + sizeof(ScanShared);
-        auto f = exact ? (filt ? scan_kernel<DPH_SCAN_EXACT, true> : scan_kernel<DPH_SCAN_EXACT, false>)
-                       : (filt ? scan_kernel<DPH_SCAN_FAST, true> : scan_kernel<DPH_SCAN_FAST, false>);
+        auto f = exact ? (qfilt ? scan_kernel<DPH_SCAN_EXACT, DPH_FILT_QUERY> : filt ? scan_kernel<DPH_SCAN_EXACT, DPH_FILT_MASK> : scan_kernel<DPH_SCAN_EXACT, DPH_FILT_NONE>)
+                       : (qfilt ? scan_kernel<DPH_SCAN_FAST, DPH_FILT_QUERY> : filt ? scan_kernel<DPH_SCAN_FAST, DPH_FILT_MASK> : scan_kernel<DPH_SCAN_FAST, DPH_FILT_NONE>);
         f<<<grid, NT, smem, st>>>(a);
     } else {
         GroupScanArgs a;

@@ -12,7 +12,8 @@ static int keep_pair(int k) { return k + std::max(k / 2, DPH_KEEP_SLACK); }
 static int keep_quad(int k) { return k + std::max(2 * k, 100); }
 
 // The scan of a batch of n queries.  A grouped mode runs while its keep fits its kernel's candidate buffers: quad for k <= 85,
-// pair for k <= 683, one query per gather above.
+// pair for k <= 683, one query per gather above.  A per-query filter always runs the one-query scan (DESIGN.md 3.7): its queries
+// read few blocks, mostly not the same ones.
 static DphSearchPlan search_plan(const dph_index* ix, int64_t n, int k) {
     // sharing gathers between the queries that probe a list pays when lists are probed by >= ~1.5 queries of the batch on average
     const int64_t eff_probe = std::min<int64_t>(ix->nprobe, ix->nlist);
@@ -27,6 +28,7 @@ static DphSearchPlan search_plan(const dph_index* ix, int64_t n, int k) {
     else if (ix->scan_mode == DPH_SCAN_QUAD || (ix->scan_mode == DPH_SCAN_FAST && shared)) p.group = 4;
     if (p.group == 4 && keep_quad(k) > DPH_QUAD_KEEP_MAX) p.group = 2;
     if (p.group == 2 && keep_pair(k) > DPH_PAIR_KEEP_MAX) p.group = 1;
+    if (ix->qfilter) p.group = 1;
     p.keep = p.group == 4 ? keep_quad(k) : p.group == 2 ? keep_pair(k) : keep_single(k);     // one query: every k fits (scan.cu)
     p.item_q = p.group == 4 ? DPH_QUAD_ITEM_Q : p.group;      // quad: an item runs one code read through two packed tables
     return p;
@@ -119,6 +121,13 @@ int dph_scan_passes(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
 static int active_mask(const dph_index* ix, const uint32_t** mask) {
     const dph_filter* f = ix->filter;
     *mask = nullptr;
+    if (ix->qfilter) {
+        const dph_query_filter* qf = ix->qfilter;
+        DPH_CHECK(qf->ix == ix, "search: the query filter was built for another index; build it with this index's make_query_filters");
+        DPH_CHECK(qf->version == ix->layout_version,
+                  "search: the query filter is stale (the index's lists changed since it was built: set_lists, add, remove, merge or "
+                  "sync_list_len); rebuild the filter");
+    }
     if (!f) return 0;
     DPH_CHECK(f->ix == ix, "search: the filter was built for another index; build it with this index's make_filter");
     DPH_CHECK(f->version == ix->layout_version,
@@ -128,20 +137,36 @@ static int active_mask(const dph_index* ix, const uint32_t** mask) {
     return 0;
 }
 
+// A search of n queries with a per-query filter set needs the filter's n (checked before the search changes anything).
+static int check_query_filter_n(const dph_index* ix, int64_t n) {
+    if (!ix->qfilter) return 0;
+    DPH_CHECK(ix->qfilter->n == n, "search: the query filter was built for " + std::to_string(ix->qfilter->n) + " queries, the batch has " +
+                                   std::to_string(n));
+    return 0;
+}
+
 // Scan stage, from the rotated queries in xr and the probes in (key, cd): the tables, then the passes over the shard's codes -- in
 // host mode slice by slice, the tables built once for all slices.  Every search path passes here, so the active filter applies here.
-static int scan_stage(dph_index* ix, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
+// q0: the chunk's first query in the batch (the row of a per-query filter's assignment).
+static int scan_stage(dph_index* ix, int64_t n, int k, float* D, int64_t* I, uint32_t* G, int64_t q0 = 0) {
     cudaStream_t st = ix->stream;
     const uint32_t* mask;
     DPH_TRY(active_mask(ix, &mask));
+    const DphQfView* qf = nullptr;
+    if (ix->qfilter) {
+        const DphQfView v = ix->qfilter->view(q0);
+        DPH_TRY(ix->qfview.ensure(sizeof(DphQfView)));
+        DPH_CUDA(cudaMemcpyAsync(ix->qfview.p, &v, sizeof v, cudaMemcpyHostToDevice, st));
+        qf = ix->qfview.as<DphQfView>();
+    }
     const DphSearchPlan p = search_plan(ix, n, k);
     DPH_TRY(size_scan(ix, p, n));
     ix->last_group = p.group;
     DPH_TRY(dph_launch_lut(ix->xr.as<float>(), n, ix->pq, ix->lut_canon.as<float>(), ix->lutmax.as<float>(),
                            ix->lutmin.as<float>(), ix->lutmaxv.as<float>(), p.grouped() ? ix->lutq.p : nullptr,
                            p.grouped() ? ix->qparams.as<float2>() : nullptr, st, p.group));
-    if (ix->on_host) return dph_host_scan(ix, p, n, k, D, I, G, mask);
-    const DphCodeSrc src{ix->codes, (const long long*)ix->blk_off, ix->list_lo, ix->list_hi, mask};
+    if (ix->on_host) return dph_host_scan(ix, p, n, k, D, I, G, mask, qf);
+    const DphCodeSrc src{ix->codes, (const long long*)ix->blk_off, ix->list_lo, ix->list_hi, mask, qf};
     return dph_scan_passes(ix, p, src, n, k, D, I, G);
 }
 
@@ -159,19 +184,21 @@ static int64_t chunk_size(const dph_index* ix, int64_t n) {
 
 DPH_API int dph_index_search_partial(dph_index* ix, const float* x_dev, int64_t n, int k, float* D, int64_t* I, uint32_t* G) {
     DPH_TRY(check_ready(ix, k));
+    DPH_TRY(check_query_filter_n(ix, n));
     DPH_CUDA(cudaSetDevice(ix->device));
     reset_fetch(ix);
     const int64_t cs = chunk_size(ix, n);
     for (int64_t o = 0; o < n; o += cs) {
         const int64_t m = std::min(cs, n - o);
         DPH_TRY(coarse_stage(ix, x_dev + o * ix->d, m, nullptr));
-        DPH_TRY(scan_stage(ix, m, k, D + o * k, I + o * k, G + o * k));
+        DPH_TRY(scan_stage(ix, m, k, D + o * k, I + o * k, G + o * k, o));
     }
     return 0;
 }
 
 DPH_API int dph_index_search(dph_index* ix, const float* x, int64_t n, int k, float* D, int64_t* I, int mem) {
     DPH_TRY(check_ready(ix, k));
+    DPH_TRY(check_query_filter_n(ix, n));
     DPH_CUDA(cudaSetDevice(ix->device));
     if (n == 0) return 0;
     DPH_TRY(ix->Gp.ensure((size_t)n * k * 4));
@@ -200,6 +227,7 @@ DPH_API int dph_index_search_preassigned(dph_index* ix, const uint64_t* keys_gat
     DPH_TRY(check_ready(ix, k));
     DPH_CUDA(cudaSetDevice(ix->device));
     DPH_CHECK(n == ix->last_coarse_n, "search_preassigned must follow coarse_local with the same batch");
+    DPH_TRY(check_query_filter_n(ix, n));
     reset_fetch(ix);
     DPH_TRY(size_coarse(ix, n));
     DPH_TRY(dph_launch_coarse_merge((const unsigned long long*)keys_gathered_dev, nshards, n, ix->nprobe, ix->key.as<int32_t>(), ix->cd.as<float>(),
@@ -243,6 +271,7 @@ DPH_API int dph_index_coarse_split(dph_index* ix, const float* x_dev, int64_t n_
 DPH_API int dph_index_search_assigned(dph_index* ix, const float* rec_dev, int64_t n, int k, float* D_dev, int64_t* I_dev, uint32_t* G_dev) {
     DPH_TRY(check_ready(ix, k));
     DPH_CUDA(cudaSetDevice(ix->device));
+    DPH_TRY(check_query_filter_n(ix, n));
     if (n == 0) return 0;
     reset_fetch(ix);
     DPH_TRY(size_coarse(ix, n));

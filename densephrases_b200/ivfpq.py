@@ -28,6 +28,7 @@ class IvfPqIndex:
         self._h = C.c_void_p()
         L.check(L.lib().dph_index_create(C.byref(self._h), d, nlist, M, nbits, device))
         self.device = device
+        self.shard = (0, nlist)             # this handle's lists [lo, hi) (set_shard)
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -80,6 +81,7 @@ class IvfPqIndex:
 
     def set_shard(self, lo, hi):
         L.check(L.lib().dph_index_set_shard(self._h, lo, hi))
+        self.shard = (int(lo), int(hi))
 
     def set_lists(self, list_len, codes, ids=None):
         list_len = np.ascontiguousarray(list_len, dtype=np.int64)
@@ -261,19 +263,66 @@ class IvfPqIndex:
         del keep
         return IndexFilter(self, h)
 
+    def make_query_filters(self, sels, assign=None):
+        """Per-query filters for one batch, for search(..., filter=) -> QueryFilters (DESIGN.md 3.7).  sels: a list of selectors of
+        make_filter (int64 numpy or torch label arrays, or step-1 ranges); assign: int array [n], query i uses sels[assign[i]], -1 = no
+        filter (default: arange(len(sels))).  Row i of a search of n queries with it is exactly search(x[i:i+1], k,
+        filter=make_filter(sels[assign[i]])), or the unfiltered search for -1.  Each selector is held as the blocks of this shard that
+        hold a selected row, with their mask words (8 bytes each) and a 4-byte offset per list of the shard; the scan reads only those
+        blocks.  There is no per-query exclude: make_filter(sel, exclude=True) serves it for the whole batch.  The index is not changed;
+        the filter is valid until its lists change, as an IndexFilter."""
+        sels = list(sels)
+        nsel = len(sels)
+        assign = np.arange(nsel) if assign is None else np.asarray(assign)
+        if assign.ndim != 1 or (assign.size and not np.issubdtype(assign.dtype, np.integer)):
+            raise TypeError("make_query_filters: assign must be a 1-d int array")
+        if assign.size and (assign.min() < -1 or assign.max() >= nsel):
+            raise ValueError(f"make_query_filters: assign entries must be in [-1, {nsel})")
+        assign = np.ascontiguousarray(assign, dtype=np.int32)
+        ranges = np.zeros((nsel, 2), dtype=np.int64)
+        counts = np.zeros(nsel, dtype=np.int64)
+        parts, dev = [], None
+        for i, sel in enumerate(sels):
+            args, keep = self._selector(sel, "make_query_filters")
+            if isinstance(sel, range):
+                ranges[i] = args[2], args[3]
+                continue
+            counts[i] = args[1]
+            if args[4] == L.MEM_DEVICE:
+                dev = keep.device
+            parts.append(keep)
+        label_off = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+        if dev is not None:                     # device labels: concatenated on that device
+            import torch
+            labels = torch.cat([torch.as_tensor(p).to(dev) for p in parts]).contiguous() if parts else None
+            ptr, mem = (labels.data_ptr() if labels is not None and labels.numel() else None), L.MEM_DEVICE
+        else:
+            labels = np.ascontiguousarray(np.concatenate(parts + [np.zeros(0, np.int64)]).astype(np.int64, copy=False))
+            ptr, mem = (_np_ptr(labels) if len(labels) else None), L.MEM_HOST
+        h = C.c_void_p()
+        L.check(L.lib().dph_query_filter_create(C.byref(h), self._h, ptr, _np_ptr(label_off), _np_ptr(ranges), nsel, _np_ptr(assign),
+                                                len(assign), mem))
+        qf = QueryFilters(self, h, nsel, len(assign))
+        qf._spec = (sels, assign)
+        return qf
+
     @contextlib.contextmanager
     def _filtered(self, filter):
-        """The filter applies to the searches inside the block, and to no other."""
+        """The filter (an IndexFilter or QueryFilters) applies to the searches inside the block, and to no other."""
         if filter is None:
             yield
             return
-        if not isinstance(filter, IndexFilter):
-            raise TypeError(f"filter: expected an IndexFilter from make_filter, got {type(filter)!r}")
-        L.check(L.lib().dph_index_set_filter(self._h, filter._h))
+        if isinstance(filter, IndexFilter):
+            set_filter = L.lib().dph_index_set_filter
+        elif isinstance(filter, QueryFilters):
+            set_filter = L.lib().dph_index_set_query_filter
+        else:
+            raise TypeError(f"filter: expected an IndexFilter from make_filter or QueryFilters from make_query_filters, got {type(filter)!r}")
+        L.check(set_filter(self._h, filter._h))
         try:
             yield
         finally:
-            L.lib().dph_index_set_filter(self._h, None)
+            set_filter(self._h, None)
 
     def remove_ids(self, sel):
         """== faiss index.remove_ids(IDSelectorBatch(sel)) for a label array, index.remove_ids(IDSelectorRange(lo, hi)) for
@@ -650,6 +699,65 @@ class IndexFilter:
         """-> uint32 [code blocks of the shard]: bit l of word b = row l of block b is selected (blocks in the shard's list order)."""
         out = np.empty(self.nbytes // 4, dtype=np.uint32)
         L.check(L.lib().dph_filter_copy_mask(self._h, _np_ptr(out)))
+        return out
+
+
+class QueryFilters:
+    """Per-query filters of one IvfPqIndex for one batch of n queries (make_query_filters): nsel selectors, each the shard's blocks that
+    hold a selected row with their mask words, and the selector of every query."""
+
+    def __init__(self, index, h, nsel, n):
+        self.index = index          # the filter belongs to this handle; keeping it alive keeps the handle alive
+        self._h = h
+        self.nsel, self.n = nsel, n
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        index = getattr(self, "index", None)
+        if h and getattr(index, "_h", None) and L is not None and getattr(L, "_lib", None) is not None:   # the handle outlives the filter
+            L._lib.dph_query_filter_free(h)
+
+    def rows(self, i):
+        """Selected rows of the shard by selector i."""
+        if not 0 <= i < self.nsel:
+            raise IndexError(i)
+        return int(L.lib().dph_query_filter_rows(self._h, i))
+
+    @property
+    def nbytes(self):
+        """Device bytes of the filter: 8 per selected block, 4 per list of the shard per selector, the assignment and the bases."""
+        return int(L.lib().dph_query_filter_bytes(self._h))
+
+    def csr(self, i):
+        """Selector i -> (off [lists of the shard + 1] u32, blk [m] u32, word [m] u32): list lo + j's blocks are blk[off[j]:off[j+1]]
+        (ascending block numbers of the list) with their mask words (bit l = lane l's row is selected)."""
+        if not 0 <= i < self.nsel:
+            raise IndexError(i)
+        m = int(L.lib().dph_query_filter_blocks(self._h, i))
+        lo, hi = self.index.shard
+        off = np.empty(hi - lo + 1, dtype=np.uint32)
+        blk, word = np.empty(m, dtype=np.uint32), np.empty(m, dtype=np.uint32)
+        L.check(L.lib().dph_query_filter_copy_selector(self._h, i, _np_ptr(off), _np_ptr(blk), _np_ptr(word)))
+        return off, blk, word
+
+    def for_rows(self, a, b):
+        """The filter of queries a..b-1 of this batch (a new QueryFilters of the same index, holding only the selectors they use)."""
+        sels, assign = self._spec
+        used, sub = np.unique(assign[a:b], return_inverse=True)
+        keep = used >= 0
+        remap = np.full(len(used), -1, dtype=np.int64)
+        remap[keep] = np.arange(int(keep.sum()))
+        return self.index.make_query_filters([sels[i] for i in used[keep]], remap[sub.ravel()])
+
+    def mask(self, i):
+        """Selector i expanded to the row mask of make_filter (uint32 per code block of the shard)."""
+        off, blk, word = self.csr(i)
+        lo, hi = self.index.shard
+        nb = (self.index.list_len()[lo:hi] + 31) // 32
+        first = np.concatenate([[0], np.cumsum(nb)])[:-1]
+        out = np.zeros(int(nb.sum()), dtype=np.uint32)
+        lists = np.repeat(np.arange(hi - lo), np.diff(off.astype(np.int64)))
+        out[first[lists] + blk] = word
         return out
 
 

@@ -232,19 +232,61 @@ class MIPS(object):
             word[sel] = self.idx_f[str(g)]['word'][row[sel]]
         return doc, word
 
+    def _doc_runs(self):
+        """doc -> label runs, built once: (doc, first label, end label) of every run of equal documents in every idx2id group, sorted
+        by document.  A document's phrases are one contiguous run of its group (build_phrase_index.py:231-236); a document split over
+        several runs or groups has several entries."""
+        if getattr(self, '_runs', None) is None:
+            docs, los, his = [], [], []
+            for g, t in self.idx_f.items():
+                d = np.asarray(t['doc'], dtype=np.int64)
+                if len(d) == 0:
+                    continue
+                start = np.flatnonzero(np.concatenate([[True], d[1:] != d[:-1]]))
+                docs.append(d[start])
+                los.append(int(g) + start)
+                his.append(int(g) + np.concatenate([start[1:], [len(d)]]))
+            cat = [np.concatenate(a + [np.zeros(0, np.int64)]).astype(np.int64) for a in (docs, los, his)]
+            order = np.argsort(cat[0], kind='stable')
+            self._runs = tuple(a[order] for a in cat)
+        return self._runs
+
+    def doc_labels(self, doc_ids):
+        """The labels of the phrases of the documents doc_ids (int64, sorted): a phrase's label is its offset group plus its row in that
+        group's idx2id arrays (the inverse of get_idxs)."""
+        rdoc, rlo, rhi = self._doc_runs()
+        docs = np.unique(np.asarray(doc_ids, dtype=np.int64))
+        a, b = np.searchsorted(rdoc, docs, 'left'), np.searchsorted(rdoc, docs, 'right')
+        runs = np.concatenate([np.arange(x, y) for x, y in zip(a, b)] + [np.zeros(0, np.int64)]).astype(np.int64)
+        lens = rhi[runs] - rlo[runs]
+        labels = np.repeat(rlo[runs] - np.concatenate([[0], np.cumsum(lens)[:-1]]), lens) + np.arange(int(lens.sum()))
+        return np.sort(labels.astype(np.int64))
+
     def doc_filter(self, doc_ids, exclude=False):
         """A filter of the index (make_filter) that selects the phrases of the documents doc_ids (exclude=True: of every other
-        document), for search / search_dense(doc_filter=...).  A phrase's label is its offset group plus its row in that group's
-        idx2id arrays (the inverse of get_idxs)."""
-        docs = np.unique(np.asarray(doc_ids, dtype=np.int64))
-        labels = [int(g) + np.flatnonzero(np.isin(t['doc'], docs)) for g, t in self.idx_f.items()]
-        return self.index.make_filter(np.concatenate(labels + [np.zeros(0, np.int64)]).astype(np.int64), exclude=exclude)
+        document), for search / search_dense(doc_filter=...)."""
+        return self.index.make_filter(self.doc_labels(doc_ids), exclude=exclude)
+
+    def doc_filters(self, per_question):
+        """Per-question document filters (make_query_filters) for search / search_dense(doc_filter=...) of B questions:
+        per_question[i] is a doc-id array, or None for no filter.  The search stacks the start and end halves into 2B rows, so rows i
+        and B + i share question i's selector."""
+        per_question = list(per_question)
+        sels, sel_of = [], []
+        for docs in per_question:
+            if docs is None:
+                sel_of.append(-1)
+            else:
+                sel_of.append(len(sels))
+                sels.append(self.doc_labels(docs))
+        assign = np.asarray(sel_of + sel_of, dtype=np.int64)
+        return self.index.make_query_filters(sels, assign)
 
     def search_dense(self, query, q_texts, nprobe=256, top_k=10, doc_filter=None):
         """Start and end halves of `query [B, 2d]` are stacked into one [2B, d] search (index.py:195-202).
         `nprobe` is accepted and ignored, like the reference (its assignment is commented out at index.py:191).
-        doc_filter (doc_filter()): only phrases of the selected documents are hits; a query may then get fewer than top_k, and the
-        padded slots (label -1) get document and word -1, which the phrase stage drops."""
+        doc_filter (doc_filter(), or doc_filters() for these B questions): only phrases of the selected documents are hits; a query may
+        then get fewer than top_k, and the padded slots (label -1) get document and word -1, which the phrase stage drops."""
         B = query.shape[0]
         tic = time()
         kw = {} if doc_filter is None else {'filter': doc_filter}
@@ -464,8 +506,9 @@ class MIPS(object):
                nprobe=256, top_k=10,
                aggregate=False, return_idxs=False,
                max_answer_length=10, agg_strat='opt1', return_sent=False, doc_filter=None):
-        """query [B, 2*768] (start || end) -> list[B] of result dicts sorted by score (index.py:450-482).  doc_filter (doc_filter()):
-        only phrases of the selected documents are hits (search_dense); the phrase windows around a hit are not filtered."""
+        """query [B, 2*768] (start || end) -> list[B] of result dicts sorted by score (index.py:450-482).  doc_filter (doc_filter(),
+        or doc_filters() per question): only phrases of the selected documents are hits (search_dense); the phrase windows around a hit
+        are not filtered."""
         tic = time()
         dense = self.search_dense(query, q_texts=q_texts, nprobe=nprobe, top_k=top_k, doc_filter=doc_filter)
         s_doc, s_word, s_lab, e_doc, e_word, e_lab, s_sc, e_sc = dense

@@ -300,7 +300,9 @@ class DensePhrases(object):
             evaluate_fn = evaluate
         return evaluate_fn(new_args, self.mips, self.model, self.tokenizer)
 
-    def search(self, query='', retrieval_unit='phrase', top_k=10, truecase=True, return_meta=False):
+    def search(self, query='', retrieval_unit='phrase', top_k=10, truecase=True, return_meta=False, doc_filter=None):
+        """doc_filter (optional): restrict hits to documents -- one doc-id array for every question, or one entry per question (a
+        doc-id array, or None for no restriction)."""
         single = isinstance(query, str)
         batch_query = [query] if single else query
         assert isinstance(batch_query, list)
@@ -318,8 +320,14 @@ class DensePhrases(object):
             outs = self.query2vec(batch_query)
             query_vec = np.concatenate([np.concatenate([o[0] for o in outs], 0), np.concatenate([o[1] for o in outs], 0)], 1)
         search_top_k = top_k * 2 if retrieval_unit in ('sentence', 'paragraph', 'document') else top_k
+        kw = {}
+        if doc_filter is not None:
+            per_question = isinstance(doc_filter, (list, tuple)) and not (len(doc_filter) and np.isscalar(doc_filter[0]))
+            if per_question and len(doc_filter) != len(batch_query):
+                raise ValueError(f'doc_filter: {len(doc_filter)} entries for {len(batch_query)} questions')
+            kw['doc_filter'] = self.mips.doc_filters(doc_filter) if per_question else self.mips.doc_filter(doc_filter)
         rets = self.mips.search(query_vec, q_texts=batch_query, nprobe=256, top_k=search_top_k, max_answer_length=10, return_idxs=False,
-                                aggregate=True, agg_strat=self._AGG[retrieval_unit], return_sent=retrieval_unit == 'sentence')
+                                aggregate=True, agg_strat=self._AGG[retrieval_unit], return_sent=retrieval_unit == 'sentence', **kw)
         rets = [ret[:top_k] for ret in rets]
         field = {'phrase': lambda r: r['answer'], 'sentence': lambda r: r['context'], 'paragraph': lambda r: r['context'],
                  'document': lambda r: r['title'][0]}[retrieval_unit]

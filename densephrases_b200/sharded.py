@@ -7,7 +7,7 @@ With world_size 1 it degenerates to IvfPqIndex.  This is the call a user (MIPS.s
 import numpy as np
 import torch
 
-from .ivfpq import IvfPqIndex, default_stream_bytes, merge_shards, merge_shards_packed, pack_topk
+from .ivfpq import IvfPqIndex, QueryFilters, default_stream_bytes, merge_shards, merge_shards_packed, pack_topk
 
 
 def shard_ranges(list_len, world):
@@ -197,6 +197,11 @@ class ShardedIvfPq:
         selector."""
         return self.local.make_filter(sel, exclude)
 
+    def make_query_filters(self, sels, assign=None):
+        """Per-query filters for search / search_device (IvfPqIndex.make_query_filters): every rank builds the filter of its own shard
+        from the same selectors, with no exchange.  A collective by convention: every rank passes the same selectors and assignment."""
+        return self.local.make_query_filters(sels, assign)
+
     def set_resident_lists(self, lists):
         """Host mode: every rank keeps in device memory the given lists that fall in its own range (IvfPqIndex.set_resident_lists)."""
         lists = np.asarray(lists, dtype=np.int64).ravel()
@@ -253,20 +258,21 @@ class ShardedIvfPq:
         return self.world > 1 and (self.query_split is True or (self.query_split is None and use_query_split(n, self.world, self.local.nlist)))
 
     def _local_steps(self, filter):
-        """This rank's search steps of both protocols, with `filter` (make_filter) applied to each."""
+        """This rank's search steps of both protocols, with `filter` (make_filter or make_query_filters) applied to each."""
         if filter is None:
             return self.local.search_assigned, self.local.search_preassigned
         return (lambda rec, k: self.local.search_assigned(rec, k, filter=filter),
                 lambda keys, k: self.local.search_preassigned(keys, k, filter=filter))
 
     def search_device(self, x, k, filter=None):
-        """x torch cuda [n,d] (same on every rank) -> (D, I) torch cuda [n,k] (same on every rank).  filter (make_filter): only
-        selected rows can be results (IvfPqIndex.search)."""
+        """x torch cuda [n,d] (same on every rank) -> (D, I) torch cuda [n,k] (same on every rank).  filter (make_filter, or
+        make_query_filters for these n queries): only selected rows can be results (IvfPqIndex.search)."""
         if self.world == 1:
             return self.local.search(x, k, filter=filter)
         n = x.shape[0]
-        if n > 4096:        # one chunk per collective round
-            parts = [self.search_device(x[i:i + 4096], k, filter) for i in range(0, n, 4096)]
+        if n > 4096:        # one chunk per collective round; a per-query filter is cut to each chunk's rows
+            per = (lambda i: filter.for_rows(i, i + 4096)) if isinstance(filter, QueryFilters) else (lambda i: filter)
+            parts = [self.search_device(x[i:i + 4096], k, per(i)) for i in range(0, n, 4096)]
             return torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts])
         assigned, preassigned = self._local_steps(filter)
         if self._qsplit(n):

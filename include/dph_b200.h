@@ -282,6 +282,32 @@ int dph_filter_copy_mask(const dph_filter* f, uint32_t* out_host);
  * dph_index_set_nprobe.  Rejected when f was built for another index.  A search with a stale filter is rejected. */
 int dph_index_set_filter(dph_index* ix, const dph_filter* f);
 
+/* ---- per-query filters (a different IDSelector per query of one batch; DESIGN.md 3.7 "Per-query filters") ----
+ * A query filter holds nsel label selectors and the selector assign[q] of each of the n queries of one batch (-1: the query is not
+ * filtered).  A search of those n queries with it set (dph_index_set_query_filter) computes row q exactly as the search of query q alone
+ * with the row mask of its selector (dph_filter_create, exclude = 0), or unfiltered for -1: D bits and I.  Each selector is held sparse:
+ * per list of the shard, the ascending numbers of the list's blocks that hold a selected row, with their mask words -- 8 bytes per
+ * selected block, plus a 4-byte offset per list of the shard per selector.  Selector s is the label set labels[label_off[s] ..
+ * label_off[s + 1]) (labels in `mem`; any order, duplicates allowed, absent or negative labels match nothing), or, when ranges is not
+ * NULL and (ranges[2s], ranges[2s + 1]) != (0, 0), the label range [ranges[2s], ranges[2s + 1]) -- not both; neither selects nothing.
+ * label_off [nsel + 1], ranges [2 nsel] and assign [n] are host arrays; label_off may be NULL when every selector is a range.
+ * Rejected (nothing created) when an assign entry is outside [-1, nsel) or a selector has both forms.  Built on the device in one
+ * call for all selectors; the index is not changed.  It belongs to ix and ix's current list layout, as a dph_filter does.
+ * Synchronises the stream.  exclude has no per-query form: use a dph_filter for it. */
+typedef struct dph_query_filter dph_query_filter;
+int dph_query_filter_create(dph_query_filter** out, dph_index* ix, const int64_t* labels, const int64_t* label_off, const int64_t* ranges,
+                            int64_t nsel, const int32_t* assign, int64_t n, int mem);
+void dph_query_filter_free(dph_query_filter* f);          /* a query filter set on its index is cleared there */
+int64_t dph_query_filter_bytes(const dph_query_filter* f);                  /* device bytes of the filter */
+int64_t dph_query_filter_rows(const dph_query_filter* f, int64_t s);        /* selected rows of the shard by selector s */
+int64_t dph_query_filter_blocks(const dph_query_filter* f, int64_t s);      /* blocks held for selector s */
+/* Selector s's CSR into host memory: off [lists of the shard + 1] (list lo + i's entries are [off[i], off[i + 1])), blk and word
+ * [dph_query_filter_blocks(f, s)]: the list's block number and its mask word. */
+int dph_query_filter_copy_selector(const dph_query_filter* f, int64_t s, uint32_t* off_out, uint32_t* blk_out, uint32_t* word_out);
+/* Applies f (NULL clears) to every later search of ix, as dph_index_set_filter; it replaces a dph_filter set on ix (and that one
+ * replaces it).  A search whose batch is not f's n queries is rejected, and so is one with a stale filter. */
+int dph_index_set_query_filter(dph_index* ix, const dph_query_filter* f);
+
 /* Per-query flags of the last search (device pointer, int32 [n]): bit0 = fast filter could not prove
  * exactness and the query was re-run through the exact kernel. */
 const int32_t* dph_index_last_flags(const dph_index* ix);
