@@ -70,8 +70,6 @@ _SIGS = {
     "dph_sgemm_nt_seq": (_i32, [_vp, _i64, _vp, _i64, _i64, _vp, _vp]),
     "dph_gemm_tf32_nt": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp]),
     "dph_encoder_set_precision": (_i32, [_vp, _i32]),
-    "dph_gemm_tf32_set_mode": (_i32, [_i32]),
-    "dph_set_tuning": (_i32, [_i32, _i32]),
     "dph_encoder_set_attention": (_i32, [_vp, _i32]),
     "dph_attention_bert": (_i32, [_vp, _vp, _i32, _i32, _vp, _i32, _vp]),
     "dph_index_window_scores": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _i32]),

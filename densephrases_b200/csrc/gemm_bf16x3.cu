@@ -84,6 +84,6 @@ int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const
     ap.M = M; ap.N = N; ap.K = K; ap.act = act;
     ap.tiles_m = tm; ap.tiles_n = N / BN; ap.total_tiles = group * tm * ap.tiles_n;
     const int grid = ap.total_tiles < num_sms ? ap.total_tiles : num_sms;
-    if (BN == 256) return gw_launch<GW_BF16X3, 128, 2, 1, 4>(mp, ap, grid, st);
-    return gw_launch<GW_BF16X3, 192, 1, 1, 4>(mp, ap, grid, st);
+    if (BN == 256) return gw_launch<GW_BF16X3, 128, 2, 4>(mp, ap, grid, st);
+    return gw_launch<GW_BF16X3, 192, 1, 4>(mp, ap, grid, st);
 }

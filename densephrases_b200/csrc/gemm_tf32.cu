@@ -5,8 +5,8 @@
 // fp32 operands in shared memory, wgmma kind tf32 (the precision torch 1.9 -- the reference's pin -- used for fp32 matmuls on
 // Ampere+ by default), fp32 accumulators in registers; the kernel itself is gemm_wgmma_kernel (gemm_wgmma.cuh).
 //
-// Three schedules of the same wgmma sequence (dph_gemm_tf32_set_mode; bit-identical outputs): one 128 x 128 tile per CTA (also
-// the 3xTF32 split kernel), the same as 2-CTA clusters sharing the A tile by TMA multicast, and persistent 128 x 256 tiles (default).
+// Two schedules of the same wgmma sequence (bit-identical outputs): persistent 128 x 256 tiles, one CTA per SM, when N % 256 == 0,
+// else one 128 x 128 tile per CTA (also the 3xTF32 split kernel).
 #include "gemm_wgmma.cuh"
 #include "../../include/dph_b200.h"
 
@@ -64,11 +64,6 @@ int dph_launch_gemm_bf16x3(int group, const void* const* A_hi, const void* const
                            const float* const* bias, const float* const* residual, float* const* out, void* const* out_hi, void* const* out_lo,
                            int M, int N, int K, int act, cudaStream_t st);
 
-// how 1xTF32 GEMMs are scheduled: 0 one 128x128 tile per CTA; 1 the same as 2-CTA clusters sharing the A tile by TMA multicast
-// (needs an even number of N tiles); 2 persistent 128x256 tiles, one CTA per SM (needs N % 256 == 0)
-static int g_gemm_mode = 2;
-DPH_API int dph_gemm_tf32_set_mode(int mode) { DPH_CHECK(mode >= 0 && mode <= 2, "gemm mode 0..2"); g_gemm_mode = mode; return 0; }
-
 // Grouped launch used by the encoder: problems share M, N, K and the epilogue; pointers are device pointers.
 // A_lo / W_lo non-null -> 3xTF32 mode (A, W are then the hi parts).
 int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W, const float* const* bias, const float* const* residual,
@@ -76,8 +71,7 @@ int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W
     DPH_CHECK(group >= 1 && group <= GW_MAX_GROUP, "gemm group size");
     DPH_CHECK(N % 128 == 0 && K % GW_BK == 0 && M >= 1, "gemm_tf32 needs N % 128 == 0 and K % 32 == 0");
     const bool split = A_lo != nullptr && W_lo != nullptr;
-    const bool persist = !split && g_gemm_mode == 2 && N % 256 == 0;
-    const bool cluster = !split && g_gemm_mode == 1 && ((N / 128) % 2 == 0);
+    const bool persist = !split && N % 256 == 0;
     const int BN = persist ? 256 : 128;
     GwMaps maps;
     GwArgs args;
@@ -85,8 +79,7 @@ int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W
         const int s = g < group ? g : 0;
         DPH_TRY(dph_make_map_f32(&maps.a[g], A[s], M, K, K, GW_BM));
         DPH_TRY(dph_make_map_f32(&maps.b[g], W[s], N, K, K, BN));
-        if (cluster) DPH_TRY(dph_make_map_f32(&maps.a2[g], A[s], M, K, K, GW_BM / 2));
-        else DPH_TRY(dph_make_map_f32(&maps.a2[g], split ? A_lo[s] : A[s], M, K, K, GW_BM));
+        DPH_TRY(dph_make_map_f32(&maps.a2[g], split ? A_lo[s] : A[s], M, K, K, GW_BM));
         DPH_TRY(dph_make_map_f32(&maps.b2[g], split ? W_lo[s] : W[s], N, K, K, BN));
         args.bias[g] = bias ? bias[s] : nullptr;
         args.residual[g] = residual ? residual[s] : nullptr;
@@ -95,13 +88,12 @@ int dph_launch_gemm_tf32(int group, const float* const* A, const float* const* W
     }
     args.M = M; args.N = N; args.K = K; args.act = act;
     args.tiles_m = (M + GW_BM - 1) / GW_BM; args.tiles_n = N / BN; args.total_tiles = group * args.tiles_m * args.tiles_n;
-    if (split) return gw_launch<GW_TF32X3, 128, 1, 1, 3>(maps, args, args.total_tiles, st);
-    if (cluster) return gw_launch<GW_TF32, 128, 1, 2, 4>(maps, args, args.total_tiles, st);
-    if (!persist) return gw_launch<GW_TF32, 128, 1, 1, 4>(maps, args, args.total_tiles, st);
+    if (split) return gw_launch<GW_TF32X3, 128, 1, 3>(maps, args, args.total_tiles, st);
+    if (!persist) return gw_launch<GW_TF32, 128, 1, 4>(maps, args, args.total_tiles, st);
     int dev = 0, num_sms = 0;
     DPH_CUDA(cudaGetDevice(&dev));
     DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    return gw_launch<GW_TF32, 128, 2, 1, 4>(maps, args, args.total_tiles < num_sms ? args.total_tiles : num_sms, st);
+    return gw_launch<GW_TF32, 128, 2, 4>(maps, args, args.total_tiles < num_sms ? args.total_tiles : num_sms, st);
 }
 
 // C ABI (test / standalone use): out [M,N] = act(A [M,K] . W[N,K]^T + bias) + residual, device pointers, fp32 in/out.

@@ -6,13 +6,11 @@
 // each own 64 rows of the tile and issue m64 x WN wgmmas from shared memory into fp32 register accumulators, then run the epilogue
 // (bias / erf-GELU / residual -> fp32 rows and/or the (hi, lo) bf16 planes the next bf16x3 layer consumes) straight from the
 // registers.  The producer runs ahead across tile boundaries, so the next tile's operands stream in during the epilogue.
-// Every output element sees the same wgmma sequence whatever the schedule (tile per CTA, 2-CTA cluster, persistent), so the
-// schedules are bit-identical.
+// Every output element sees the same wgmma sequence whatever the schedule (tile per CTA, persistent), so the schedules are
+// bit-identical.
 //
 // KIND: GW_TF32 one TF32 MMA per product; GW_TF32X3 / GW_BF16X3: each operand arrives as an exact (hi, lo) pair and the kernel
 // accumulates hi.lo + lo.hi + hi.hi (small cross terms first) in one fp32 accumulator.
-// CL == 2: the two CTAs of a cluster are neighbours along N (same m block): each loads half of the shared A tile and multicasts it
-// to both, so a stage may be refilled only when the consumers of BOTH CTAs have released it (empty barriers count 2 x CL arrivals).
 #pragma once
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
@@ -23,7 +21,7 @@
 #define GW_THREADS 384
 enum { GW_TF32 = 0, GW_TF32X3 = 1, GW_BF16X3 = 2 };
 
-// a2 / b2: the lo planes (split kinds); in the cluster variant a2 is A with a 64-row box
+// a2 / b2: the lo planes (split kinds)
 struct GwMaps { CUtensorMap a[GW_MAX_GROUP], b[GW_MAX_GROUP], a2[GW_MAX_GROUP], b2[GW_MAX_GROUP]; };
 struct GwArgs {
     const float* bias[GW_MAX_GROUP]; const float* residual[GW_MAX_GROUP];
@@ -52,10 +50,9 @@ __device__ __forceinline__ void gw_mma(float (&d)[WN / 2], unsigned long long a,
     else wgmma_tf32<WN>(d, a, b, acc);
 }
 
-template <int KIND, int WN, int NSUB, int CL, int STAGES>
+template <int KIND, int WN, int NSUB, int STAGES>
 __global__ void __launch_bounds__(GW_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ GwMaps maps, const GwArgs args) {
     using C = GwCfg<KIND, WN, NSUB, STAGES>;
-    static_assert(CL == 1 || KIND == GW_TF32, "cluster variant: 1xTF32 only");
     constexpr int KSTEP_BYTES = 32;                                 // k = 8 tf32 or 16 bf16 per wgmma
     extern __shared__ unsigned char gw_raw[];
     unsigned char* gsm = (unsigned char*)((((unsigned long long)gw_raw) + 1023ull) & ~1023ull);   // swizzle atoms: 1024-byte aligned
@@ -66,12 +63,10 @@ __global__ void __launch_bounds__(GW_THREADS, 1) gemm_wgmma_kernel(const __grid_
     const int per_group = args.tiles_m * args.tiles_n;
 
     if (tid == 0) {
-        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2 * CL); }
+        for (int s = 0; s < STAGES; s++) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 2); }   // empty: both consumer warpgroups
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    unsigned crank = 0;
-    if (CL == 2) { crank = cluster_ctarank(); cluster_sync_all(); }      // the peer's barriers are initialised before anything signals them
 
     if (wg == 0) {
         if (tid == 0) {
@@ -83,8 +78,7 @@ __global__ void __launch_bounds__(GW_THREADS, 1) gemm_wgmma_kernel(const __grid_
                     mbar_wait(empty0 + 8 * s, ph ^ 1u);
                     mbar_expect_tx(full0 + 8 * s, C::STAGE_BYTES);
                     const unsigned dst = stage0 + s * C::STAGE_BYTES, full = full0 + 8 * s;
-                    if (CL == 2) tma_load_2d_mc(dst + crank * (C::A_BYTES / 2), &maps.a2[g], kb * GW_BK, m_blk * GW_BM + (int)crank * (GW_BM / 2), full, (unsigned short)3);
-                    else tma_load_2d(dst, &maps.a[g], kb * GW_BK, m_blk * GW_BM, full);
+                    tma_load_2d(dst, &maps.a[g], kb * GW_BK, m_blk * GW_BM, full);
                     tma_load_2d(dst + C::A_BYTES, &maps.b[g], kb * GW_BK, n_blk * C::BN, full);
                     if (C::PLANES == 2) {
                         tma_load_2d(dst + C::A_BYTES + C::B_BYTES, &maps.a2[g], kb * GW_BK, m_blk * GW_BM, full);
@@ -97,11 +91,7 @@ __global__ void __launch_bounds__(GW_THREADS, 1) gemm_wgmma_kernel(const __grid_
         const int cw = wg - 1;                                       // rows 64 cw .. 64 cw + 63 of the tile
         const int warp = (tid >> 5) & 3, lane = tid & 31;
         const bool leader = (tid & 127) == 0;
-        auto release = [&](unsigned s) {
-            if (!leader) return;
-            if (CL == 2) { mbar_arrive_cluster(empty0 + 8 * s, 0); mbar_arrive_cluster(empty0 + 8 * s, 1); }
-            else mbar_arrive(empty0 + 8 * s);
-        };
+        auto release = [&](unsigned s) { if (leader) mbar_arrive(empty0 + 8 * s); };
         float acc[NSUB][WN / 2];
         unsigned it = 0;
         for (int t = blockIdx.x; t < args.total_tiles; t += gridDim.x) {
@@ -177,26 +167,16 @@ __global__ void __launch_bounds__(GW_THREADS, 1) gemm_wgmma_kernel(const __grid_
             }
         }
     }
-    if (CL == 2) cluster_sync_all();       // the peer may still multicast into this CTA's shared memory / signal its barriers
 }
 
-// Launch with `grid` CTAs (grid < total_tiles: persistent); CL == 2 launches clusters of two CTAs along x.
-template <int KIND, int WN, int NSUB, int CL, int STAGES>
+// Launch with `grid` CTAs (grid < total_tiles: persistent).
+template <int KIND, int WN, int NSUB, int STAGES>
 static int gw_launch(const GwMaps& maps, const GwArgs& args, int grid, cudaStream_t st) {
-    auto kern = gemm_wgmma_kernel<KIND, WN, NSUB, CL, STAGES>;
+    auto kern = gemm_wgmma_kernel<KIND, WN, NSUB, STAGES>;
     constexpr int smem = GwCfg<KIND, WN, NSUB, STAGES>::SMEM;
     static DphPerDeviceOnce once;
     if (once.first()) DPH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    if (CL == 1) {
-        kern<<<grid, GW_THREADS, smem, st>>>(maps, args);
-    } else {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(grid); cfg.blockDim = dim3(GW_THREADS); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = CL; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-        cfg.attrs = at; cfg.numAttrs = 1;
-        DPH_CUDA(cudaLaunchKernelEx(&cfg, kern, maps, args));
-    }
+    kern<<<grid, GW_THREADS, smem, st>>>(maps, args);
     DPH_CUDA(cudaGetLastError());
     return 0;
 }

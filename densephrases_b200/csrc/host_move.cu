@@ -63,7 +63,7 @@ int dph_host_capacity_check(const dph_index* ix, const DphLayout& nw, const char
 
 DphHostMover::~DphHostMover() {
     for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
-    if (ws && ws != rs) cudaStreamDestroy(ws);
+    if (ws) cudaStreamDestroy(ws);
     if (rs) cudaStreamDestroy(rs);
 }
 
@@ -73,8 +73,7 @@ int DphHostMover::prepare(dph_index* ix, DevTmp& tmp, int64_t blocks, const char
     DPH_TRY(tmp.alloc(&buf[0], (size_t)chunk_blocks * DPH_BLK_BYTES, oom));
     DPH_TRY(tmp.alloc(&buf[1], (size_t)chunk_blocks * DPH_BLK_BYTES, oom));
     DPH_CUDA(cudaStreamCreateWithFlags(&rs, cudaStreamNonBlocking));
-    if (g_dph_tune[3]) ws = rs;                       // measurement hook: gathers and write-backs on one stream, no overlap
-    else DPH_CUDA(cudaStreamCreateWithFlags(&ws, cudaStreamNonBlocking));
+    DPH_CUDA(cudaStreamCreateWithFlags(&ws, cudaStreamNonBlocking));
     DPH_CUDA(cudaEventCreate(&ev[0]));
     DPH_CUDA(cudaEventCreate(&ev[1]));
     for (int i = 2; i < 6; i++) DPH_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));

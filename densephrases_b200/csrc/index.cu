@@ -8,12 +8,6 @@ static thread_local std::string g_err;
 void dph_set_error(const std::string& msg) { g_err = msg; }
 DPH_API const char* dph_last_error(void) { return g_err.c_str(); }
 DPH_API int dph_version(void) { return 103; }
-int g_dph_tune[8] = {1, 0, 0, 0, 0, 0, 0, 0};      // [0] quad-scan IMAD level, [1] SGEMM tile (0 auto), [2] PQ-table kernel shape (0 auto)
-DPH_API int dph_set_tuning(int knob, int value) {
-    DPH_CHECK(knob >= 0 && knob < 8, "dph_set_tuning: unknown knob");
-    g_dph_tune[knob] = value;
-    return 0;
-}
 
 int DevBuf::ensure(size_t bytes) {
     if (bytes <= cap) return 0;

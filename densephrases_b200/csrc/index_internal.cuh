@@ -261,8 +261,6 @@ struct DphSearchPlan {
     int pass_keep(bool exact) const { return exact ? k : keep; }
 };
 
-// process-wide variant selection (dph_set_tuning, measurement hook): [0] quad-scan IMAD level, [1] SGEMM tile
-extern int g_dph_tune[8];
 // ---- prep.cu ----
 int dph_launch_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m, int K, float* out, cudaStream_t st);
 int dph_launch_coarse_select(const float* S, int64_t n, int64_t nlist, int nprobe, int32_t* key, float* cd, cudaStream_t st,
@@ -278,7 +276,7 @@ int dph_launch_lut(const float* xr, int64_t n, const float* pq, float* lut_canon
 int dph_launch_plan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, bool exact, const int32_t* only_flagged,
                     cudaStream_t st);
 // ---- scan.cu ----
-// One pass: scan_kernel<EXACT> (exact), else by p.group scan_kernel<FAST>, scan_pair_kernel or scan_quad_kernel<IMADL>.
+// One pass: scan_kernel<EXACT> (exact), else by p.group scan_kernel<FAST>, scan_pair_kernel or scan_quad_kernel.
 int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src, int64_t n, bool exact, cudaStream_t st);
 // Labels are read through the shard's own layout (ix->blk_off), the codes of the exact re-scoring from `codes`.
 int dph_launch_merge(dph_index* ix, const uint8_t* codes, int64_t n, int k, int mode, const int32_t* only_flagged, float* D, int64_t* I,

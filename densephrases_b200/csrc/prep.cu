@@ -257,21 +257,20 @@ int dph_launch_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m
     if (n == 0 || m == 0) return 0;
     const bool k64 = (K % GRK) == 0;                       // the row-tiled kernels step k by 64
     dim3 grid((unsigned)((m + GBN - 1) / GBN), (unsigned)((n + GBM - 1) / GBM));
-    const int variant = g_dph_tune[1];
     int dev = 0, num_sms = 0;
     DPH_CUDA(cudaGetDevice(&dev));
     DPH_CUDA(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    if (variant == 1 || (variant == 0 && (long long)grid.x * grid.y >= 2 * num_sms)) {
+    if ((long long)grid.x * grid.y >= 2 * num_sms) {
         sgemm_nt_seq_kernel<<<grid, 256, 0, st>>>(X, n, W, m, K, out);
         DPH_CUDA(cudaGetLastError());
         return 0;
     }
     // pick the LARGEST tile that still gives >= 128 CTAs: with fewer CTAs than SMs the smaller tiles' extra parallelism outweighs
-    // their lower reuse (compare the variants with tools/bench_variants.py sgemm)
+    // their lower reuse
     const long long ct = (m + 63) / 64;
-    if (!k64 || variant == 2 || (variant == 0 && ct * ((n + 63) / 64) >= 128)) {
+    if (!k64 || ct * ((n + 63) / 64) >= 128) {
         sgemm_nt_seq_small_kernel<<<dim3((unsigned)ct, (unsigned)((n + 63) / 64)), 256, 0, st>>>(X, n, W, m, K, out);
-    } else if (variant == 3 || (variant == 0 && ct * ((n + 31) / 32) >= 128)) {
+    } else if (ct * ((n + 31) / 32) >= 128) {
         sgemm_nt_seq_rows_kernel<2><<<dim3((unsigned)ct, (unsigned)((n + 31) / 32)), 256, 0, st>>>(X, n, W, m, K, out);
     } else {
         sgemm_nt_seq_rows_kernel<1><<<dim3((unsigned)ct, (unsigned)((n + 15) / 16)), 256, 0, st>>>(X, n, W, m, K, out);
@@ -538,12 +537,13 @@ int dph_launch_coarse_select(const float* S, int64_t n, int64_t nlist, int nprob
 // sub-quantizer, from L2) is used for four queries, so the L2 -> SM stream is n/4 x 786 KB instead of n x 786 KB (at 1024 queries per
 // batch that stream -- 805 MB -- was what the kernel's 128 us were spent on, not the 100 MB of table writes).
 #define LUT_TILE_LD 257                                  // [query][sub-quantizer][code] tile, code rows padded: conflict-free both ways
-// LQ queries x MS sub-quantizers per CTA (MS = 32 or 16; grid.y = 96 / MS).  <4, 32> reads n/4 x 786 KB of codebook; <8, 16> has the same
-// 131 KB tile and half that stream (every codebook entry serves eight queries), its table rows are written as 64-byte runs.
-template <int LQ, int MS>
+// LQ = 4 queries x MS = 32 sub-quantizers per CTA (grid.y = 96 / MS).  Eight queries x 16 sub-quantizers (the same 131 KB tile, half
+// the codebook stream) was no faster on one shard of C4 (1024 queries; rank step 4.499 vs 4.500 ms at nprobe 256, 1.500 vs 1.479 ms at
+// nprobe 32): the kernel is bound by its per-CTA latency chain, not by the codebook stream.
 __global__ void __launch_bounds__(256) lut_kernel(const float* __restrict__ xr, const float* __restrict__ pq, long long n,
                                                    float* __restrict__ lut_canon,
                                                    float* __restrict__ lutmax, float* __restrict__ lutmin, float* __restrict__ lutmaxv) {
+    constexpr int LQ = 4, MS = 32;
     extern __shared__ __align__(16) float lut_sm[];
     float* __restrict__ tile = lut_sm;                    // [LQ][MS][LUT_TILE_LD]
     __shared__ __align__(16) float xs[LQ * MS * 8];       // a separate object: stores to `tile` cannot alias it, loads can be hoisted
@@ -660,17 +660,9 @@ int dph_launch_lut(const float* xr, int64_t n, const float* pq, float* lut_canon
                    void* lutq, float2* qparams, cudaStream_t st, int group) {
     if (n == 0) return 0;
     static DphPerDeviceOnce lut_once;
-    constexpr int lut_smem = 4 * 32 * LUT_TILE_LD * 4;        // both shapes: 128 (query, sub-quantizer) rows
-    if (lut_once.first()) {
-        DPH_CUDA(cudaFuncSetAttribute(lut_kernel<4, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, lut_smem));
-        DPH_CUDA(cudaFuncSetAttribute(lut_kernel<8, 16>, cudaFuncAttributeMaxDynamicSharedMemorySize, lut_smem));
-    }
-    // knob 2 of dph_set_tuning: 2 selects <8, 16>.  Measured on one shard of C4 (1024 queries, tools/bench_variants.py shard,
-    // profiles/r2p_variants.txt): no faster than <4, 32> (rank step 4.499 vs 4.500 ms at nprobe 256, 1.500 vs 1.479 ms at nprobe 32) -- the
-    // kernel is bound by its per-CTA latency chain, not by the codebook stream -- so <4, 32> stays the default.
-    const int lv = g_dph_tune[2];
-    if (lv == 2) lut_kernel<8, 16><<<dim3((unsigned)((n + 7) / 8), 6), 256, lut_smem, st>>>(xr, pq, n, lut_canon, lutmax, lutmin, lutmaxv);
-    else lut_kernel<4, 32><<<dim3((unsigned)((n + 3) / 4), 3), 256, lut_smem, st>>>(xr, pq, n, lut_canon, lutmax, lutmin, lutmaxv);
+    constexpr int lut_smem = 4 * 32 * LUT_TILE_LD * 4;        // LQ x MS = 128 (query, sub-quantizer) rows
+    if (lut_once.first()) DPH_CUDA(cudaFuncSetAttribute(lut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, lut_smem));
+    lut_kernel<<<dim3((unsigned)((n + 3) / 4), 3), 256, lut_smem, st>>>(xr, pq, n, lut_canon, lutmax, lutmin, lutmaxv);
     DPH_CUDA(cudaGetLastError());
     if (lutq) {
         if (group == 4) lutq_kernel<unsigned char, DPH_QMAX8><<<dim3((unsigned)n, 3), 256, 0, st>>>(lut_canon, lutmin, lutmaxv, (unsigned char*)lutq, qparams);

@@ -645,9 +645,9 @@ __device__ __forceinline__ unsigned imad_add(unsigned x, unsigned one, unsigned 
     return d;
 }
 // Four gathers of one table (code bytes T0..T0+3 of a segment, addresses built by quad_word) into that table's sums.
-// IMADL: how many of the running-sum additions go to the FMA pipe: 0 = none (all IADD3), 1 = the raw sums, 2 = the raw sums and
-// half of the odd-byte sums, 3 = all of them.
-template <int T0, int TAB, int IMADL> __device__ __forceinline__ void quad_gather(const unsigned (&ad)[4], unsigned one, unsigned (&sr)[4], unsigned (&ab)[4]) {
+// The raw sums are added on the FMA pipe (imad_add), the odd-byte sums by IADD3.  Moving the odd-byte sums to the FMA pipe as well
+// (half or all of them) makes the issue slots the limit instead (DESIGN.md 4.1).
+template <int T0, int TAB> __device__ __forceinline__ void quad_gather(const unsigned (&ad)[4], unsigned one, unsigned (&sr)[4], unsigned (&ab)[4]) {
     constexpr int S = T0 >> 5;
     constexpr int TB = DPH_DYN_SMEM_BASE + (S < 2 ? TAB : 2) * 65536 + (S < 2 ? S : TAB) * 128;
     constexpr int A = (T0 >> 2) & 1;                  // two accumulator sets, alternating per code word
@@ -658,41 +658,31 @@ template <int T0, int TAB, int IMADL> __device__ __forceinline__ void quad_gathe
     // 8-bit entries: the odd bytes are widened per gather (a lane-wise add of two words could carry).  A 7-bit variant that widens
     // once per TWO gathers is faster but doubles eps, and then the exactness proof fails for ~10 % of the queries at C2 (measured
     // on B200); the exact fallback costs far more than it saves.
-    if (IMADL >= 1) {
-        sr[2 * A] = imad_add(w1, one, imad_add(w0, one, sr[2 * A]));
-        sr[2 * A + 1] = imad_add(w3, one, imad_add(w2, one, sr[2 * A + 1]));
-    } else {
-        sr[2 * A] += w0 + w1;
-        sr[2 * A + 1] += w2 + w3;
-    }
+    sr[2 * A] = imad_add(w1, one, imad_add(w0, one, sr[2 * A]));
+    sr[2 * A + 1] = imad_add(w3, one, imad_add(w2, one, sr[2 * A + 1]));
     const unsigned e0 = __byte_perm(w0, 0u, 0x4341), e1 = __byte_perm(w1, 0u, 0x4341);
     const unsigned e2 = __byte_perm(w2, 0u, 0x4341), e3 = __byte_perm(w3, 0u, 0x4341);
-    if (IMADL >= 3 || (IMADL == 2 && A == 1)) {
-        ab[2 * A] = imad_add(e1, one, imad_add(e0, one, ab[2 * A]));
-        ab[2 * A + 1] = imad_add(e3, one, imad_add(e2, one, ab[2 * A + 1]));
-    } else {
-        ab[2 * A] += e0 + e1;
-        ab[2 * A + 1] += e2 + e3;
-    }
+    ab[2 * A] += e0 + e1;
+    ab[2 * A + 1] += e2 + e3;
 }
 // Byte b of rot[r] = ((lane + 3r + b) & 31) * 4, the rotated word offset of step t = 3r + b of a segment; byte 3 is zero.
 // Selector of code byte i at step t: [rotated offset of t, code byte i, 0, 0].
 template <int T> struct RotSel { static constexpr int reg = (T & 31) / 3, sel = 0x7700 | (4 + (T & 31) % 3); };
-template <int T0, int NTAB, int IMADL> __device__ __forceinline__ void quad_word(unsigned wv, const unsigned (&rot)[11], unsigned one,
-                                                                                  unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
+template <int T0, int NTAB> __device__ __forceinline__ void quad_word(unsigned wv, const unsigned (&rot)[11], unsigned one,
+                                                                        unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
     const unsigned ad[4] = {__byte_perm(wv, rot[RotSel<T0>::reg], RotSel<T0>::sel | 0x00),
                             __byte_perm(wv, rot[RotSel<T0 + 1>::reg], RotSel<T0 + 1>::sel | 0x10),
                             __byte_perm(wv, rot[RotSel<T0 + 2>::reg], RotSel<T0 + 2>::sel | 0x20),
                             __byte_perm(wv, rot[RotSel<T0 + 3>::reg], RotSel<T0 + 3>::sel | 0x30)};
-    quad_gather<T0, 0, IMADL>(ad, one, sr[0], ab[0]);
-    if (NTAB == 2) quad_gather<T0, 1, IMADL>(ad, one, sr[1], ab[1]);
+    quad_gather<T0, 0>(ad, one, sr[0], ab[0]);
+    if (NTAB == 2) quad_gather<T0, 1>(ad, one, sr[1], ab[1]);
 }
-template <int C, int NTAB, int IMADL> __device__ __forceinline__ void quad_chunk(const uint4& v, const unsigned (&rot)[11], unsigned one,
-                                                                                   unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
-    quad_word<C * 16 + 0, NTAB, IMADL>(v.x, rot, one, sr, ab);
-    quad_word<C * 16 + 4, NTAB, IMADL>(v.y, rot, one, sr, ab);
-    quad_word<C * 16 + 8, NTAB, IMADL>(v.z, rot, one, sr, ab);
-    quad_word<C * 16 + 12, NTAB, IMADL>(v.w, rot, one, sr, ab);
+template <int C, int NTAB> __device__ __forceinline__ void quad_chunk(const uint4& v, const unsigned (&rot)[11], unsigned one,
+                                                                         unsigned (&sr)[2][4], unsigned (&ab)[2][4]) {
+    quad_word<C * 16 + 0, NTAB>(v.x, rot, one, sr, ab);
+    quad_word<C * 16 + 4, NTAB>(v.y, rot, one, sr, ab);
+    quad_word<C * 16 + 8, NTAB>(v.z, rot, one, sr, ab);
+    quad_word<C * 16 + 12, NTAB>(v.w, rot, one, sr, ab);
 }
 // append with an overflow latch: the round loop polls ONE flag instead of every buffer's counter
 __device__ __forceinline__ void warp_append_latch(bool pass, unsigned long long key, unsigned long long* cb, int* cnt, int* full, int lane) {
@@ -747,7 +737,7 @@ __device__ __forceinline__ void quad_prefetch_next(const GroupScanArgs& a, const
 // of blocks, then a barrier, the compaction of the buffers over keep and the refresh of the thresholds; until every warp is done.
 // The code stream is loaded with the evict_first policy `pol`: each block is read once per batch.
 // FILT: nmask is the mask word of the block in nxt (in and out), mrow[b] the mask word of the item's list's block b.
-template <int NTAB, int IMADL, bool FILT>
+template <int NTAB, bool FILT>
 __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadShared* sh, const DphUnit* dsc, const uint4* lbase, unsigned b,
                                                  unsigned bp, uint4 (&nxt)[6], const unsigned (&rot)[11], unsigned one, int total_units,
                                                  unsigned long long pol, unsigned long long* ph, unsigned long long& ph_t, unsigned& nmask,
@@ -781,12 +771,12 @@ __device__ __forceinline__ void quad_item_rounds(const GroupScanArgs& a, QuadSha
             }
             if (FILT && cmask == 0) continue;                      // warp-uniform: no row of the block is selected
             unsigned sr[2][4] = {}, ab[2][4] = {};
-            quad_chunk<0, NTAB, IMADL>(cur6[0], rot, one, sr, ab);
-            quad_chunk<1, NTAB, IMADL>(cur6[1], rot, one, sr, ab);
-            quad_chunk<2, NTAB, IMADL>(cur6[2], rot, one, sr, ab);
-            quad_chunk<3, NTAB, IMADL>(cur6[3], rot, one, sr, ab);
-            quad_chunk<4, NTAB, IMADL>(cur6[4], rot, one, sr, ab);
-            quad_chunk<5, NTAB, IMADL>(cur6[5], rot, one, sr, ab);
+            quad_chunk<0, NTAB>(cur6[0], rot, one, sr, ab);
+            quad_chunk<1, NTAB>(cur6[1], rot, one, sr, ab);
+            quad_chunk<2, NTAB>(cur6[2], rot, one, sr, ab);
+            quad_chunk<3, NTAB>(cur6[3], rot, one, sr, ab);
+            quad_chunk<4, NTAB>(cur6[4], rot, one, sr, ab);
+            quad_chunk<5, NTAB>(cur6[5], rot, one, sr, ab);
             const unsigned j = bcur * 32u + lane;
             const bool valid = (int)j < len && (!FILT || ((cmask >> lane) & 1u));
             // thresholds are compared in the float domain (one FSETP per query); the order-preserving integer key is built only for
@@ -864,7 +854,7 @@ __device__ __forceinline__ void quad_first_block(const GroupScanArgs& a, const D
 // out of blocks prefetches its first blocks of the next item into L2 (quad_prefetch_next), and every warp loads its first block of the
 // next item into registers before the candidates are published, so those are in flight during the publish and the next table build.
 // The table sources (a few MB per batch, re-read at every item) are loaded evict_last, the code stream evict_first.
-template <int IMADL, bool FILT>
+template <bool FILT>
 __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
     unsigned char* const smem = dph_smem;
     QuadShared* sh = reinterpret_cast<QuadShared*>(smem + SMEM_QUAD_TABLES);
@@ -967,8 +957,8 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
         }
         asm volatile("cp.async.commit_group;" ::: "memory");
         const unsigned* mrow = FILT ? a.mask + a.mask_off[dsc->list] : nullptr;
-        if (ntab == 2) quad_item_rounds<2, IMADL, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
-        else quad_item_rounds<1, IMADL, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
+        if (ntab == 2) quad_item_rounds<2, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
+        else quad_item_rounds<1, FILT>(a, sh, dsc, lbase, b, bp, nxt, rot, one, total_units, pol_stream, ph, ph_t, nmask, mrow);
         // every warp waited for its copies before the rounds' last barrier: the next record is visible
         any_unit = nu < total_units;
         if (any_unit) quad_first_block<FILT>(a, &sh->desc[cur ^ 1], nxt, pol_stream, nmask);
@@ -1006,10 +996,6 @@ __global__ void __launch_bounds__(QNT, 1) scan_quad_kernel(GroupScanArgs a) {
 #undef QPH_MARK
 
 __global__ void smem_base_probe_kernel(unsigned* out) { *out = (unsigned)__cvta_generic_to_shared(dph_smem); }
-// scan_quad_kernel by filter (unfiltered, filtered) and IMAD level, knob 0 of dph_set_tuning (out of range: the default, 1)
-static void (*const quad_kernels[2][4])(GroupScanArgs) = {
-    {scan_quad_kernel<0, false>, scan_quad_kernel<1, false>, scan_quad_kernel<2, false>, scan_quad_kernel<3, false>},
-    {scan_quad_kernel<0, true>, scan_quad_kernel<1, true>, scan_quad_kernel<2, true>, scan_quad_kernel<3, true>}};
 
 static int dph_scan_setup_attrs() {
     static DphPerDeviceOnce once;
@@ -1029,8 +1015,8 @@ static int dph_scan_setup_attrs() {
         DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_EXACT + (int)sizeof(ScanShared)));
     for (auto f : {scan_pair_kernel<false>, scan_pair_kernel<true>})
         DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LUT_FAST + (int)sizeof(PairShared)));
-    for (auto& row : quad_kernels)
-        for (auto f : row) DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
+    for (auto f : {scan_quad_kernel<false>, scan_quad_kernel<true>})
+        DPH_CUDA(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_QUAD_TABLES + (int)sizeof(QuadShared)));
     return 0;
 }
 
@@ -1062,8 +1048,7 @@ int dph_launch_scan(dph_index* ix, const DphSearchPlan& p, const DphCodeSrc& src
         a.list_lo = src.lo; a.list_hi = src.hi; a.nprobe = ix->nprobe; a.keep = keep;
         a.udesc = ix->grp_udesc.as<DphUnit>(); a.one = 1u;
         a.mask = src.mask; a.mask_off = (const long long*)ix->blk_off;
-        const int lv = g_dph_tune[0] >= 0 && g_dph_tune[0] <= 3 ? g_dph_tune[0] : 1;
-        if (group == 4) quad_kernels[filt][lv]<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
+        if (group == 4) (filt ? scan_quad_kernel<true> : scan_quad_kernel<false>)<<<grid, QNT, SMEM_QUAD_TABLES + sizeof(QuadShared), st>>>(a);
         else (filt ? scan_pair_kernel<true> : scan_pair_kernel<false>)<<<grid, NT, SMEM_LUT_FAST + sizeof(PairShared), st>>>(a);
     }
     DPH_CUDA(cudaGetLastError());

@@ -1,4 +1,4 @@
-// wgmma.cuh -- thin PTX wrappers for the sm_90a tensor-core path (mbarrier, TMA tensor loads, cluster helpers, wgmma.mma_async
+// wgmma.cuh -- thin PTX wrappers for the sm_90a tensor-core path (mbarrier, TMA tensor loads, wgmma.mma_async
 // with shared-memory matrix descriptors) shared by gemm_tf32.cu, gemm_bf16x3.cu and attention_tc.cu, plus the host-side
 // tensor-map encoder.
 #pragma once
@@ -19,26 +19,10 @@ __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity) {
         "bra WAIT_LOOP;\n\t"
         "DONE:\n\t}" ::"r"(bar), "r"(parity) : "memory");
 }
-// arrive on the barrier at this CTA-relative offset in CTA `cta` of the cluster (the own CTA included)
-__device__ __forceinline__ void mbar_arrive_cluster(unsigned bar, unsigned cta) {
-    asm volatile(
-        "{\n\t.reg .b32 ra;\n\t"
-        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar), "r"(cta) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(unsigned bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
 __device__ __forceinline__ void tma_load_2d(unsigned dst, const CUtensorMap* map, int c0, int c1, unsigned bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                  ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
-}
-// multicast variant: the box lands at the same CTA-relative offset (and signals the same barrier offset) in every CTA of cta_mask
-__device__ __forceinline__ void tma_load_2d_mc(unsigned dst, const CUtensorMap* map, int c0, int c1, unsigned bar, unsigned short cta_mask) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%2, %3}], [%4], %5;"
-                 ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ unsigned cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 // generic-proxy shared-memory stores -> visible to the tensor core's async-proxy reads
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }

@@ -379,15 +379,6 @@ int dph_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m, int64
 int dph_gemm_tf32_nt(const float* A, const float* W, const float* bias, const float* residual, float* out, int64_t M, int64_t N,
                      int64_t K, int act, int precise /* 0: 1xTF32, 1: 3xTF32 split (fp32-accurate), 2: bf16x3 split (N % 256 == 0) */,
                      void* cuda_stream);
-/* Scheduling of the 1xTF32 GEMMs (process-wide; every mode issues the same MMAs in the same order -> bit-identical results):
- * 0: one 128x128 tile per CTA;  1: the same as 2-CTA thread-block clusters sharing the A tile through TMA multicast (N/128 even);
- * 2 (default): one persistent CTA per SM walking 128x256 tiles (N % 256 == 0, else mode 0). */
-int dph_gemm_tf32_set_mode(int mode);
-/* Measurement hook (process-wide): choose between kernel variants that compute bit-identical results, for A/B timing on hardware
- * (tools/bench_variants.py).  knob 0: additions of the quad scan issued on the FMA pipe (0 none .. 3 all; default 1);
- * knob 1: tile shape of the sequential-k SGEMM (0 auto, 1: 128x128, 2: 64x64, 3: 32x64, 4: 16x64);
- * knob 2: shape of the PQ-table kernel (default: 4 queries x 32 sub-quantizers per CTA; 2: 8 x 16). */
-int dph_set_tuning(int knob, int value);
 
 #ifdef __cplusplus
 }

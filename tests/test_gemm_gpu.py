@@ -7,7 +7,6 @@ import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
-DEFAULT_MODE = 2      # the library default of dph_gemm_tf32_set_mode
 
 
 def run_gemm(A, W, bias, resid, act, precise=0):
@@ -63,27 +62,22 @@ def test_gemm_tf32_matches_torch_fp32(M, N, K, variant):
     assert (out2.double() - ref2).abs().max() < 1e-3 * max(1.0, ref2.abs().max().item() * 1e-3)
 
 
-@pytest.mark.parametrize("mode", [1, 2])
-@pytest.mark.parametrize("M,N,K", [(4096, 768, 768), (333, 2304, 768), (64, 3072, 768), (1000, 256, 3072), (20000, 768, 96)])
-def test_gemm_schedules_are_bit_identical(M, N, K, mode):
-    """mode 1 (2-CTA clusters sharing the A tile by TMA multicast) and mode 2 (persistent 128x256 tiles, one CTA per SM)
-    issue the same MMAs per output element in the same order as mode 0 (one 128x128 tile per CTA)."""
+@pytest.mark.parametrize("M,N,K", [(4096, 768, 768), (333, 2304, 768), (64, 3072, 768), (1000, 256, 3072), (20000, 768, 96), (1, 256, 32),
+                                   (127, 512, 64), (129, 768, 3072), (4096, 2304, 768), (4097, 3072, 768)])
+def test_gemm_schedules_are_bit_identical(M, N, K):
+    """N % 256 == 0 runs persistent 128x256 tiles, one CTA per SM; the same problem with W, bias and residual padded by 128 output
+    columns (N % 256 != 0) runs one 128x128 tile per CTA.  Both issue the same MMAs per output element in the same order."""
     import torch
-    from densephrases_b200 import _lib as L
+    assert N % 256 == 0
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     A = torch.randn((M, K), generator=g, device="cuda")
-    W = torch.randn((N, K), generator=g, device="cuda") * 0.05
-    bias = torch.randn((N,), generator=g, device="cuda")
-    resid = torch.randn((M, N), generator=g, device="cuda")
-    try:
-        L.check(L.lib().dph_gemm_tf32_set_mode(0))
-        base = run_gemm(A, W, bias, resid, 1)
-        L.check(L.lib().dph_gemm_tf32_set_mode(mode))
-        other = run_gemm(A, W, bias, resid, 1)
-    finally:
-        L.check(L.lib().dph_gemm_tf32_set_mode(DEFAULT_MODE))
-    assert torch.isfinite(other).all()
-    assert torch.equal(base, other), f"max|diff| {(base - other).abs().max().item():.3e}"
+    W = torch.randn((N + 128, K), generator=g, device="cuda") * 0.05
+    bias = torch.randn((N + 128,), generator=g, device="cuda")
+    resid = torch.randn((M, N + 128), generator=g, device="cuda")
+    persistent = run_gemm(A, W[:N], bias[:N], resid[:, :N].contiguous(), 1)
+    per_tile = run_gemm(A, W, bias, resid, 1)[:, :N]
+    assert torch.isfinite(persistent).all()
+    assert torch.equal(persistent, per_tile), f"max|diff| {(persistent - per_tile).abs().max().item():.3e}"
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 256, 32), (4096, 768, 768), (4096, 2304, 768), (4096, 3072, 768), (4096, 768, 3072), (100, 256, 64), (1, 256, 96),

@@ -1,6 +1,6 @@
 """The search at its arithmetic limits, against the C oracle: saturated packed sums, worst-case LUT rounding, extreme query scales,
-batches over several chunks, batch invariance at C2's list length, the k edges of the scan modes, and every bit-identical kernel
-variant of dph_set_tuning.  Scores are compared bit for bit, labels up to exact-tie groups (tests/helpers.py)."""
+batches over several chunks, batch invariance at C2's list length and the k edges of the scan modes.  Scores are compared bit for
+bit, labels up to exact-tie groups (tests/helpers.py)."""
 import numpy as np
 import pytest
 
@@ -8,7 +8,6 @@ from tests.helpers import assert_topk_equal, near_queries, uniform_lens
 from tests.test_search_gpu import make_pair
 from tests.test_search_limits_cpu import (QMAX, keep_pair, keep_quad, rounding_case, saturated_codes, saturating_codebooks,
                                           limit_query)
-from tests.test_sgemm_seq_gpu import tuning
 
 pytestmark = pytest.mark.gpu
 EYE = np.eye(768, dtype=np.float32)
@@ -59,13 +58,11 @@ def test_saturated_codes_every_lane(oracle, codebooks):
         q = np.repeat(x[None], copies, axis=0)
         Dr, Ir = ref.search(q, k, 2)
         assert set(Ir[:, 0].tolist()) <= sat_labels
-        runs = [(2, 0, 0), (4, 0, 0), (4, 1, 0), (4, 2, 0), (4, 3, 0), (4, 1, 2), (0, 0, 0), (0, 3, 0)]   # (mode, IMAD level, table kernel)
-        for mode, lvl, lut in runs:
-            with tuning(0, lvl), tuning(2, lut):
-                gpu.set_scan_mode(mode)
-                D, I = gpu.search(q, k)
-                assert gpu.last_group_size() == (2 if mode == 2 else 4)
-                assert_topk_equal(D, I, Dr, Ir, f"{codebooks} copies={copies} mode={mode} imad={lvl} lut={lut}")
+        for mode in (2, 4, 0):
+            gpu.set_scan_mode(mode)
+            D, I = gpu.search(q, k)
+            assert gpu.last_group_size() == (2 if mode == 2 else 4)
+            assert_topk_equal(D, I, Dr, Ir, f"{codebooks} copies={copies} mode={mode}")
 
 
 # ---- 2. worst-case LUT rounding -----------------------------------------------------------------------------------------
@@ -173,28 +170,26 @@ def test_batch_over_three_chunks(oracle, mode):
 
 
 def test_k_edges_in_every_mode(oracle):
-    """k on both sides of the quad (85 / 86) and pair (683 / 684) limits and at the maximum, in every forced mode and with the
-    eight-query PQ-table kernel."""
+    """k on both sides of the quad (85 / 86) and pair (683 / 684) limits and at the maximum, in every forced mode."""
     nlist, nprobe = 16, 4
     ref, gpu = make_pair(oracle, nlist, uniform_lens(nlist * 4500, nlist))
     gpu.nprobe = nprobe
     x = near_queries(ref, 12, 17)
     for k in (1, 85, 86, 683, 684, 1024):
         Dr, Ir = ref.search(x, k, nprobe)
-        for mode, lut in ((1, 0), (3, 0), (2, 0), (4, 0), (2, 2), (4, 2)):
-            with tuning(2, lut):
-                gpu.set_scan_mode(mode)
-                D, I = gpu.search(x, k)
+        for mode in (1, 3, 2, 4):
+            gpu.set_scan_mode(mode)
+            D, I = gpu.search(x, k)
             if mode != 1:
                 want = {3: 1, 2: 2 if k <= 683 else 1, 4: 4 if k <= 85 else (2 if k <= 683 else 1)}[mode]
                 assert gpu.last_group_size() == want, f"k={k} mode={mode}"
-            assert_topk_equal(D, I, Dr, Ir, f"k={k} mode={mode} lut={lut}")
+            assert_topk_equal(D, I, Dr, Ir, f"k={k} mode={mode}")
 
 
 def test_batch_invariance_at_c2_list_length(oracle):
     """IVF4096 over 20 M synthetic rows (C2's list length), nprobe 256: a batch of 1024 queries runs the quad scan, each of 32 of
     them searched alone runs the one-query scan; both orders are canonical, so scores and labels are byte-identical, tie order
-    included.  Every quad IMAD level and the eight-query PQ-table kernel give the same bytes; 16 rows are checked against the oracle."""
+    included; 16 rows are checked against the oracle."""
     import torch
     nlist, nprobe, k = 4096, 256, 10
     ref, gpu = make_pair(oracle, nlist, uniform_lens(20_000_000, nlist))
@@ -209,10 +204,6 @@ def test_batch_invariance_at_c2_list_length(oracle):
         D1, I1 = gpu.search(xt[r:r + 1].contiguous(), k)
         assert gpu.last_group_size() == 1
         assert np.array_equal(D1.cpu().numpy()[0].view(np.int32), D[r].view(np.int32)) and np.array_equal(I1.cpu().numpy()[0], I[r]), f"row {r}"
-    for knob, v in ((0, 0), (0, 2), (0, 3), (2, 2)):
-        with tuning(knob, v):
-            Dv, Iv = gpu.search(xt, k)
-        assert np.array_equal(Dv.cpu().numpy().view(np.int32), D.view(np.int32)) and np.array_equal(Iv.cpu().numpy(), I), f"knob {knob} = {v}"
     rows = np.sort(rng.choice(1024, 16, replace=False))
     Dr, Ir = ref.search(x[rows], k, nprobe)
     assert_topk_equal(D[rows], I[rows], Dr, Ir, "C2 lists")

@@ -1,17 +1,19 @@
-"""dph_sgemm_nt_seq (prep.cu) against the sequential-k FMA definition, for every tile kernel (knob 1 of dph_set_tuning: 0 = the
-shape rule, 1 = 128x128, 2 = 64x64 with 32-deep k tiles, 3 = 32-row tiles, 4 = 16-row tiles).  The SGEMM carries the OPQ rotation,
-the coarse scores, encode and training; every output must be the one fp32 FMA chain over k ascending from +0, bit for bit, at row
-and column counts on both sides of every tile edge, widths that are not a multiple of 4 (the scalar store tail) and depths that
-are not a multiple of 64 (the row-tiled kernels step k by 64; those depths take the 64x64 kernel)."""
+"""dph_sgemm_nt_seq (prep.cu) against the sequential-k FMA definition, through every tile kernel its shape rule picks (128x128,
+64x64 with 32-deep k tiles, 32-row tiles, 16-row tiles).  The SGEMM carries the OPQ rotation, the coarse scores, encode and
+training; every output must be the one fp32 FMA chain over k ascending from +0, bit for bit, at row and column counts on both sides
+of every kernel's tile edges, widths that are not a multiple of 4 (the scalar store tail) and depths that are not a multiple of 64
+(the row-tiled kernels step k by 64; those depths take the 64x64 kernel unless the 128x128 kernel is picked)."""
 import ctypes as C
+import itertools
 
 import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
 
-NS = (1, 15, 16, 17, 63, 64, 65, 1000, 1024, 2049)
-MS = (1, 5, 768, 1000, 1001, 4096, 20000, 65536)
+NS = (1, 15, 16, 17, 63, 64, 65, 1000, 1024, 2047, 2048, 2049)
+MS = (1, 5, 768, 1000, 1001, 1025, 3969, 4095, 4096, 20000, 65536)
+TILES = {"128x128": (128, 128), "64x64": (64, 64), "32x64": (32, 64), "16x64": (16, 64)}     # rows x columns per CTA
 
 
 def seq_matmul_ref(X, W):
@@ -31,21 +33,27 @@ def seq_matmul_ref(X, W):
     return out
 
 
-class tuning:
-    """Set one dph_set_tuning knob for a block; every knob goes back to its default afterwards (knob 0 to 1, the others to 0)."""
+def tile_kernel(n, m, K):
+    """The tile kernel dph_launch_sgemm_nt_seq (prep.cu) picks for out [n, m] at depth K."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    cdiv = lambda a, b: -(-a // b)
+    if cdiv(m, 128) * cdiv(n, 128) >= 2 * sms:
+        return "128x128"
+    ct = cdiv(m, 64)
+    if K % 64 or ct * cdiv(n, 64) >= 128:
+        return "64x64"
+    return "32x64" if ct * cdiv(n, 32) >= 128 else "16x64"
 
-    def __init__(self, knob, value):
-        self.knob, self.value = knob, value
 
-    def __enter__(self):
-        from densephrases_b200 import _lib as L
-        L.check(L.lib().dph_set_tuning(self.knob, self.value))
-
-    def __exit__(self, *exc):
-        from densephrases_b200 import _lib as L
-        for knob, v in ((0, 1), (1, 0), (2, 0)):
-            L.check(L.lib().dph_set_tuning(knob, v))
-        return False
+def assert_every_tile_edge(shapes, K):
+    """Each kernel the rule can pick at depth K gets row and column counts one below, at and one above a multiple of its tile."""
+    for kern in (TILES if K % 64 == 0 else ("128x128", "64x64")):
+        tm, tn = TILES[kern]
+        got = [(n, m) for n, m in shapes if tile_kernel(n, m, K) == kern]
+        for side, tile, vals in (("rows", tm, [n for n, _ in got]), ("columns", tn, [m for _, m in got])):
+            missing = {tile - 1, 0, 1} - {v % tile for v in vals}
+            assert not missing, f"K={K}: no shape sends {side} = {sorted(missing)} mod {tile} to the {kern} kernel"
 
 
 def shapes():
@@ -84,28 +92,29 @@ def test_sgemm_tiles_k768_all_shapes(oracle):
     ref_tall = seq_matmul_ref(X, W[:4096])
     Xd, Wd = torch.from_numpy(X).cuda(), torch.from_numpy(W).cuda()
     assert len(shapes()) >= 60
+    assert_every_tile_edge(shapes(), K)
     for n, m in shapes():
         ref = ref_wide[:n, :m] if n <= 65 else ref_tall[:n, :m]
         refd = torch.from_numpy(np.ascontiguousarray(ref)).cuda()
-        for v in (0, 1, 2, 3, 4):
-            with tuning(1, v):
-                out = run_gpu(Xd[:n].contiguous(), Wd[:m].contiguous(), K)
-            bad = (out.view(torch.int32) != refd.view(torch.int32))
-            assert not bool(bad.any()), f"n={n} m={m} variant {v}: {int(bad.sum())} outputs differ, first at {bad.nonzero()[0].tolist()}"
+        out = run_gpu(Xd[:n].contiguous(), Wd[:m].contiguous(), K)
+        bad = (out.view(torch.int32) != refd.view(torch.int32))
+        assert not bool(bad.any()), f"n={n} m={m} ({tile_kernel(n, m, K)}): {int(bad.sum())} outputs differ, first at {bad.nonzero()[0].tolist()}"
 
 
 @pytest.mark.parametrize("K", [32, 64, 96, 128])
 def test_sgemm_tiles_short_k(oracle, K):
-    """K = 32 and 96 are not multiples of the row-tiled kernels' 64-deep k tile: every variant but 1 then runs the 64x64 kernel."""
+    """K = 32 and 96 are not multiples of the row-tiled kernels' 64-deep k tile: every shape the 128x128 kernel does not take then
+    runs the 64x64 kernel."""
     import torch
+    shapes = sorted({(1, 1), (17, 5), (64, 1000), (65, 1001), (130, 768), (3, 129)} |
+                    set(itertools.product((257, 2047, 2048, 2049), (63, 65, 1023, 1024, 2175, 2176, 2177))))
+    assert_every_tile_edge(shapes, K)
     rng = np.random.default_rng(K)
-    X = rng.standard_normal((130, K)).astype(np.float32)
-    W = rng.standard_normal((1001, K)).astype(np.float32)
+    X = rng.standard_normal((2049, K)).astype(np.float32)
+    W = rng.standard_normal((2177, K)).astype(np.float32)
     Xd, Wd = torch.from_numpy(X).cuda(), torch.from_numpy(W).cuda()
     ref = seq_matmul_ref(X, W)
-    for n, m in ((1, 1), (17, 5), (64, 1000), (65, 1001), (130, 768), (3, 129)):
+    for n, m in shapes:
         refd = torch.from_numpy(np.ascontiguousarray(ref[:n, :m])).cuda()
-        for v in (0, 1, 2, 3, 4):
-            with tuning(1, v):
-                out = run_gpu(Xd[:n].contiguous(), Wd[:m].contiguous(), K)
-            assert torch.equal(out.view(torch.int32), refd.view(torch.int32)), f"K={K} n={n} m={m} variant {v}"
+        out = run_gpu(Xd[:n].contiguous(), Wd[:m].contiguous(), K)
+        assert torch.equal(out.view(torch.int32), refd.view(torch.int32)), f"K={K} n={n} m={m} ({tile_kernel(n, m, K)})"

@@ -156,7 +156,10 @@ def test_train_add_search_and_faiss_file_round_trip(trained, tmp_path):
 
 def test_trained_recall_meets_torch_trainer(trained):
     """The clustered data of test_build_index: the GPU trainer meets that test's thresholds and is within 0.02 of the torch trainer's
-    quality and recall on the same sample with the same iteration counts."""
+    quality and recall on the same sample with the same iteration counts.  The torch trainer runs on one CPU thread: its QR and
+    reductions round differently when split over threads, and on this sample that alone moves its recall by more than 0.01 (0.8275 on
+    one thread, 0.84 on eight), so with the default thread count the reference would depend on the machine's core count."""
+    import torch
     from densephrases_b200 import IvfPqIndex
     from densephrases_b200.build_index import build_index
     x, _, _ = trained
@@ -176,7 +179,12 @@ def test_trained_recall_meets_torch_trainer(trained):
     g.add_with_ids(x, None)
     g.nprobe = 8
     gpu = scores(g.search(q, 50)[1])
-    t = build_index(x[:3000], x, nlist=16, seed=5, niter_opq=2, niter_km=6, niter_pq=4)
+    threads = torch.get_num_threads()
+    torch.set_num_threads(1)
+    try:
+        t = build_index(x[:3000], x, nlist=16, seed=5, niter_opq=2, niter_km=6, niter_pq=4)
+    finally:
+        torch.set_num_threads(threads)
     ti = IvfPqIndex.from_arrays(t["A"], t["centroids"], t["pq"], t["list_len"], t["codes"], t["ids"])
     ti.nprobe = 8
     ref = scores(ti.search(q, 50)[1])

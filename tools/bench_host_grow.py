@@ -3,9 +3,8 @@
   python tools/bench_host_grow.py [--legs c2,build,reserve] [--build-max-rows N] [--out DIR]
 
 c2:      a C2-shaped host index (100 M rows, IVF4096, 9.6 GB of codes, synthetic) with a reserved capacity: add 1 M rows, remove a
-         1 M-label range, merge a 10 M-row device-resident source.  Each call runs twice, with the mover's gathers and write-backs
-         overlapped (two streams) and serialised (one stream, dph_set_tuning knob 3): time, blocks the mover read and wrote, its rate,
-         and the device-resident twin's time for the same call.  Reference rates: cudaMemcpyAsync host-to-device and device-to-host
+         1 M-label range, merge a 10 M-row device-resident source.  Each call: time, blocks the mover read and wrote, its rate, and
+         the device-resident twin's time for the same call.  Reference rates: cudaMemcpyAsync host-to-device and device-to-host
          of 1 GiB from page-locked memory, alone and both directions at once.
 build:   an empty host index grown by adds of 10 M rows (one device batch, reused) up to the largest multiple of 10 M rows whose codes
          fit 60 % of MemAvailable (capped by --build-max-rows): time per add against rows held.
@@ -24,7 +23,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import bench  # noqa: E402  (seeds and workloads shared with the benchmark)
-from densephrases_b200 import IvfPqIndex, _lib  # noqa: E402
+from densephrases_b200 import IvfPqIndex  # noqa: E402
 from tools.bench_host_codes import card, mem_available  # noqa: E402
 
 GiB = 1 << 30
@@ -111,28 +110,24 @@ def c2_leg():
     out["bits_equal_before"] = same_bits(ix, twin, q)
     src_lens = np.random.default_rng(3).multinomial(10_000_000, np.full(nlist, 1 / nlist)).astype(np.int64)
     src = make(src_lens, nlist, False, seed=SEED + 1)
-    xs = [batch(ix, 1_000_000, 100 + i) for i in range(2)]
+    x = batch(ix, 1_000_000, 100)
     calls = {
-        "add_1M": lambda g, i: g.add(xs[i]),
-        "remove_1M_range": lambda g, i: g.remove_ids(range(40_000_000 + i * 1_000_000, 41_000_000 + i * 1_000_000)),
-        "merge_10M_source": lambda g, i: g.merge_from(src, add_id=(i + 1) * 10**9),
+        "add_1M": lambda g: g.add(x),
+        "remove_1M_range": lambda g: g.remove_ids(range(40_000_000, 41_000_000)),
+        "merge_10M_source": lambda g: g.merge_from(src, add_id=10**9),
     }
     for name, call in calls.items():
-        r = {}
-        for i, mode in enumerate(("overlapped", "serialised")):
-            _lib.lib().dph_set_tuning(3, int(mode == "serialised"))
-            ms, _ = timed(lambda: call(ix, i))
-            mv = ix.last_host_move()
-            _lib.lib().dph_set_tuning(3, 0)
-            tms, _ = timed(lambda: call(twin, i))
-            rd, wr = mv["blocks_read"] * 3072, mv["blocks_written"] * 3072
-            r[mode] = {"ms": round(ms, 1), "mover_ms": round(mv["ms"], 1), "GB_read": round(rd / 1e9, 2), "GB_written": round(wr / 1e9, 2),
-                       "chunks": mv["chunks"], "mover_GBps_each_way": round(max(rd, wr) / max(mv["ms"], 1e-3) / 1e6, 1),
-                       "device_twin_ms": round(tms, 1), "bits_equal": same_bits(ix, twin, q)}
+        ms, _ = timed(lambda: call(ix))
+        mv = ix.last_host_move()
+        tms, _ = timed(lambda: call(twin))
+        rd, wr = mv["blocks_read"] * 3072, mv["blocks_written"] * 3072
+        r = {"ms": round(ms, 1), "mover_ms": round(mv["ms"], 1), "GB_read": round(rd / 1e9, 2), "GB_written": round(wr / 1e9, 2),
+             "chunks": mv["chunks"], "mover_GBps_each_way": round(max(rd, wr) / max(mv["ms"], 1e-3) / 1e6, 1),
+             "device_twin_ms": round(tms, 1), "bits_equal": same_bits(ix, twin, q)}
         out[name] = r
         print("c2", name, r, flush=True)
     out["host_bytes_after"] = ix.host_bytes
-    del ix, twin, src, xs
+    del ix, twin, src, x
     torch.cuda.empty_cache()
     return out
 

@@ -1,16 +1,12 @@
-"""A/B timing of bit-identical kernel variants on hardware (dph_set_tuning):  python tools/bench_variants.py [sgemm] [c2] [shard]
-  sgemm : tile shapes of the sequential-k SGEMM at the OPQ-rotation / coarse shapes
-  c2    : BASELINE.json configs[1] (100 M phrases, IVF4096, batch 64, nprobe 256) -- quad-scan IMAD levels; results must not change
-  shard : one rank of C4 (shard 0 of 8; batch 1024) at nprobe 256 and 32 -- list-split vs query-split coarse quantizer"""
-import ctypes as C, os, sys
+"""One rank of C4 (shard 0 of 8; batch 1024) at nprobe 256 and 32: the list-split against the query-split coarse quantizer, with the
+time before the exchange and the scan time, and whether both give the same results:  python tools/bench_variants.py shard"""
+import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 import bench
-from densephrases_b200 import _lib as L, IvfPqIndex
+from densephrases_b200 import IvfPqIndex
 from densephrases_b200.sharded import shard_ranges
 
-what = set(sys.argv[1:]) or {"sgemm", "c2", "shard"}
-tune = lambda knob, v: L.check(L.lib().dph_set_tuning(knob, v))
 ev = lambda: torch.cuda.Event(enable_timing=True)
 
 
@@ -22,86 +18,41 @@ def timeit(fn, reps, warm=3):
     return e0.elapsed_time(e1) / reps
 
 
-if "sgemm" in what:
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    for n, m in [(1024, 768), (1024, 8192), (64, 768), (64, 4096), (128, 768)]:
-        X = torch.randn(n, 768, device="cuda"); W = torch.randn(m, 768, device="cuda")
-        outs = []
-        for v in (0, 1, 2, 3, 4):
-            tune(1, v)
-            out = torch.empty(n, m, device="cuda")
-            ms = timeit(lambda i: L.lib().dph_sgemm_nt_seq(X.data_ptr(), n, W.data_ptr(), m, 768, out.data_ptr(), st), 20)
-            outs.append(out)
-            print(f"sgemm n={n:5d} m={m:6d} variant {v}: {ms * 1000:8.1f} us  {2 * n * m * 768 / ms / 1e9:6.1f} TFLOP/s  same bits {bool((out == outs[0]).all())}", flush=True)
-        tune(1, 0)
-
-
-def near_queries(ix, N, nb, B):
-    g = torch.Generator().manual_seed(4321)
-    ids = torch.randint(0, N, (nb * B,), generator=g, dtype=torch.int64)
-    noise = torch.randn((nb * B, 768), generator=g, dtype=torch.float32) * 0.3
-    v, found = ix.reconstruct_batch(ids.cuda())
-    q = bench.finish_queries(v.cpu(), noise, ix.opq_matrix())
-    return q.reshape(nb, B, 768).cuda(), found
-
-
-if "c2" in what:
-    wl = bench.workload("C2")
-    ix = IvfPqIndex(wl["nlist"])
-    ix.set_opq(bench.opq_matrix(1234)); ix.gen_centroids(1234); ix.gen_pq(1234); ix.set_lists_synthetic(wl["lens"], 1234)
-    ix.nprobe = 256; ix.set_profile(True)
-    Q, _ = near_queries(ix, wl["N"], 12, 64)
+N, NLIST, WORLD, B, K = 1_000_000_000, 65536, 8, 1024, 10
+lens = bench.uniform_lens(N, NLIST)
+lo, hi = shard_ranges(lens, WORLD)[0]
+ix = IvfPqIndex(NLIST)
+ix.set_opq(bench.opq_matrix(1234)); ix.gen_centroids(1234); ix.gen_pq(1234); ix.set_shard(lo, hi); ix.set_lists_synthetic(lens, 1234)
+ix.set_profile(True)
+g = torch.Generator(device="cuda").manual_seed(4321)
+X = [0.5 * torch.randn((B, 768), generator=g, device="cuda") for _ in range(6)]
+for nprobe in (256, 32):
+    ix.nprobe = nprobe
+    keys_all = []
+    for x in X:
+        ix.search_partial(x, K)
+        pr = torch.from_numpy(ix.last_probes(B).astype(np.int64)).cuda()
+        cd = torch.from_numpy(ix.last_coarse(B)).cuda()
+        bits = cd.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
+        fkey = torch.where(bits >= 0x80000000, (~bits) & 0xFFFFFFFF, bits | 0x80000000)
+        kg = torch.zeros((WORLD, B, nprobe), dtype=torch.int64, device="cuda"); kg[0] = (fkey << 32) | (0xFFFFFFFF - pr)
+        keys_all.append(kg)
+    # records of the query-split protocol: every "rank" assigns its slice of 128 queries over all lists (here: this GPU, 8 times)
+    per = B // WORLD
+    recs = [torch.cat([ix.coarse_split(x[r * per:(r + 1) * per].contiguous()) for r in range(WORLD)]).contiguous() for x in X]
     base = None
-    for lvl in (0, 1, 2, 3, 1):
-        tune(0, lvl)
-        ms = timeit(lambda i: ix.search(Q[i % 12], 10), 40, warm=4)
-        scan = np.mean(ix.profile_scan_ms()[-40:])
-        D, I = ix.search(Q[0], 10)
+    for proto in ("list-split", "query-split"):
+        if proto == "list-split":
+            fn = lambda i: (ix.coarse_local(X[i % 6]), ix.search_preassigned(keys_all[i % 6], K))
+            pre = lambda i: ix.coarse_local(X[i % 6])
+        else:
+            fn = lambda i: (ix.coarse_split(X[i % 6][:per]), ix.search_assigned(recs[i % 6], K))
+            pre = lambda i: ix.coarse_split(X[i % 6][:per])
+        ms_pre = timeit(pre, 12, warm=3)
+        ms = timeit(fn, 12, warm=3)
+        scan = np.mean(ix.profile_scan_ms()[-12:])
+        _, (D, I, G) = fn(0)
         if base is None: base = (D.clone(), I.clone())
         same = bool((D == base[0]).all() and (I == base[1]).all())
-        print(f"C2 quad imad level {lvl}: step {ms:.3f} ms = {64 / ms * 1000:.0f} QPS, scan {scan:.3f} ms, flags {int(ix.last_flags(64).sum())}, same results {same}", flush=True)
-    tune(0, 1)
-    del ix, Q
-    torch.cuda.empty_cache()
-
-if "shard" in what:
-    N, NLIST, WORLD, B, K = 1_000_000_000, 65536, 8, 1024, 10
-    lens = bench.uniform_lens(N, NLIST)
-    lo, hi = shard_ranges(lens, WORLD)[0]
-    ix = IvfPqIndex(NLIST)
-    ix.set_opq(bench.opq_matrix(1234)); ix.gen_centroids(1234); ix.gen_pq(1234); ix.set_shard(lo, hi); ix.set_lists_synthetic(lens, 1234)
-    ix.set_profile(True)
-    g = torch.Generator(device="cuda").manual_seed(4321)
-    X = [0.5 * torch.randn((B, 768), generator=g, device="cuda") for _ in range(6)]
-    for nprobe in (256, 32):
-        ix.nprobe = nprobe
-        keys_all = []
-        for x in X:
-            ix.search_partial(x, K)
-            pr = torch.from_numpy(ix.last_probes(B).astype(np.int64)).cuda()
-            cd = torch.from_numpy(ix.last_coarse(B)).cuda()
-            bits = cd.view(torch.int32).to(torch.int64) & 0xFFFFFFFF
-            fkey = torch.where(bits >= 0x80000000, (~bits) & 0xFFFFFFFF, bits | 0x80000000)
-            kg = torch.zeros((WORLD, B, nprobe), dtype=torch.int64, device="cuda"); kg[0] = (fkey << 32) | (0xFFFFFFFF - pr)
-            keys_all.append(kg)
-        # records of the query-split protocol: every "rank" assigns its slice of 128 queries over all lists (here: this GPU, 8 times)
-        per = B // WORLD
-        recs = [torch.cat([ix.coarse_split(x[r * per:(r + 1) * per].contiguous()) for r in range(WORLD)]).contiguous() for x in X]
-        base = None
-        for proto in ("list-split", "query-split", "query-split lut<8,16>"):
-            tune(2, 2 if proto.endswith("16>") else 1)
-            if proto == "list-split":
-                fn = lambda i: (ix.coarse_local(X[i % 6]), ix.search_preassigned(keys_all[i % 6], K))
-                pre = lambda i: ix.coarse_local(X[i % 6])
-            else:
-                fn = lambda i: (ix.coarse_split(X[i % 6][:per]), ix.search_assigned(recs[i % 6], K))
-                pre = lambda i: ix.coarse_split(X[i % 6][:per])
-            ms_pre = timeit(pre, 12, warm=3)
-            ms = timeit(fn, 12, warm=3)
-            scan = np.mean(ix.profile_scan_ms()[-12:])
-            _, (D, I, G) = fn(0)
-            if base is None: base = (D.clone(), I.clone())
-            same = bool((D == base[0]).all() and (I == base[1]).all())
-            print(f"C4 shard nprobe {nprobe} {proto}: rank step {ms:.3f} ms (before the exchange {ms_pre:.3f}) -> {B / ms * 1000:.0f} QPS on 8 GPUs, "
-                  f"scan {scan:.3f} ms, same results {same}", flush=True)
-        tune(2, 0)
+        print(f"C4 shard nprobe {nprobe} {proto}: rank step {ms:.3f} ms (before the exchange {ms_pre:.3f}) -> {B / ms * 1000:.0f} QPS on 8 GPUs, "
+              f"scan {scan:.3f} ms, same results {same}", flush=True)
