@@ -53,6 +53,8 @@ struct dph_encoder {
     long long *ids = nullptr, *mask = nullptr, *tt = nullptr;
     float *out_s = nullptr, *out_e = nullptr;
     int64_t cap_b = 0;
+    float* qvec = nullptr;                       // dph_encoder_read: q_start [B,768] | q_end [B,768], apart from the workspace
+    int64_t cap_q = 0;
     int* bad_ids = nullptr;                      // device flag: an input id / token type was outside the embedding tables
     bool bad_pending = false;                    // an asynchronous (device-buffer) forward has not had its flag checked yet
 };
@@ -146,12 +148,17 @@ __global__ void __launch_bounds__(256) embed_ln_kernel(EmbedArgs a) {
 }
 struct LnArgs { const float* in[2]; const float* g[2]; const float* b[2]; float* out[2]; long long rows; long long in_stride, out_stride;
                 unsigned short* out_hi[2]; unsigned short* out_lo[2];             // nullable: dense [rows, 768] bf16 planes of the output
-                const float* filt; float* filt_out; };                            // FILTER: filter_linear weight [2,768] | bias [2] -> [rows, 2]
+                const float* filt; float* filt_out;                               // LN_FILTER, LN_READ: filter_linear weight [2,768] | bias [2] -> [rows, 2]
+                const float* q; float* lg_s; float* lg_e; int S; };               // LN_READ: q_start [B,768] | q_end [B,768] -> [rows] each
+enum { LN_PLAIN = 0, LN_FILTER = 1, LN_READ = 2 };
 // One warp per row, 24 elements per lane as six float4: no shared memory, no block barrier; two-pass mean / variance like
 // torch.nn.LayerNorm.  in/out row strides allow normalising only the [CLS] rows of the last layer.
-// FILTER (last layer of the phrase path): the filter head, 768 -> 2 in fp32, on the normalised row while it is in registers.
-template <bool FILTER>
+// LN_FILTER (last layer of the phrase path): the filter head, 768 -> 2 in fp32, on the normalised row while it is in registers.
+// LN_READ (last layer of the phrase path in Encoder.forward with a question): the same filter head, plus the row's dot products with
+// its own sequence's q_start and q_end (row / S) in the same fixed fmaf order; the normalised row itself is not written.
+template <int EPI>
 __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
+    constexpr bool FILTER = EPI != LN_PLAIN, READ = EPI == LN_READ;
     const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
     const int tw = blockIdx.y, lane = threadIdx.x & 31;
     if (row >= a.rows) return;
@@ -175,13 +182,25 @@ __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
     const float4* g = reinterpret_cast<const float4*>(a.g[tw]);
     const float4* b = reinterpret_cast<const float4*>(a.b[tw]);
     float4* o = reinterpret_cast<float4*>(a.out[tw] + row * a.out_stride);
-    float f0 = 0.f, f1 = 0.f;
+    float f0 = 0.f, f1 = 0.f, d0 = 0.f, d1 = 0.f;
+    const float4* qs = nullptr; const float4* qe = nullptr;
+    if constexpr (READ) {
+        const long long seq = row / a.S, nseq = a.rows / a.S;
+        qs = reinterpret_cast<const float4*>(a.q + seq * ENC_H);
+        qe = reinterpret_cast<const float4*>(a.q + (nseq + seq) * ENC_H);
+    }
 #pragma unroll
     for (int i = 0; i < 6; i++) {
         const float4 gg = g[lane + 32 * i], bb = b[lane + 32 * i];
         const float4 r4 = make_float4(v[i].x * rstd * gg.x + bb.x, v[i].y * rstd * gg.y + bb.y, v[i].z * rstd * gg.z + bb.z, v[i].w * rstd * gg.w + bb.w);
-        o[lane + 32 * i] = r4;
-        if (a.out_hi[tw]) {
+        if constexpr (READ) {
+            const float4 s4 = qs[lane + 32 * i], e4 = qe[lane + 32 * i];
+            d0 = fmaf(r4.x, s4.x, fmaf(r4.y, s4.y, fmaf(r4.z, s4.z, fmaf(r4.w, s4.w, d0))));
+            d1 = fmaf(r4.x, e4.x, fmaf(r4.y, e4.y, fmaf(r4.z, e4.z, fmaf(r4.w, e4.w, d1))));
+        } else {
+            o[lane + 32 * i] = r4;
+        }
+        if (!READ && a.out_hi[tw]) {
             uint2 h4, l4;
             enc_split2(r4.x, r4.y, h4.x, l4.x); enc_split2(r4.z, r4.w, h4.y, l4.y);
             reinterpret_cast<uint2*>(a.out_hi[tw] + row * ENC_H)[lane + 32 * i] = h4;
@@ -197,6 +216,11 @@ __global__ void __launch_bounds__(256) layernorm_kernel(LnArgs a) {
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) { f0 += __shfl_xor_sync(0xffffffffu, f0, off); f1 += __shfl_xor_sync(0xffffffffu, f1, off); }
         if (lane == 0) *reinterpret_cast<float2*>(a.filt_out + row * 2) = make_float2(f0 + a.filt[2 * ENC_H], f1 + a.filt[2 * ENC_H + 1]);
+    }
+    if constexpr (READ) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) { d0 += __shfl_xor_sync(0xffffffffu, d0, off); d1 += __shfl_xor_sync(0xffffffffu, d1, off); }
+        if (lane == 0) { a.lg_s[row] = d0; a.lg_e[row] = d1; }
     }
 }
 // gather rows b*S of [B*S, 768] into a dense [B, 768] buffer (the [CLS] rows the last layer's output actually needs)
@@ -416,7 +440,7 @@ DPH_API void dph_encoder_free(dph_encoder* e) {
         float* ws[] = {e->x[t], e->qkv[t], e->ctx[t], e->a[t], e->ffn[t], e->act_hi[t], e->act_lo[t]};
         for (float* p : ws) if (p) cudaFree(p);
     }
-    void* misc[] = {e->ids, e->mask, e->tt, e->out_s, e->out_e, e->bad_ids, e->filt};
+    void* misc[] = {e->ids, e->mask, e->tt, e->out_s, e->out_e, e->bad_ids, e->filt, e->qvec};
     for (void* p : misc) if (p) cudaFree(p);
     delete e;
 }
@@ -587,8 +611,11 @@ static int end_forward(dph_encoder* e, int mem) {
 //     ctx[t] ([B,768]; x[t] when S == 1).  Attention: tensor cores for S <= 64, SIMT above.
 //   phrase path (phrase = true, nt = 1): every layer on every token; the last LayerNorm writes final_out [T,768] and, with
 //     filter_out, the filter head's logits [T,2].  Attention: tensor cores at every S (attention_flash.cu above 64).
+//     With `read`, the last LayerNorm writes no row: it writes the filter logits and each token's dot products with its
+//     sequence's question vectors instead (dph_encoder_read).
+struct ReadEpilogue { const float* q; float* start; float* end; };      // q: q_start [B,768] | q_end [B,768]; start / end: [T]
 static int encoder_forward(dph_encoder* e, const int* tws, int nt, const long long* d_ids, const long long* d_mask, const long long* d_tt, int B, int S,
-                           bool phrase, float* final_out, float* filter_out) {
+                           bool phrase, float* final_out, float* filter_out, const ReadEpilogue* read = nullptr) {
     cudaStream_t st = e->stream;
     const int64_t T = (int64_t)B * S;
     // bf16x3 mode: (hi, lo) planes of the three T x 768 GEMM inputs (x, ctx, a) live in act_hi / act_lo; their producers (LayerNorm,
@@ -697,7 +724,7 @@ static int encoder_forward(dph_encoder* e, const int* tws, int nt, const long lo
         LnArgs ln1{}; for (int t = 0; t < nt; t++) { ln1.in[t] = e->a[t]; ln1.out[t] = e->a[t]; ln1.out_hi[t] = bx ? ah[t] : nullptr; ln1.out_lo[t] = bx ? al[t] : nullptr; }
         ln1.g[0] = Lt[0]->ln1g; ln1.g[1] = Lt[1]->ln1g; ln1.b[0] = Lt[0]->ln1b; ln1.b[1] = Lt[1]->ln1b;
         ln1.rows = rows; ln1.in_stride = ENC_H; ln1.out_stride = ENC_H;
-        layernorm_kernel<false><<<dim3((unsigned)((rows + 7) / 8), (unsigned)nt), 256, 0, st>>>(ln1);
+        layernorm_kernel<LN_PLAIN><<<dim3((unsigned)((rows + 7) / 8), (unsigned)nt), 256, 0, st>>>(ln1);
         DPH_CUDA(cudaGetLastError());
         DPH_TRY(linear(l, 2, A2, bi, nullptr, FF, ENC_FF, ENC_H, 1, rows, bx));                          // intermediate + erf-GELU
         float* XO[2] = {last ? e->ctx[0] : e->x[0], last ? e->ctx[1] : e->x[1]};                         // last layer: dense [B,768] result in ctx
@@ -711,11 +738,15 @@ static int encoder_forward(dph_encoder* e, const int* tws, int nt, const long lo
         ln2.g[0] = Lt[0]->ln2g; ln2.g[1] = Lt[1]->ln2g; ln2.b[0] = Lt[0]->ln2b; ln2.b[1] = Lt[1]->ln2b;
         ln2.rows = rows; ln2.in_stride = ENC_H; ln2.out_stride = ENC_H;
         const dim3 lgrid((unsigned)((rows + 7) / 8), (unsigned)nt);
-        if (final_ln && filter_out) {
+        if (final_ln && read) {
             ln2.filt = e->filt; ln2.filt_out = filter_out;
-            layernorm_kernel<true><<<lgrid, 256, 0, st>>>(ln2);
+            ln2.q = read->q; ln2.lg_s = read->start; ln2.lg_e = read->end; ln2.S = S;
+            layernorm_kernel<LN_READ><<<lgrid, 256, 0, st>>>(ln2);
+        } else if (final_ln && filter_out) {
+            ln2.filt = e->filt; ln2.filt_out = filter_out;
+            layernorm_kernel<LN_FILTER><<<lgrid, 256, 0, st>>>(ln2);
         } else {
-            layernorm_kernel<false><<<lgrid, 256, 0, st>>>(ln2);
+            layernorm_kernel<LN_PLAIN><<<lgrid, 256, 0, st>>>(ln2);
         }
         DPH_CUDA(cudaGetLastError());
     }
@@ -778,6 +809,46 @@ DPH_API int dph_encoder_embed_phrase(dph_encoder* e, const int64_t* ids, const i
     if (mem == DPH_MEM_HOST) {
         DPH_CUDA(cudaMemcpyAsync(out, d_out, (size_t)T * ENC_H * 4, cudaMemcpyDeviceToHost, st));
         if (filter_out) DPH_CUDA(cudaMemcpyAsync(filter_out, d_filt, (size_t)T * 2 * 4, cudaMemcpyDeviceToHost, st));
+    }
+    return end_forward(e, mem);
+}
+
+// == Encoder.forward(input_ids, ..., input_ids_, ...) without return_phrase / return_query (encoder.py:120-153, 206-208, 260):
+// the question's two [CLS] vectors first (query path, kept in qvec because the phrase tower reuses the workspace), then the
+// phrase tower, whose last LayerNorm turns each token row into start_out[t] = row . q_start, end_out[t] = row . q_end (fp32, fixed
+// order) and filter_out[t] = filter_linear(row) without writing the [B,S,768] rows.  Padding positions get logits too.
+DPH_API int dph_encoder_read(dph_encoder* e, const int64_t* ids, const int64_t* mask, const int64_t* tt, int B, int S, const int64_t* q_ids,
+                             const int64_t* q_mask, const int64_t* q_tt, int Sq, float* start_out, float* end_out, float* filter_out, int mem) {
+    DPH_CHECK(e && e->blob[0] && e->blob[1], "query towers (query_start_encoder, query_end_encoder) not loaded");
+    DPH_CHECK(e->blob[2], "phrase tower (phrase_encoder) not loaded");
+    DPH_CHECK(e->filt, "filter head (filter_linear) not loaded");
+    DPH_CHECK(ids && mask && tt && q_ids && q_mask && q_tt && start_out && end_out && filter_out, "encoder_read: null buffer");
+    DPH_CHECK(B >= 1 && B <= 65535 && S >= 1 && S <= ENC_MAX_S_PHRASE && S <= e->max_pos,
+              "context: 1 <= B <= 65535 and 1 <= S <= min(512, max_position_embeddings)");
+    DPH_CHECK(Sq >= 1 && Sq <= ENC_MAX_S && Sq <= e->max_pos, "question: 1 <= Sq <= min(384, max_position_embeddings)");
+    DPH_CHECK(e->attention_tc || S <= ENC_MAX_S, "the SIMT attention (set_attention(0)) handles S <= 384");
+    DPH_CUDA(cudaSetDevice(e->device));
+    cudaStream_t st = e->stream;
+    const long long *d_ids, *d_mask, *d_tt;
+    DPH_TRY(begin_forward(e, q_ids, q_mask, q_tt, (int64_t)B * Sq, 0, 2, mem, &d_ids, &d_mask, &d_tt));
+    if (B > e->cap_q) { e->cap_q = 0; DPH_TRY(regrow((void**)&e->qvec, (size_t)2 * B * ENC_H * 4)); e->cap_q = B; }
+    const int qtws[2] = {0, 1};
+    DPH_TRY(encoder_forward(e, qtws, 2, d_ids, d_mask, d_tt, B, Sq, false, nullptr, nullptr));
+    for (int t = 0; t < 2; t++)        // [CLS] rows: ctx (Sq >= 2) or x (Sq == 1), as in dph_encoder_embed_query
+        DPH_CUDA(cudaMemcpyAsync(e->qvec + (size_t)t * B * ENC_H, Sq >= 2 ? e->ctx[t] : e->x[t], (size_t)B * ENC_H * 4, cudaMemcpyDeviceToDevice, st));
+    const int64_t T = (int64_t)B * S;
+    DPH_TRY(begin_forward(e, ids, mask, tt, T, 0, 1, mem, &d_ids, &d_mask, &d_tt));
+    // host buffers: the logits go to workspace that is dead by the last LayerNorm (ctx, qkv), then to the caller
+    float* d_s = mem == DPH_MEM_HOST ? e->ctx[0] : start_out;
+    float* d_e = mem == DPH_MEM_HOST ? e->ctx[0] + T : end_out;
+    float* d_f = mem == DPH_MEM_HOST ? e->qkv[0] : filter_out;
+    const ReadEpilogue rd{e->qvec, d_s, d_e};
+    const int ptws[1] = {2};
+    DPH_TRY(encoder_forward(e, ptws, 1, d_ids, d_mask, d_tt, B, S, true, nullptr, d_f, &rd));
+    if (mem == DPH_MEM_HOST) {
+        DPH_CUDA(cudaMemcpyAsync(start_out, d_s, (size_t)T * 4, cudaMemcpyDeviceToHost, st));
+        DPH_CUDA(cudaMemcpyAsync(end_out, d_e, (size_t)T * 4, cudaMemcpyDeviceToHost, st));
+        DPH_CUDA(cudaMemcpyAsync(filter_out, d_f, (size_t)T * 2 * 4, cudaMemcpyDeviceToHost, st));
     }
     return end_forward(e, mem);
 }

@@ -6,7 +6,9 @@ Mirror of reference densephrases/encoder.py (class Encoder):
   `query_start_encoder.*` / `query_end_encoder.*` entries of the reference state dict;
 - phrase side: `embed_phrase` (:92-99) and `forward(input_ids=..., attention_mask=..., token_type_ids=..., return_phrase=True)`
   (:130-144) -> (start, end, filter_start_logits, filter_end_logits): the `phrase_encoder.*` tower over every token (start and end
-  are the same [B,S,768] tensor) and the `filter_linear` head (768 -> 2) on it.
+  are the same [B,S,768] tensor) and the `filter_linear` head (768 -> 2) on it;
+- reading: `forward(input_ids=..., input_ids_=..., ...)` with neither flag (:120-153, 206-208, 260) -> (start_logits, end_logits,
+  filter_start_logits, filter_end_logits), each [B,S]: every token's phrase vector dotted with its question's two vectors.
 Legacy names `bert_start.*` / `bert_q_start.*` / `bert_q_end.*` are accepted like single_utils.backward_compat (:36-56).  Training
 losses are out of scope (SURVEY.md 8a).  Compute: libdph_b200 (wgmma TF32 / bf16 GEMMs, tensor-core attention, fp32 everything else)."""
 import ctypes as C
@@ -210,14 +212,52 @@ class Encoder(object):
         out, _ = self._phrase(input_ids, attention_mask, token_type_ids, with_filter=False)
         return out, out
 
+    def read(self, input_ids, attention_mask, token_type_ids, input_ids_, attention_mask_, token_type_ids_):
+        """Context int64 [B,S] (S <= 512) and question int64 [B,Sq] (Sq <= 384) tensors (cuda or cpu) -> (start_logits, end_logits,
+        filter_start_logits, filter_end_logits), fp32 [B,S] on the GPU (encoder.py:120-153, 206-208, 260): the phrase tower's
+        token vectors dotted with their question's q_start / q_end, and the filter head; padding positions included."""
+        if not self.has_query:
+            raise NotImplementedError('this encoder has no query towers (phrase-only)')
+        if not self.has_phrase:
+            raise NotImplementedError('this encoder has no phrase tower: load a state dict with phrase_encoder.* weights')
+        if not self.has_filter:
+            raise NotImplementedError('this encoder has no filter head: load a state dict with filter_linear.{weight,bias}')
+        B, S = check_phrase_shape(self.config, input_ids.shape)
+        if len(input_ids_.shape) != 2 or int(input_ids_.shape[0]) != B:
+            raise ValueError(f'question batch {tuple(input_ids_.shape)} does not match the context batch {tuple(input_ids.shape)}')
+        Sq = int(input_ids_.shape[1])
+        limit = min(384, self.config.max_position_embeddings)
+        if not 1 <= Sq <= limit:
+            raise ValueError(f'question length {Sq} outside 1..{limit}')
+        attention_mask = torch.ones_like(input_ids) if attention_mask is None else attention_mask
+        token_type_ids = torch.zeros_like(input_ids) if token_type_ids is None else token_type_ids
+        attention_mask_ = torch.ones_like(input_ids_) if attention_mask_ is None else attention_mask_
+        token_type_ids_ = torch.zeros_like(input_ids_) if token_type_ids_ is None else token_type_ids_
+        self._check_ids(input_ids, token_type_ids)
+        self._check_ids(input_ids_, token_type_ids_)
+        ids, mask, tt, qids, qmask, qtt = (x.to(self.device, dtype=torch.int64).contiguous() for x in
+                                           (input_ids, attention_mask, token_type_ids, input_ids_, attention_mask_, token_type_ids_))
+        start = torch.empty((B, S), dtype=torch.float32, device=self.device)
+        end = torch.empty_like(start)
+        filt = torch.empty((B, S, 2), dtype=torch.float32, device=self.device)
+        L.check(L.lib().dph_encoder_set_stream(self._h, C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)))
+        L.check(L.lib().dph_encoder_read(self._h, ids.data_ptr(), mask.data_ptr(), tt.data_ptr(), B, S, qids.data_ptr(), qmask.data_ptr(),
+                                         qtt.data_ptr(), Sq, start.data_ptr(), end.data_ptr(), filt.data_ptr(), L.MEM_DEVICE))
+        return start, end, filt[..., 0], filt[..., 1]
+
     def forward(self, input_ids=None, attention_mask=None, token_type_ids=None, input_ids_=None, attention_mask_=None, token_type_ids_=None,
-                return_phrase=False, return_query=False, **unused):
+                start_positions=None, end_positions=None, return_phrase=False, return_query=False, neg_input_ids=None,
+                neg_attention_mask=None, neg_token_type_ids=None, **unused):
+        if any(x is not None for x in (start_positions, end_positions, neg_input_ids, neg_attention_mask, neg_token_type_ids)):
+            raise NotImplementedError('training arguments (start_positions, end_positions, neg_*) are not supported: inference only')
         if input_ids is not None and return_phrase:
             out, filt = self._phrase(input_ids, attention_mask, token_type_ids, with_filter=True)
             return out, out, filt[..., 0], filt[..., 1]
+        if input_ids is not None and input_ids_ is not None and not return_query:
+            return self.read(input_ids, attention_mask, token_type_ids, input_ids_, attention_mask_, token_type_ids_)
         if input_ids is not None or not return_query:
-            raise NotImplementedError('on the GPU: the phrase side with return_phrase=True (encoder.py:130-144) and the query side with '
-                                      'return_query=True (encoder.py:146-152)')
+            raise NotImplementedError('on the GPU: the phrase side with return_phrase=True (encoder.py:130-144), the query side with '
+                                      'return_query=True (encoder.py:146-152), and both sides without either (encoder.py:120-153, 260)')
         assert len(input_ids_.size()) == 2
         return self.embed_query(input_ids_, attention_mask_, token_type_ids_)
 

@@ -368,6 +368,28 @@ int dph_encoder_embed_query(dph_encoder* e, const int64_t* input_ids, const int6
  * (start logit, end logit).  Host buffers: synchronous; device buffers: asynchronous on the encoder's stream. */
 int dph_encoder_embed_phrase(dph_encoder* e, const int64_t* input_ids, const int64_t* attention_mask, const int64_t* token_type_ids,
                              int B, int S, float* out, float* filter_out, int mem);
+/* Encoder.forward with a context and a question (encoder.py:120-153, 206-208, 260): context ids / mask / token types int64 [B,S]
+ * (S <= min(512, max_position_embeddings), B <= 65535), question ids / mask / token types int64 [B,Sq] (Sq <= 384) ->
+ * start_out, end_out fp32 [B,S] = each token's phrase vector . its question's q_start / q_end, filter_out fp32 [B,S,2] = the
+ * filter head as in dph_encoder_embed_phrase (bit-identical).  The [B,S,768] phrase vectors are never written.  Needs all three
+ * towers and the filter head.  Host buffers: synchronous; device buffers: asynchronous on the encoder's stream. */
+int dph_encoder_read(dph_encoder* e, const int64_t* input_ids, const int64_t* attention_mask, const int64_t* token_type_ids, int B, int S,
+                     const int64_t* input_ids_, const int64_t* attention_mask_, const int64_t* token_type_ids_, int Sq,
+                     float* start_out, float* end_out, float* filter_out, int mem);
+
+/* ---- span decoding of compute_predictions_logits (densephrases/utils/squad_metrics.py:408-684), spans.cu ----
+ * start / end / sft / eft fp32 [F,S] (S <= 512), n_tokens int32 [F] (<= S), start_ok / end_ok uint32 bit masks [F, ceil(S/32)]
+ * (bit s of row f: token s of feature f may start / end a span), ex_off int64 [E+1] (the features of example x are
+ * ex_off[x] .. ex_off[x+1]-1, at least one each).  Per example: cand int32 [E,K,3] = the first n_cand[x] (<= K) prelim
+ * candidates (feature within the example, start, end) in the reference's order (score double(start)+double(end) descending,
+ * ties in enumeration order), total_count / vec_count int64 [E] = valid spans before / after the filter test, and for
+ * version_2 the null feature int32 [E] (within the example; -1 if no feature scores below 1e6) with its (start, end) logits
+ * fp32 [E,2].  1 <= max_answer_length <= 64, 1 <= K <= 1024.  mem: every buffer on the host or every buffer on the device.
+ * Synchronous on cuda_stream. */
+int dph_rc_spans(const float* start, const float* end, const float* sft, const float* eft, int F, int S, const int32_t* n_tokens,
+                 const uint32_t* start_ok, const uint32_t* end_ok, const int64_t* ex_off, int E, int max_answer_length,
+                 double filter_threshold, int K, int version_2, int32_t* cand, int32_t* n_cand, int64_t* total_count,
+                 int64_t* vec_count, int32_t* null_feature, float* null_logits, int mem, void* cuda_stream);
 
 /* ---- exact sequential-k fp32 GEMM (the inner-product definition shared with the oracle): out [n,m] = X [n,K] . W [m,K]^T,
  * acc = fmaf(x[t], w[t], acc) for t ascending; device pointers; K % 32 == 0.  Used for the OPQ rotation and the coarse quantizer. */
