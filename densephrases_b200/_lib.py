@@ -70,6 +70,8 @@ _SIGS = {
     "dph_encoder_read": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32]),
     "dph_rc_spans": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, C.c_double, _i32, _i32, _vp, _vp, _vp, _vp,
                             _vp, _vp, _i32, _vp]),
+    "dph_dump_layout": (_i64, [_i64, _i32, _i32, _vp]),
+    "dph_dump_select": (_i32, [_vp, _vp, _i32, _i32, _vp, _i32, _vp, _i32, C.c_double, C.c_double, C.c_double, _vp, _i64, _vp]),
     "dph_sgemm_nt_seq": (_i32, [_vp, _i64, _vp, _i64, _i64, _vp, _vp]),
     "dph_gemm_tf32_nt": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _i64, _i32, _i32, _vp]),
     "dph_encoder_set_precision": (_i32, [_vp, _i32]),

@@ -707,7 +707,7 @@ def read_idx2id(path):
 
 
 class _H5Writer:
-    """Emits the same subset: superblock v0, version-1 object headers, one-level group B-trees (<= 256 links per group),
+    """Emits the same subset: superblock v0, version-1 object headers, group B-trees of as many levels as the links need,
     contiguous datasets.  Test / export helper."""
     LEAF_K, INTERNAL_K = 4, 16
 
@@ -790,7 +790,7 @@ class _H5Writer:
 
     def _attr_msgs(self, attrs):
         """{name: str (variable-length UTF-8 string in a global heap collection, what h5py writes for `g.attrs[k] = "text"`) |
-        bytes (fixed-length string)} -> version-1 attribute messages."""
+        bytes (fixed-length string) | float (float64 scalar) | int (int64 scalar)} -> version-1 attribute messages."""
         if not attrs:
             return []
         vlen = [(k, v.encode('utf-8')) for k, v in attrs.items() if isinstance(v, str)]
@@ -812,6 +812,12 @@ class _H5Writer:
                 dt = struct.pack('<BBBBI', 0x19, 0x01, 0x01, 0, 16) + struct.pack('<BBBBI', 0x13, 0x10, 0, 0, 1)   # vlen string of UTF-8 chars
                 idx, n = objs[k]
                 data = struct.pack('<IQI', n, coll_at, idx)
+            elif isinstance(v, float):                                                     # what h5py writes for a Python float
+                dt = struct.pack('<BBBBI', 0x11, 0x20, 63, 0, 8) + struct.pack('<HHBBBBI', 0, 64, 52, 11, 0, 52, 1023)
+                data = struct.pack('<d', v)
+            elif isinstance(v, int) and not isinstance(v, bool):                           # ... and for a Python int
+                dt = struct.pack('<BBBBI', 0x10, 0x08, 0, 0, 8) + struct.pack('<HH', 0, 64)
+                data = struct.pack('<q', v)
             else:
                 raw = bytes(v) + b'\0'
                 dt = struct.pack('<BBBBI', 0x13, 0x00, 0, 0, len(raw))                      # null-terminated ASCII string
@@ -823,8 +829,6 @@ class _H5Writer:
     def group(self, links, attrs=None):
         """links {name: object header address} -> (header address, btree address, heap address)"""
         names = sorted(links)                                  # the B-tree orders links by name
-        if len(names) > 2 * self.LEAF_K * 2 * self.INTERNAL_K:
-            raise ValueError('too many links for the one-level group writer')
         heap = bytearray(8)                                    # offset 0: the empty name
         offs = {}
         for n in names:
@@ -841,12 +845,28 @@ class _H5Writer:
             ent += b'\0' * (40 * (per - len(part)))
             snods.append(self.alloc(b'SNOD' + struct.pack('<BBH', 1, 0, len(part)) + ent))
             keys.append(offs[part[-1]])
-        node = b'TREE' + struct.pack('<BBHQQ', 0, 0, len(snods), _UNDEF, _UNDEF) + struct.pack('<Q', keys[0])
-        for s, k in zip(snods, keys[1:]):
-            node += struct.pack('<QQ', s, k)
-        node += b'\0' * (24 + 8 * (2 * self.INTERNAL_K + 1) + 8 * 2 * self.INTERNAL_K - len(node))
-        tree_at = self.alloc(node)
+        # B-tree levels bottom up, at most 2 * INTERNAL_K children per node; the nodes of a level are linked to their left and right
+        # siblings (libhdf5 may walk a level through them).  Up to 256 links this is the single level-0 node written before.
+        fan, level, children = 2 * self.INTERNAL_K, 0, snods
+        while True:
+            parts = [(children[i:i + fan], keys[i:i + fan + 1]) for i in range(0, len(children), fan)]
+            nodes = [self._tree_node(level, c, k) for c, k in parts]
+            for left, right in zip(nodes, nodes[1:]):
+                struct.pack_into('<Q', self.b, left + 16, right)
+                struct.pack_into('<Q', self.b, right + 8, left)
+            if len(nodes) == 1:
+                tree_at = nodes[0]
+                break
+            keys = [k[0] for _, k in parts] + [parts[-1][1][-1]]
+            children, level = nodes, level + 1
         return self._header([self._msg(0x0011, struct.pack('<QQ', tree_at, heap_at))] + self._attr_msgs(attrs)), tree_at, heap_at
+
+    def _tree_node(self, level, children, keys):
+        node = b'TREE' + struct.pack('<BBHQQ', 0, level, len(children), _UNDEF, _UNDEF) + struct.pack('<Q', keys[0])
+        for c, k in zip(children, keys[1:]):
+            node += struct.pack('<QQ', c, k)
+        node += b'\0' * (24 + 8 * (2 * self.INTERNAL_K + 1) + 8 * 2 * self.INTERNAL_K - len(node))
+        return self.alloc(node)
 
     def finish(self, root):
         header, tree, heap = root
@@ -861,7 +881,8 @@ class _H5Writer:
 def write_hdf5(path, tree, chunks=None, attrs=None):
     """tree: nested dict {name: dict | ndarray} -> HDF5 file in the subset read_hdf5 understands.
     chunks {dataset name: chunk shape}: store those datasets chunked with shuffle + deflate instead of contiguous.
-    attrs {group name: {attribute: str | bytes}}: string attributes of the groups with that name (phrase dumps: context / title)."""
+    attrs {group name: {attribute: str | bytes | float | int}}: attributes of the groups with that name (phrase dumps: context /
+    title / offset / scale)."""
     w = _H5Writer()
     chunks = chunks or {}
     attrs = attrs or {}

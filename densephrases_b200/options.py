@@ -90,13 +90,19 @@ class Options(object):
         p.add_argument("--truecase_path", type=str, default='truecase/english_with_questions.dist')
         p.add_argument("--truecase", action="store_true")
 
-    # accepted for command-line compatibility; nothing on the retrieval path reads them
+    # the lambda_* flags are accepted for command-line compatibility; the dump flags are read by dump.py (generate_phrase_vecs.py)
     def add_rc_options(self):
         p = self.parser
         for name in ('lambda_kl', 'lambda_neg', 'lambda_flt'):
             p.add_argument(f'--{name}', default=0.0, type=float)
+        p.add_argument('--predict_file', type=str, default=None)
+        p.add_argument('--append_title', action='store_true')
+        p.add_argument('--per_gpu_eval_batch_size', type=int, default=12)
+        p.add_argument('--do_dump', action='store_true')
+        p.add_argument('--filter_only', action='store_true')
         p.add_argument('--dense_offset', type=float, default=-2)
         p.add_argument('--dense_scale', type=float, default=20)
+        p.add_argument('--filter_threshold', type=float, default=-1e8)
 
     def add_qsft_options(self):
         p = self.parser

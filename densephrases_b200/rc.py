@@ -121,6 +121,13 @@ def tokens_to_string(tokenizer, tokens):
 def get_final_text(pred_text, orig_text, do_lower_case, verbose_logging=False):
     """Map a normalised prediction back onto the original text: basic-tokenise orig_text, align the two texts character by
     character once spaces are removed, and cut orig_text at the aligned ends.  orig_text when the alignment fails."""
+    lo, hi = final_text_span(pred_text, orig_text, do_lower_case, verbose_logging)
+    return orig_text[lo:hi] if (lo, hi) != (0, len(orig_text)) else orig_text
+
+
+def final_text_span(pred_text, orig_text, do_lower_case, verbose_logging=False):
+    """get_final_text(..., return_pos=True): the aligned [start, end) character range in orig_text, (0, len(orig_text)) when the
+    alignment fails."""
     def no_spaces(text):
         chars, where = [], {}
         for i, c in enumerate(text):
@@ -131,29 +138,30 @@ def get_final_text(pred_text, orig_text, do_lower_case, verbose_logging=False):
 
     tok_text = ' '.join(basic_tokenize(orig_text, do_lower_case=do_lower_case))
     first = tok_text.find(pred_text)
+    fail = (0, len(orig_text))
     if first == -1:
         if verbose_logging:
             logger.info("Unable to find text: '%s' in '%s'", pred_text, orig_text)
-        return orig_text
+        return fail
     last = first + len(pred_text) - 1
     orig_ns, orig_map = no_spaces(orig_text)
     tok_ns, tok_map = no_spaces(tok_text)
     if len(orig_ns) != len(tok_ns):
         if verbose_logging:
             logger.info("Length not equal after stripping spaces: '%s' vs '%s'", orig_ns, tok_ns)
-        return orig_text
+        return fail
     tok_to_ns = {pos: i for i, pos in tok_map.items()}
     lo = orig_map.get(tok_to_ns[first]) if first in tok_to_ns else None
     if lo is None:
         if verbose_logging:
             logger.info("Couldn't map start position")
-        return orig_text
+        return fail
     hi = orig_map.get(tok_to_ns[last]) if last in tok_to_ns else None
     if hi is None:
         if verbose_logging:
             logger.info("Couldn't map end position")
-        return orig_text
-    return orig_text[lo:hi + 1]
+        return fail
+    return lo, hi + 1
 
 
 def _compute_softmax(scores):

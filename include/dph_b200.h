@@ -391,6 +391,25 @@ int dph_rc_spans(const float* start, const float* end, const float* sft, const f
                  double filter_threshold, int K, int version_2, int32_t* cand, int32_t* n_cand, int64_t* total_count,
                  int64_t* vec_count, int32_t* null_feature, float* null_logits, int mem, void* cuda_stream);
 
+/* ---- phrase dump (generate_phrase_vecs.py --do_dump; embed_utils.py get_metadata -> filter_metadata -> compress_metadata) ----
+ * dph_dump_layout: byte offsets [7] inside the output buffer of one dph_dump_select call with R valid rows, n_doc documents and
+ * L = max_answer_length -- n_kept int64, doc_kept int32 [n_doc], fallback f2o int64 [n_doc], kept rows int8 [R,768], f2o int64 [R],
+ * start2end int32 [R,L], fallback rows int8 [n_doc,768] -- and returns the buffer size (-1 on bad arguments).
+ * dph_dump_select: start fp32 [B,S,768] and filter logits fp32 [B,S,2] on the device (Encoder's phrase outputs); feat int32 [B,4]
+ * on the host: per feature its valid rows [row_lo, row_hi), its document slot (0, 1, ... over consecutive features) and the
+ * document-level index of row_lo; doc int32 [n_doc,2] on the host: rows the document kept in earlier batches, and 1 when it still
+ * needs filter_metadata's fallback row (the first row with filter_start > -999999, looked for only when the document keeps no row
+ * in this batch either; written to the fallback slot, f2o -1 if none).
+ * A row is kept when filter_start or filter_end > fp32(filter_threshold); kept rows are written in batch order, quantised as
+ * rint(clip((x - offset) * scale, -128, 127)), with their document-level f2o index and start2end remapped to the document's short
+ * indices (-1 for ends outside the feature or failing the filter_end test).  out: page-locked host memory of at least
+ * dph_dump_layout bytes, written by the kernels through its device mapping.  start 16-byte, filt and out 8-byte aligned.
+ * S <= 512, 1 <= L <= 64.  Synchronous on cuda_stream. */
+int64_t dph_dump_layout(int64_t R, int n_doc, int L, int64_t* offsets);
+int dph_dump_select(const float* start, const float* filt, int B, int S, const int32_t* feat, int n_doc, const int32_t* doc,
+                    int max_answer_length, double filter_threshold, double dense_offset, double dense_scale, void* out,
+                    int64_t out_bytes, void* cuda_stream);
+
 /* ---- exact sequential-k fp32 GEMM (the inner-product definition shared with the oracle): out [n,m] = X [n,K] . W [m,K]^T,
  * acc = fmaf(x[t], w[t], acc) for t ascending; device pointers; K % 32 == 0.  Used for the OPQ rotation and the coarse quantizer. */
 int dph_sgemm_nt_seq(const float* X, int64_t n, const float* W, int64_t m, int64_t K, float* out, void* cuda_stream);
