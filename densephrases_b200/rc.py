@@ -9,7 +9,7 @@ csrc/spans.cu): per example it returns the first K prelim candidates in the refe
 descending, ties in enumeration order), the counts before and after the filter, and the version-2 null choice.  The host keeps
 the text side: get_final_text, the softmax, the null handling, the "empty" nonce entries and the files.  The n-best loop skips
 duplicate texts, so it can use up the K candidates of an example before it has n_best_size entries; that example is then decoded
-again with 2K (up to 1024), so the result stays exact.
+again with 2K (up to 1024), and past 1024 its spans are enumerated on the host (host_spans), so the result stays exact.
 
 Reference behaviour reproduced on purpose (pinned by tests/golden/rc_reference.json.gz):
 - the end index runs up to start + max_answer_length - 2, so a span has at most max_answer_length - 1 tokens;
@@ -110,6 +110,27 @@ def best_spans(start, end, sft, eft, n_tokens, start_ok, end_ok, ex_off, max_ans
         out = {n: v.cpu().numpy() for n, v in out.items()}
     return Spans(**out)
 
+
+def host_spans(start, end, sft, eft, n_tokens, start_ok, end_ok, max_answer_length, filter_threshold):
+    """Every span of one example that is valid and passes the filter, in the order of best_spans -> int32 [n,3] (feature within the
+    example, start, end).  numpy [F,S] arrays and masks as best_spans takes them.  For the rare example whose n-best list needs more
+    than MAX_K candidates."""
+    F, S = start.shape
+    bits = lambda m: np.unpackbits(np.ascontiguousarray(m).view('<u4').view(np.uint8), axis=1, bitorder='little')[:, :S].astype(bool)   # noqa: E731
+    inside = np.arange(S)[None, :] < np.asarray(n_tokens)[:, None]
+    thr = float(filter_threshold)
+    s_ok = bits(start_ok) & inside & ~(np.asarray(sft, np.float64) < thr)
+    e_ok = bits(end_ok) & inside & ~(np.asarray(eft, np.float64) < thr)
+    s, j = np.meshgrid(np.arange(S), np.arange(max(0, int(max_answer_length) - 1)), indexing='ij')
+    s, e = s.ravel(), (s + j).ravel()
+    s, e = s[e < S], e[e < S]                          # (start, end) in enumeration order
+    rows, scores = [], []
+    for f in range(F):
+        ok = s_ok[f, s] & e_ok[f, e]
+        rows.append(np.stack([np.full(int(ok.sum()), f), s[ok], e[ok]], 1))
+        scores.append(np.asarray(start[f], np.float64)[s[ok]] + np.asarray(end[f], np.float64)[e[ok]])
+    rows, scores = np.concatenate(rows), np.concatenate(scores)
+    return rows[np.lexsort((np.arange(len(scores)), -scores))].astype(np.int32)   # score descending (-0.0 == 0.0), then enumeration
 
 # ---- text side (squad_metrics.py:256-406) -------------------------------------------------------------------------------------------
 def tokens_to_string(tokenizer, tokens):
@@ -269,17 +290,21 @@ def compute_predictions_logits(all_examples, all_features, all_results, n_best_s
         id2candidates[example.qas_id] = {'candidates': [], 'text': example.context_text, 'answer': example.answers, 'recall': False}
         id2candidates[features[-1].qas_id]['save_rate'] = float(0 / int(sp.total_count[x]))
         cand, n_cand, k = sp.cand[x], int(sp.n_cand[x]), k0
-        while True:
-            got = nbest_of(x, example, cand, n_cand, null)
-            if got is not None:
-                break
-            if k >= MAX_K:
-                raise RuntimeError(f'example {x}: more than {MAX_K} candidates needed to fill n_best_size={n_best_size} distinct texts')
-            k = min(MAX_K, 2 * k)
+        got = nbest_of(x, example, cand, n_cand, null)
+        while got is None:
             a, b = ex_off[x], ex_off[x + 1]
-            one = best_spans(st[a:b], en[a:b], sft[a:b], eft[a:b], n_tokens[a:b], start_ok[a:b], end_ok[a:b], np.array([0, b - a], np.int64),
-                             max_answer_length, filter_threshold, k, version_2_with_negative)
-            cand, n_cand = one.cand[0], int(one.n_cand[0])
+            if k < MAX_K:
+                k = min(MAX_K, 2 * k)
+                one = best_spans(st[a:b], en[a:b], sft[a:b], eft[a:b], n_tokens[a:b], start_ok[a:b], end_ok[a:b], np.array([0, b - a], np.int64),
+                                 max_answer_length, filter_threshold, k, version_2_with_negative)
+                cand, n_cand = one.cand[0], int(one.n_cand[0])
+            else:          # past the decoder's K bound (repeated tokens): the whole ordered list, enumerated on the host
+                cand = host_spans(st[a:b], en[a:b], sft[a:b], eft[a:b], n_tokens[a:b], start_ok[a:b], end_ok[a:b], max_answer_length,
+                                  filter_threshold)
+                n_cand = len(cand)
+                if n_cand != int(sp.vec_count[x]):
+                    raise RuntimeError(f'example {x}: {n_cand} spans enumerated on the host, the decoder counted {int(sp.vec_count[x])}')
+            got = nbest_of(x, example, cand, n_cand, null)
         nbest, seen = got
         if version_2_with_negative:
             if '' not in seen:
