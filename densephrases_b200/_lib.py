@@ -80,6 +80,7 @@ _SIGS = {
     "dph_index_window_scores": (_i32, [_vp, _vp, _vp, _i64, _i32, _vp, _i32]),
     "dph_index_encode": (_i32, [_vp, _vp, _i64, _vp, _vp, _i32]),
     "dph_index_add_with_ids": (_i32, [_vp, _vp, _i64, _vp, _i32]),
+    "dph_index_add_int8": (_i32, [_vp, _vp, _i64, _f32, _f32, _vp, _i32]),
     "dph_index_copy_lists": (_i32, [_vp, _vp, _vp]),
     "dph_index_get_list_len": (_i32, [_vp, _vp]),
     "dph_index_last_add_ms": (_i32, [_vp, _vp]),

@@ -403,6 +403,38 @@ def read_meta(path):
         return pickle.load(f)
 
 
+def compress_meta(doc_groups):
+    """compress_metadata.py:compress (:32-70) of {doc_idx: {word2char_start, word2char_end, f2o_start, context, title}}, in place:
+    the three arrays as blosc-zlib frames of typesize 1, the context as a blosc-zlib frame of its UTF-8 bytes (python-blosc's
+    defaults: typesize 8, byte shuffle, level 9), the arrays' dtypes under 'dtypes', the title as it is.  The frames decode to the
+    same bytes as c-blosc's; the bytes of the frames themselves may differ."""
+    for rec in doc_groups.values():
+        dtypes = {name: rec[name].dtype for name in ('word2char_start', 'word2char_end', 'f2o_start')}
+        for name in dtypes:
+            rec[name] = blosc_compress(np.ascontiguousarray(rec[name]).tobytes(), typesize=1, clevel=9)
+        rec['context'] = blosc_compress(rec['context'].encode('utf-8'), typesize=8, clevel=9)
+        rec['dtypes'] = dtypes
+    return doc_groups
+
+
+def write_meta(input_dump_dir, output_dir):
+    """scripts/preprocess/compress_metadata.py (:72-111): the metadata of every `*hdf5*` file of input_dump_dir (sorted; a document in
+    several files keeps its first position and its last record), compressed by compress_meta, pickled to
+    output_dir/meta_compressed.pkl, which MIPS reads.  -> the output path."""
+    doc_groups = {}
+    for name in sorted(n for n in os.listdir(input_dump_dir) if 'hdf5' in n):
+        h = open_hdf5(os.path.join(input_dump_dir, name))
+        for key, addr in h.children(h.root_addr).items():
+            members, attrs = h.children(addr), h.attributes(addr)
+            rec = {t: h.dataset(members[t]) for t in ('word2char_start', 'word2char_end', 'f2o_start')}
+            rec['context'], rec['title'] = attrs['context'], attrs['title']
+            doc_groups[key] = rec
+    out = os.path.join(output_dir, 'meta_compressed.pkl')
+    with open(out, 'wb') as f:
+        pickle.dump(compress_meta(doc_groups), f)
+    return out
+
+
 def decode_meta_field(value, dtype=None):
     """A metadata field as stored by the reference (blosc frame), by this repo's converter (zlib stream) or raw."""
     if isinstance(value, (bytes, bytearray, memoryview)):

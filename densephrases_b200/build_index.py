@@ -33,10 +33,17 @@ Merging sub-indexes (the merge stage of build_phrase_index.py:282-338, DESIGN.md
     # several at once: ix.merge_from([a, b, c], add_id=offset) appends them in order, labels + offset; the sources stay as they were
 add_to_index below is the PyTorch encoder that runs without a GPU; its argmax / argmin have no fixed floating-point order, so on
 ties and near-ties it may pick other lists or codewords than IvfPqIndex.encode."""
+import logging
+import os
+import pickle
+import random
+import time
+
 import numpy as np
 import torch
 
 D, M, KSUB, DSUB = 768, 96, 256, 8
+logger = logging.getLogger(__name__)
 
 
 def _kmeans(x, k, niter, seed, assign_ip=False):
@@ -148,3 +155,309 @@ def build_index(x_train, x_add, nlist, ids=None, seed=123, device=None, **train_
 def save_container(path, index_arrays):
     """Write the `index.dph.npz` container MIPS.__init__ reads (next to where the reference expects index.faiss)."""
     np.savez(path, **index_arrays)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------------
+# build_phrase_index.py over a phrase dump (DESIGN.md 3.8): the stages coarse / fine / all / add / merge of run_index (:341-405)
+# ---------------------------------------------------------------------------------------------------------------------------------
+NO_FILTER = -1e8
+
+
+def int8_to_float(q, offset, scale):
+    """The reference's int8_to_float (embed_utils.py:148-149) as numpy 1.x computed it: the group's float64 offset and scale attributes
+    become fp32 under value-based casting, and the arithmetic is fp32, fl32(fl32(float(q) / scale) + offset).  Numpy 2 would compute
+    in float64; this keeps the fp32 chain.  IvfPqIndex.add_int8 computes the same values on the device."""
+    return np.asarray(q).astype(np.float32) / np.float32(scale) + np.float32(offset)
+
+
+def get_args(argv=None):
+    """build_phrase_index.py:get_args (:19-44): the reference's flags (Options.add_index_options) and the paths derived from them."""
+    from .options import Options
+    options = Options()
+    options.add_index_options()
+    return derive_paths(options.parse(argv))
+
+
+def derive_paths(args):
+    """index_name = <num_clusters>_flat_<fine_quant>[_first][_ft<int>], index_dir = dump_dir/start/<index_name>, and the file paths in
+    it; with --dump_paths the sub-index paths index/<offset>.faiss and index/<offset>.hdf5 and the dump paths under phrase_dir."""
+    coarse = 'hnsw' if args.hnsw else 'flat'
+    args.index_name = f'{args.num_clusters}_{coarse}_{args.fine_quant}{"_first" if args.first_passage else ""}'
+    if args.index_filter != NO_FILTER:
+        args.index_name = args.index_name + f'_ft{int(args.index_filter)}'
+    args.index_dir = os.path.join(args.dump_dir, 'start', args.index_name)
+    args.quantizer_path = os.path.join(args.index_dir, args.quantizer_path)
+    args.trained_index_path = os.path.join(args.index_dir, args.trained_index_path)
+    args.inv_path = os.path.join(args.index_dir, args.inv_path)
+    args.subindex_dir = os.path.join(args.index_dir, args.subindex_name)
+    if args.dump_paths is None:
+        args.index_path = os.path.join(args.index_dir, args.index_path)
+        args.idx2id_path = os.path.join(args.index_dir, args.idx2id_path)
+    else:
+        args.dump_paths = [os.path.join(args.dump_dir, args.phrase_dir, path) for path in args.dump_paths.split(',')]
+        args.index_path = os.path.join(args.subindex_dir, '%d.faiss' % args.offset)
+        args.idx2id_path = os.path.join(args.subindex_dir, '%d.hdf5' % args.offset)
+    return args
+
+
+class _Dump(object):
+    """One dump file through artifacts' HDF5 reader: its documents in the group B-tree's byte-wise name order, which is the order
+    h5py yields them in ("10" before "2")."""
+
+    def __init__(self, path):
+        from . import artifacts
+        self.h = artifacts.open_hdf5(path)
+        self.docs = list(self.h.children(self.h.root_addr).items())
+
+    def members(self, addr):
+        return self.h.children(addr)
+
+    def dataset(self, members, name):
+        return self.h.dataset(members[name])
+
+
+def sample_data(dump_paths, doc_sample_ratio=0.2, vec_sample_ratio=0.2, seed=29, norm_th=999):
+    """build_phrase_index.py:sample_data (:60-93): random.sample of the documents of each file and np.random.choice (with replacement)
+    of the rows of each sampled document, both seeded once with 29, dequantised in fp32 and cut at fp32 norm <= norm_th.
+    -> (sample [n, 768] f32, avg_vec [1, 768], std_vec [1, 768])."""
+    random.seed(seed)
+    np.random.seed(seed)
+    out = []
+    for path in dump_paths:
+        f = _Dump(path)
+        doc_ids = [name for name, _ in f.docs]
+        addr = dict(f.docs)
+        for doc_id in random.sample(doc_ids, int(doc_sample_ratio * len(doc_ids))):
+            members = f.members(addr[doc_id])
+            start = f.dataset(members, 'start')
+            if len(start.shape) < 2 or start.shape[0] == 0:
+                continue
+            idx = np.random.choice(start.shape[0], int(vec_sample_ratio * start.shape[0]))
+            attrs = f.h.attributes(addr[doc_id])
+            vec = int8_to_float(start, attrs['offset'], attrs['scale'])[idx]
+            out.append(vec[np.linalg.norm(vec, axis=1) <= norm_th])
+    x = np.concatenate(out) if out else np.zeros((0, D), np.float32)
+    return x, np.mean(x, axis=0, keepdims=True), np.std(x, axis=0, keepdims=True)
+
+
+def train_phrase_index(x, num_clusters, trained_index_path, device=0):
+    """train_index (:96-142) for OPQ96: IvfPqIndex.train (faiss' recipe, DESIGN.md 3.3), written as trained.faiss with empty lists."""
+    from . import artifacts
+    from .ivfpq import IvfPqIndex
+    if len(x) < max(num_clusters, KSUB):
+        raise ValueError(f'the training sample holds {len(x)} vectors; training IVF{num_clusters} with PQ96 needs at least '
+                         f'max(num_clusters, 256) = {max(num_clusters, KSUB)} (raise doc_sample_ratio / vec_sample_ratio)')
+    ix = IvfPqIndex(num_clusters, device=device)
+    ix.train(np.ascontiguousarray(x, dtype=np.float32))
+    artifacts.write_faiss_index(trained_index_path, ix.opq_matrix(), ix.centroids(), ix.pq_codebooks(), np.zeros(num_clusters, np.int64),
+                                np.zeros((0, M), np.uint8), np.zeros(0, np.int64))
+
+
+def _trained_index(trained_index_path, device=0):
+    from . import artifacts
+    from .ivfpq import IvfPqIndex
+    t = artifacts.read_faiss_index(trained_index_path)
+    return t, IvfPqIndex.from_arrays(t['A'], t['centroids'], t['pq'], np.zeros(len(t['list_len']), np.int64), np.zeros((0, M), np.uint8),
+                                     device=device)
+
+
+def pinned_rows(n):
+    """A page-locked int8 [n, 768] numpy array (add_int8 reads it in place through its device mapping)."""
+    return torch.empty((n, D), dtype=torch.int8).pin_memory().numpy()
+
+
+class _Adder(object):
+    """Gathers the int8 rows of about num_docs_per_add documents into one reused page-locked buffer and hands each run of documents
+    with the same (offset, scale) to add_int8, labels offset + running total.  Host memory stays one batch."""
+
+    def __init__(self, ix, label0, timings):
+        self.ix, self.next_label, self.t = ix, label0, timings
+        self.pending, self.buf = [], None
+
+    def push(self, rows, offset, scale):
+        self.pending.append((rows, float(offset), float(scale)))
+
+    def flush(self):
+        runs, i = [], 0
+        while i < len(self.pending):
+            j = i
+            while j < len(self.pending) and self.pending[j][1:] == self.pending[i][1:]:
+                j += 1
+            runs.append((self.pending[i:j], self.pending[i][1], self.pending[i][2]))
+            i = j
+        self.pending = []
+        for docs, offset, scale in runs:
+            n = sum(len(r) for r, _, _ in docs)
+            if n == 0:
+                continue
+            t0 = time.perf_counter()
+            if self.buf is None or len(self.buf) < n:
+                self.buf = pinned_rows(max(n, 2 * len(self.buf) if self.buf is not None else n))
+            at = 0
+            for r, _, _ in docs:
+                self.buf[at:at + len(r)] = r
+                at += len(r)
+            t1 = time.perf_counter()
+            self.ix.add_int8(self.buf[:n], np.arange(self.next_label, self.next_label + n, dtype=np.int64), offset, scale)
+            t2 = time.perf_counter()
+            self.next_label += n
+            self.t['gather'] = self.t.get('gather', 0.0) + t1 - t0
+            self.t['add'] = self.t.get('add', 0.0) + t2 - t1
+            self.t['rows'] = self.t.get('rows', 0) + n
+            self.t['h2d_bytes'] = self.t.get('h2d_bytes', 0) + n * D
+
+
+def add_dump_to_index(dump_paths, trained_index_path, target_index_path, idx2id_path, num_docs_per_add=1000, offset=0,
+                 first_passage=False, index_filter=NO_FILTER, device=0, timings=None):
+    """build_phrase_index.py:add_to_index (:156-279) for OPQ96 on the GPU: every document with rows, in the dumps' order and each file's
+    h5py order, its rows cut to the first passage (f2o_start < len_per_para[0]) or to the rows the filter dump keeps (index_filter),
+    added through add_int8 with labels offset + running total.  Writes target_index_path (the trained tables and the lists) and
+    idx2id_path ({str(offset): doc, word int32, attrs offset}).  -> the IvfPqIndex.  The reference computes norms against norm_th
+    here but adds every row, and so does this."""
+    from . import artifacts
+    timings = {} if timings is None else timings
+    t, ix = _trained_index(trained_index_path, device)
+    adder = _Adder(ix, offset, timings)
+    doc_out, word_out = [], []
+    for path in dump_paths:
+        t0 = time.perf_counter()
+        f = _Dump(path)
+        ff = _Dump(path.replace('/phrase/', '/filter/')) if index_filter != NO_FILTER else None
+        faddr = dict(ff.docs) if ff is not None else None
+        last = len(f.docs) - 1
+        for i, (doc_idx, addr) in enumerate(f.docs):
+            members = f.members(addr)
+            start = f.dataset(members, 'start')
+            if start.shape[0] == 0:
+                continue
+            attrs = f.h.attributes(addr)
+            if first_passage:
+                f2o = f.dataset(members, 'f2o_start')
+                cut = int((f2o < f.dataset(members, 'len_per_para')[0]).sum())
+                start, words = start[:cut], np.arange(cut)
+            elif index_filter != NO_FILTER:
+                fm = ff.members(faddr[doc_idx])
+                fs, fe = ff.dataset(fm, 'filter_start'), ff.dataset(fm, 'filter_end')
+                o2f = {orig: ft for ft, orig in enumerate(f.dataset(members, 'f2o_start').tolist())}
+                keep = set(np.concatenate([np.where(fs > index_filter)[0], np.where(fe > index_filter)[0]]).tolist())
+                words = np.asarray(sorted(o2f[si] for si in keep if si in o2f), dtype=np.int64)
+                start = start[words]
+            else:
+                words = np.arange(len(start))
+            adder.push(start, attrs['offset'], attrs['scale'])
+            doc_out.append(np.full(len(start), int(doc_idx), dtype=np.int32))
+            word_out.append(words.astype(np.int32))
+            if i % num_docs_per_add == 0 or i == last:
+                timings['read'] = timings.get('read', 0.0) + time.perf_counter() - t0
+                adder.flush()
+                t0 = time.perf_counter()
+        timings['read'] = timings.get('read', 0.0) + time.perf_counter() - t0
+        adder.flush()
+    t0 = time.perf_counter()
+    list_len, codes, ids = ix.lists()
+    artifacts.write_faiss_index(target_index_path, t['A'], t['centroids'], t['pq'], list_len, codes, ids)
+    doc = np.concatenate(doc_out) if doc_out else np.zeros(0, np.int32)
+    word = np.concatenate(word_out) if word_out else np.zeros(0, np.int32)
+    artifacts.write_hdf5(idx2id_path, {str(offset): {'doc': doc, 'word': word}}, attrs={str(offset): {'offset': int(offset)}})
+    timings['write'] = timings.get('write', 0.0) + time.perf_counter() - t0
+    return ix
+
+
+def merge_indexes(subindex_dir, trained_index_path, target_index_path, target_idx2id_path, target_inv_path):
+    """build_phrase_index.py:merge_indexes (:282-338) without a GPU: each list holds the sub-indexes' entries of that list in source
+    order (faiss OnDiskInvertedLists.merge_from), written as index.faiss with its lists in the side file target_inv_path, and the
+    idx2id groups of every sub-index in one idx2id.hdf5.  The sub-indexes are taken in ascending offset order; the reference takes
+    os.listdir's order, which depends on the file system.  A sub-index whose OPQ matrix, centroids or PQ codebooks differ in any bit
+    from trained.faiss is rejected."""
+    from . import artifacts
+    names = os.listdir(subindex_dir)
+    offsets = sorted(int(n[:-len('.faiss')]) for n in names if n.endswith('.faiss'))
+    if sorted(int(n[:-len('.hdf5')]) for n in names if n.endswith('.hdf5')) != offsets:
+        raise ValueError(f'{subindex_dir}: the .faiss and .hdf5 sub-index files do not pair up')
+    t = artifacts.read_faiss_index(trained_index_path)
+    nlist = len(t['list_len'])
+    list_no, codes, ids, idx2id = [], [], [], {}
+    for off in offsets:
+        sub = artifacts.read_faiss_index(os.path.join(subindex_dir, '%d.faiss' % off))
+        for key in ('A', 'centroids', 'pq'):
+            if sub[key].shape != t[key].shape or not np.array_equal(sub[key].view(np.uint32), t[key].view(np.uint32)):
+                raise ValueError(f'{off}.faiss: its {key} is not bit-identical to {trained_index_path}')
+        list_no.append(np.repeat(np.arange(nlist, dtype=np.int64), sub['list_len']))
+        codes.append(sub['codes']); ids.append(sub['ids'])
+        for key, g in artifacts.read_idx2id(os.path.join(subindex_dir, '%d.hdf5' % off)).items():
+            if key in idx2id:
+                raise ValueError(f'idx2id group {key} appears in two sub-indexes')
+            idx2id[key] = g
+    list_len, codes, ids = to_list_major(np.concatenate(list_no + [np.zeros(0, np.int64)]),
+                                         np.concatenate(codes + [np.zeros((0, M), np.uint8)]),
+                                         np.concatenate(ids + [np.zeros(0, np.int64)]), nlist)
+    artifacts.write_faiss_index(target_index_path, t['A'], t['centroids'], t['pq'], list_len, codes, ids,
+                                ondisk_payload=os.path.basename(target_inv_path))
+    artifacts.write_hdf5(target_idx2id_path, {k: {'doc': g['doc'], 'word': g['word']} for k, g in idx2id.items()},
+                         attrs={k: {'offset': int(k)} for k in idx2id})
+    return list_len, codes, ids
+
+
+def check_args(args):
+    """The refusals of this builder: it builds the OPQ96 / IVF-flat index only (DESIGN.md 0) and has no `move` stage."""
+    if args.stage not in ('all', 'coarse', 'fine', 'add', 'merge'):
+        raise ValueError(f'--stage {args.stage!r}: this builder runs all, coarse, fine, add and merge (move is not supported)')
+    if args.fine_quant != 'OPQ96' or args.hnsw:
+        raise ValueError(f'--fine_quant {args.fine_quant}{" --hnsw" if args.hnsw else ""}: only the OPQ96 IVF-flat index '
+                         '(--fine_quant OPQ96, no --hnsw) is supported; SQ4, flat ("none") and HNSW indexes are not')
+    if args.first_passage and args.index_filter != NO_FILTER:
+        raise ValueError('--first_passage and --index_filter together: the reference fails on this combination; pass one of them')
+
+
+def run_index(args, device=0, timings=None):
+    """build_phrase_index.py:run_index (:341-405) on the GPU (with or without --cuda; there is no CPU path) for args from get_args.
+    Stage `fine` on its own draws the sample again (the reference fails there with UnboundLocalError and an unexpected hnsw= keyword
+    of sample_data).  Files that exist are kept unless --replace, as in the reference.  timings (dict): seconds of each stage."""
+    check_args(args)
+    timings = {} if timings is None else timings
+    phrase_dir = os.path.join(args.dump_dir, args.phrase_dir)
+    names = os.listdir(phrase_dir) if os.path.isdir(phrase_dir) else []
+    dump_paths = sorted(os.path.join(phrase_dir, n) for n in names if n.endswith('.hdf5'))
+    sample = None
+
+    def draw():
+        t0 = time.perf_counter()
+        out = sample_data(dump_paths, args.doc_sample_ratio, args.vec_sample_ratio, norm_th=args.norm_th)
+        timings['sample'] = timings.get('sample', 0.0) + time.perf_counter() - t0
+        return out
+
+    # The reference never writes quantizer_path for OPQ indexes, so `all` and `coarse` always draw the sample.
+    if args.stage in ('all', 'coarse') and (args.replace or not os.path.exists(args.quantizer_path)):
+        os.makedirs(args.index_dir, exist_ok=True)
+        sample, avg_vec, std_vec = draw()
+        with open(os.path.join(args.index_dir, 'avg_vec.pkl'), 'wb') as fp:
+            pickle.dump(avg_vec, fp)
+        with open(os.path.join(args.index_dir, 'std_vec.pkl'), 'wb') as fp:
+            pickle.dump(std_vec, fp)
+    if args.stage in ('all', 'fine') and (args.replace or not os.path.exists(args.trained_index_path)):
+        os.makedirs(args.index_dir, exist_ok=True)
+        if sample is None:
+            sample = draw()[0]
+        t0 = time.perf_counter()
+        train_phrase_index(sample, args.num_clusters, args.trained_index_path, device)
+        timings['train'] = time.perf_counter() - t0
+    if args.stage in ('all', 'add') and (args.replace or not os.path.exists(args.index_path)):
+        if args.dump_paths is not None:
+            dump_paths = args.dump_paths
+            os.makedirs(args.subindex_dir, exist_ok=True)
+        add_dump_to_index(dump_paths, args.trained_index_path, args.index_path, args.idx2id_path, num_docs_per_add=args.num_docs_per_add,
+                     offset=args.offset, first_passage=args.first_passage, index_filter=args.index_filter, device=device, timings=timings)
+    if args.stage == 'merge' and (args.replace or not os.path.exists(args.index_path)):
+        t0 = time.perf_counter()
+        merge_indexes(args.subindex_dir, args.trained_index_path, args.index_path, args.idx2id_path, args.inv_path)
+        timings['merge'] = time.perf_counter() - t0
+    return timings
+
+
+def main(argv=None):
+    logging.basicConfig(format='%(asctime)s - %(levelname)s - %(name)s -   %(message)s', level=logging.INFO)
+    run_index(get_args(argv))
+
+
+if __name__ == '__main__':
+    main()

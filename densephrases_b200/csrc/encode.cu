@@ -4,7 +4,9 @@
 //   tie rule), r = xr - C[list] (fp32), dist[m][j] = fmaf chain over the 8 squared differences, code[m] = argmin_j (lowest j on ties).
 #include "index_internal.cuh"
 #include <algorithm>
+#include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
 #define ENC_TILE 128           // vectors per CTA, one per thread
 #define ENC_CB_FLOATS (DPH_KSUB * DPH_DSUB)   // one sub-quantizer's codebook: 256 x 8 fp32 = 8 KB
@@ -81,6 +83,28 @@ __global__ void nonfinite_kernel(const float* __restrict__ x, long long count, i
     if (__syncthreads_or(hit) && threadIdx.x == 0) atomicOr(bad, 1);
 }
 
+// x = fl32(fl32(q / scale) + offset) for int8 q: numpy 1.x's int8_to_float (embed_utils.py:148-149) with the dump's offset and scale
+// attributes cast to fp32, as value-based casting does.  An IEEE division, not a multiply by 1 / scale, and a separate add, no FMA.
+// 16 values per thread; q is read with one 16-byte load when it is 16-byte aligned (then every group is: d is a multiple of 16),
+// else byte by byte, so that a view at any byte offset of a memory-mapped file is read correctly.
+__global__ void dequant_int8_kernel(const int8_t* __restrict__ q, long long groups, float offset, float scale, int vec, float* __restrict__ x) {
+    for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += (long long)gridDim.x * blockDim.x) {
+        int8_t b[16];
+        if (vec) {
+            const int4 v = reinterpret_cast<const int4*>(q)[g];
+            memcpy(b, &v, 16);
+        } else {
+#pragma unroll
+            for (int i = 0; i < 16; i++) b[i] = q[g * 16 + i];
+        }
+        float4* out = reinterpret_cast<float4*>(x) + g * 4;
+#pragma unroll
+        for (int i = 0; i < 4; i++)
+            out[i] = make_float4(__fadd_rn(__fdiv_rn((float)b[4 * i], scale), offset), __fadd_rn(__fdiv_rn((float)b[4 * i + 1], scale), offset),
+                                 __fadd_rn(__fdiv_rn((float)b[4 * i + 2], scale), offset), __fadd_rn(__fdiv_rn((float)b[4 * i + 3], scale), offset));
+    }
+}
+
 int64_t dph_encode_chunk(const dph_index* ix) {
     const int64_t nlp = (ix->nlist + 127) / 128 * 128;
     int64_t c = std::min<int64_t>((1ll << 28) / nlp, 65536);           // coarse scores S [c, nlist] <= 1 GiB, as for search
@@ -146,6 +170,38 @@ int dph_encode_rows(dph_index* ix, const float* x, int64_t n, int64_t* list_out,
     for (int64_t o = 0; o < n; o += cs) {
         const int64_t m = std::min(cs, n - o);
         DPH_TRY(encode_rows_chunk(ix, x + o * ix->d, m, list_out + o, codes_out + o * DPH_M, bad));
+    }
+    return 0;
+}
+
+int dph_encode_int8(dph_index* ix, const int8_t* q, int64_t n, float offset, float scale, int mem, int64_t* list_out, uint8_t* codes_out,
+                    int* bad) {
+    const int64_t d = ix->d, cs = std::min(dph_encode_chunk(ix), n);
+    DPH_CHECK(d % 16 == 0, "add_int8: d must be a multiple of 16");
+    // Device input is read in place; so is page-locked host input, through its device mapping.  Pageable host input is copied to a
+    // device staging chunk of int8.  Either way only the int8 rows cross PCIe.
+    const int8_t* src = q;
+    bool staged = false;
+    if (mem != DPH_MEM_DEVICE) {
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, q) == cudaSuccess && a.type == cudaMemoryTypeHost && a.devicePointer) src = (const int8_t*)a.devicePointer;
+        else { cudaGetLastError(); staged = true; }
+    }
+    DPH_TRY(ix->xdev.ensure((size_t)cs * d * 4));
+    if (staged) DPH_TRY(ix->enc_q8.ensure((size_t)cs * d));
+    const int vec = ((uintptr_t)src & 15) == 0;
+    for (int64_t o = 0; o < n; o += cs) {
+        const int64_t m = std::min(cs, n - o);
+        const int8_t* qc = src + o * d;
+        if (staged) {              // stream order keeps the staging chunk until the previous chunk's dequantisation has read it
+            DPH_CUDA(cudaMemcpyAsync(ix->enc_q8.p, q + o * d, (size_t)m * d, cudaMemcpyHostToDevice, ix->stream));
+            qc = ix->enc_q8.as<int8_t>();
+        }
+        const long long groups = m * d / 16;
+        const unsigned grid = (unsigned)std::min<long long>((groups + 255) / 256, 8ll * ix->num_sms);
+        dequant_int8_kernel<<<grid, 256, 0, ix->stream>>>(qc, groups, offset, scale, staged ? 1 : vec, ix->xdev.as<float>());
+        DPH_CUDA(cudaGetLastError());
+        DPH_TRY(dph_encode_rows(ix, ix->xdev.as<float>(), m, list_out + o, codes_out + o * DPH_M, bad));
     }
     return 0;
 }

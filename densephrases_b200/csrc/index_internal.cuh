@@ -91,7 +91,7 @@ struct dph_index {
         grp_cnt, grp_fill, grp_off, grp_blockpre, grp_entries, grp_unitpre, grp_units, grp_udesc, groupwork,   // grouped plan (prep.cu)
         csplit, xsplit, candkeys, cflags, selkeys,
         rb_ids, rb_out, rb_found, ws_q, ws_id, ws_out, ws_xq,        // reconstruct_batch / window_scores staging (host-buffer calls)
-        enc_key, enc_cd, enc_list, enc_codes,                        // encode / add: top-1 coarse result, host-call output staging
+        enc_key, enc_cd, enc_list, enc_codes, enc_q8,                // encode / add: top-1 coarse result, host-call staging
         qfview;                                                      // the search chunk's DphQfView (per-query filter)
     int64_t csplit_lo = -1, csplit_nl = -1;
     int coarse_tc = 1;                 // tensor-core coarse quantizer with exact re-rank (0: always the SIMT sequential-k GEMM)
@@ -328,6 +328,10 @@ __global__ void fill_blocks_kernel(uint8_t* codes, long long nblocks, const long
 // ---- encode.cu ----
 int64_t dph_encode_chunk(const dph_index* ix);
 int dph_encode_rows(dph_index* ix, const float* x_dev, int64_t n, int64_t* list_out, uint8_t* codes_out, int* bad);
+// The input stage of add_int8: rows x = q / scale + offset of int8 q [n, d] (mem: device, or host, page-locked read in place or
+// pageable staged as int8) dequantised chunk by chunk into xdev, then dph_encode_rows.
+int dph_encode_int8(dph_index* ix, const int8_t* q, int64_t n, float offset, float scale, int mem, int64_t* list_out, uint8_t* codes_out,
+                    int* bad);
 // Top-1 coarse list of n <= dph_encode_chunk rows xr [n, d] against centroids C [nlist, d]: the encoding's assignment (tensor-core
 // candidates + exact re-rank where the shape allows, else the SIMT sequential-k GEMM; smallest list id on a tie).  ix->S must hold
 // the n x nlist (padded to 128) scores.  key [n] int32, cd [n] the top-1 score.

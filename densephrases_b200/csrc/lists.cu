@@ -2,6 +2,8 @@
 // remove.cu holds remove_ids and sync_list_len; both commit their layout through dph_commit_layout below.
 #include "index_internal.cuh"
 #include <atomic>
+#include <cmath>
+#include <functional>
 #include <limits.h>
 #include <stdlib.h>
 #include <thrust/device_ptr.h>
@@ -304,34 +306,31 @@ __global__ void add_scatter_kernel(long long n, const long long* sorted_list, co
     dm_rows[dm0 + r] = blk * 32 + lane;
 }
 
-DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem) {
+// The body of add_with_ids and add_int8.  `encode` is the input stage: it assigns and encodes the n rows into list_all [n] and
+// codes_all [n,96] on the index stream and ORs 1 into flag on a non-finite value.  Validation, the new layout, the host mover and
+// the commit are shared.  `what` prefixes every error.
+static int add_rows(dph_index* ix, int64_t n, const int64_t* ids, int mem, const char* what,
+                    const std::function<int(int64_t* list_all, uint8_t* codes_all, int* flag)>& encode) {
+    const std::string w(what);
     DPH_TRY(check_ready(ix, 1));
-    DPH_CHECK(n >= 0, "add_with_ids: n must be >= 0");
+    DPH_CHECK(n >= 0, w + ": n must be >= 0");
     if (!ix->host_mutable)          // a host index without a reserved capacity (reserve_host_codes) stays read-only
-        DPH_CHECK(!ix->on_host, "add_with_ids: the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
+        DPH_CHECK(!ix->on_host, w + ": the codes of this index are in host memory, which is read-only after set_lists; the index is unchanged");
     DPH_CUDA(cudaSetDevice(ix->device));
     if (n == 0) return 0;
     cudaStream_t st = ix->stream;
     const int64_t nlist = ix->nlist, lo = ix->list_lo, hi = ix->list_hi;
     for (float& a : ix->add_ms) a = 0.f;
     DevTmp tmp;
-    const char* oom = "add_with_ids: not enough device memory for the batch; the index is unchanged";
+    const std::string oom = w + ": not enough device memory for the batch; the index is unchanged";
     int64_t *list_all, *ids_all; uint8_t* codes_all; int *flag, *cnt;
-    DPH_TRY(tmp.alloc(&list_all, n, oom)); DPH_TRY(tmp.alloc(&ids_all, n, oom)); DPH_TRY(tmp.alloc(&codes_all, (size_t)n * DPH_M, oom));
-    DPH_TRY(tmp.alloc(&flag, 1, oom)); DPH_TRY(tmp.alloc(&cnt, nlist, oom));
+    DPH_TRY(tmp.alloc(&list_all, n, oom.c_str())); DPH_TRY(tmp.alloc(&ids_all, n, oom.c_str()));
+    DPH_TRY(tmp.alloc(&codes_all, (size_t)n * DPH_M, oom.c_str()));
+    DPH_TRY(tmp.alloc(&flag, 1, oom.c_str())); DPH_TRY(tmp.alloc(&cnt, nlist, oom.c_str()));
     DPH_CUDA(cudaMemsetAsync(flag, 0, 4, st));
     DPH_CUDA(cudaMemsetAsync(cnt, 0, nlist * 4, st));
-    // 1. assign + encode (host input: bounded staging, one encode chunk at a time)
-    if (mem == DPH_MEM_DEVICE) DPH_TRY(dph_encode_rows(ix, x, n, list_all, codes_all, flag));
-    else {
-        const int64_t cs = std::min(dph_encode_chunk(ix), n);
-        DPH_TRY(ix->xdev.ensure((size_t)cs * ix->d * 4));
-        for (int64_t o = 0; o < n; o += cs) {
-            const int64_t m = std::min(cs, n - o);
-            DPH_CUDA(cudaMemcpyAsync(ix->xdev.p, x + o * ix->d, (size_t)m * ix->d * 4, cudaMemcpyHostToDevice, st));
-            DPH_TRY(dph_encode_rows(ix, ix->xdev.as<float>(), m, list_all + o, codes_all + o * DPH_M, flag));
-        }
-    }
+    // 1. assign + encode
+    DPH_TRY(encode(list_all, codes_all, flag));
     if (ids) DPH_CUDA(cudaMemcpyAsync(ids_all, ids, (size_t)n * 8, mem == DPH_MEM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
     else iota_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((long long*)ids_all, n, ix->ntotal);        // IndexIVF::add: ntotal + i
     add_validate_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>((const long long*)list_all, (const long long*)ids_all, n, flag, cnt);
@@ -341,9 +340,9 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     DPH_CUDA(cudaMemcpyAsync(&h_flag, flag, 4, cudaMemcpyDeviceToHost, st));
     DPH_CUDA(cudaMemcpyAsync(h_cnt.data(), cnt, nlist * 4, cudaMemcpyDeviceToHost, st));
     DPH_CUDA(cudaStreamSynchronize(st));
-    DPH_CHECK(!(h_flag & 1), "add_with_ids: the input holds a non-finite value; the index is unchanged");
-    DPH_CHECK(!(h_flag & 2), "add_with_ids: negative label (-1 marks padding rows); the index is unchanged");
-    DPH_CHECK(!(h_flag & 4), "add_with_ids: a vector has no best list; the index is unchanged");
+    DPH_CHECK(!(h_flag & 1), w + ": the input holds a non-finite value; the index is unchanged");
+    DPH_CHECK(!(h_flag & 2), w + ": negative label (-1 marks padding rows); the index is unchanged");
+    DPH_CHECK(!(h_flag & 4), w + ": a vector has no best list; the index is unchanged");
 
     // 2. the new layout: every list's length (all shards), this shard's tightly packed blocks
     std::vector<int64_t> len_new(nlist), bstart(nlist, 0);
@@ -352,8 +351,8 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
         if (l + 1 < nlist) bstart[l + 1] = bstart[l] + h_cnt[l];
     }
     DphLayout L;
-    DPH_TRY(L.build(ix, len_new.data(), "add_with_ids: a list would exceed 2^31 - 1 rows; the index is unchanged"));
-    DPH_TRY(dph_host_capacity_check(ix, L, "add_with_ids"));
+    DPH_TRY(L.build(ix, len_new.data(), (w + ": a list would exceed 2^31 - 1 rows; the index is unchanged").c_str()));
+    DPH_TRY(dph_host_capacity_check(ix, L, what));
     const DphLayout& old = ix->lay;
     const int64_t nb = L.nblocks;
     const bool was_explicit = ix->ids != nullptr;
@@ -362,8 +361,9 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
 
     // 3. every new buffer before anything changes: a failed allocation leaves the index as it was.  A host index re-lays its code
     //    array in place (host_move.cu) through two staging buffers instead of a new code buffer.
-    const char* oom2 = "add_with_ids: not enough device memory for the re-layout (the old and the new code buffers of the shard are live "
-                       "together); the index is unchanged";
+    const std::string oom2s = w + ": not enough device memory for the re-layout (the old and the new code buffers of the shard are live "
+                                  "together); the index is unchanged";
+    const char* oom2 = oom2s.c_str();
     uint8_t* codes_new = nullptr; int64_t *ids_new, *dm_ids_new, *dm_rows_new, *d_boff_new, *d_bstart, *d_lrs, *perm;
     DphHostMover mover;
     const int64_t d_first = ix->on_host ? dph_first_changed_block(old, L) : 0;
@@ -404,7 +404,7 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
         thrust::stable_sort_by_key(thrust::cuda::par.on(st), dk, dk + dm_cap, dv);       // equal labels keep insertion order
     } catch (const std::exception& e) {
         cudaGetLastError();
-        dph_set_error(std::string("add_with_ids: device sort failed; the index is unchanged: ") + e.what());
+        dph_set_error(w + ": device sort failed; the index is unchanged: " + e.what());
         return 1;
     }
     if (ix->on_host)        // the old blocks move up in place; each staged chunk receives the new rows that land in it
@@ -430,6 +430,28 @@ DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, con
     if (ix->on_host) DPH_TRY(dph_host_after_mutation(ix, shard_changed));
     if (prof) DPH_CUDA(cudaEventElapsedTime(&ix->add_ms[3], ix->aev[4], ix->aev[5]));
     return 0;
+}
+
+DPH_API int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem) {
+    return add_rows(ix, n, ids, mem, "add_with_ids", [&](int64_t* list_all, uint8_t* codes_all, int* flag) {
+        if (mem == DPH_MEM_DEVICE) return dph_encode_rows(ix, x, n, list_all, codes_all, flag);
+        const int64_t cs = std::min(dph_encode_chunk(ix), n);          // host input: bounded staging, one encode chunk at a time
+        DPH_TRY(ix->xdev.ensure((size_t)cs * ix->d * 4));
+        for (int64_t o = 0; o < n; o += cs) {
+            const int64_t m = std::min(cs, n - o);
+            DPH_CUDA(cudaMemcpyAsync(ix->xdev.p, x + o * ix->d, (size_t)m * ix->d * 4, cudaMemcpyHostToDevice, ix->stream));
+            DPH_TRY(dph_encode_rows(ix, ix->xdev.as<float>(), m, list_all + o, codes_all + o * DPH_M, flag));
+        }
+        return 0;
+    });
+}
+
+DPH_API int dph_index_add_int8(dph_index* ix, const int8_t* q, int64_t n, float offset, float scale, const int64_t* ids, int mem) {
+    DPH_CHECK(std::isfinite(scale) && scale != 0.0f, "add_int8: scale must be finite and non-zero; the index is unchanged");
+    DPH_CHECK(std::isfinite(offset), "add_int8: offset must be finite; the index is unchanged");
+    return add_rows(ix, n, ids, mem, "add_int8", [&](int64_t* list_all, uint8_t* codes_all, int* flag) {
+        return dph_encode_int8(ix, q, n, offset, scale, mem, list_all, codes_all, flag);
+    });
 }
 
 // The inverse of set_lists: this shard's rows as list-major host arrays, through the same bounded staging.

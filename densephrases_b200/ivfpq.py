@@ -194,6 +194,39 @@ class IvfPqIndex:
         self.set_stream(torch.cuda.current_stream(x.device).cuda_stream)
         L.check(L.lib().dph_index_add_with_ids(self._h, x.data_ptr(), n, None if ids is None else ids.data_ptr(), L.MEM_DEVICE))
 
+    def add_int8(self, q, ids, offset, scale):
+        """add_with_ids of the rows x = q / scale + offset of int8 q [n,d], computed in fp32 as the reference's int8_to_float did under
+        numpy 1.x: fl32(fl32(float(q) / fl32(scale)) + fl32(offset)) (DESIGN.md 3.8).  The index afterwards is byte-identical to
+        add_with_ids of those rows.  q is numpy (pageable, or a view of page-locked memory, read in place), a torch CPU tensor
+        (pinned or not) or a torch CUDA tensor; ids as for add_with_ids, on the same side.  Only int8 crosses PCIe.  Raises
+        RuntimeError, leaving the index unchanged, on a scale that is zero or not finite in fp32, an offset that is not finite, and
+        everything add_with_ids rejects."""
+        with np.errstate(over="ignore"):
+            off32, scale32 = float(np.float32(offset)), float(np.float32(scale))
+        if isinstance(q, np.ndarray):
+            if q.dtype != np.int8:
+                raise RuntimeError(f"add_int8: q must be int8, got {q.dtype}")
+            q = np.ascontiguousarray(q)
+            n = self._rows(q)
+            if ids is not None:
+                ids = np.ascontiguousarray(np.asarray(ids.cpu() if hasattr(ids, "cpu") else ids), dtype=np.int64)
+                if ids.shape != (n,):
+                    raise RuntimeError(f"ids has shape {ids.shape}, expected ({n},)")
+            L.check(L.lib().dph_index_add_int8(self._h, _np_ptr(q), n, off32, scale32, None if ids is None else _np_ptr(ids), L.MEM_HOST))
+            return
+        import torch
+        if q.dtype != torch.int8 or not q.is_contiguous():
+            raise RuntimeError(f"add_int8: q must be a contiguous int8 tensor, got {q.dtype}")
+        n = self._rows(q)
+        if ids is not None:
+            ids = torch.as_tensor(ids, dtype=torch.int64).to(q.device).contiguous()
+            if tuple(ids.shape) != (n,):
+                raise RuntimeError(f"ids has shape {tuple(ids.shape)}, expected ({n},)")
+        mem = L.MEM_DEVICE if q.is_cuda else L.MEM_HOST
+        if q.is_cuda:
+            self.set_stream(torch.cuda.current_stream(q.device).cuda_stream)
+        L.check(L.lib().dph_index_add_int8(self._h, q.data_ptr(), n, off32, scale32, None if ids is None else ids.data_ptr(), mem))
+
     def add(self, x):
         """== faiss index.add(x): labels ntotal + arange(n)."""
         self.add_with_ids(x, None)

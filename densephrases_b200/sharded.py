@@ -161,6 +161,10 @@ class ShardedIvfPq:
         the same global list lengths and labels (ids None -> ntotal + arange(n)) and stores the rows of its own lists."""
         self.local.add_with_ids(x, ids)
 
+    def add_int8(self, q, ids, offset, scale):
+        """add_with_ids of int8 rows dequantised in fp32 on the device (IvfPqIndex.add_int8); a collective like add_with_ids."""
+        self.local.add_int8(q, ids, offset, scale)
+
     def remove_ids(self, sel):
         """== faiss index.remove_ids (IvfPqIndex.remove_ids selectors); a collective: every rank passes the same selector.  Each rank
         removes the rows of its own lists; the per-list counts are all-reduced so that every rank sets the same global list lengths

@@ -12,6 +12,7 @@
  *   dph_index_create/set_*      <- faiss.read_index(...) / IndexPreTransform(OPQMatrix, IndexIVFPQ(...))
  *                                  densephrases/index.py:30 ; build_phrase_index.py:113-116,149-150
  *   dph_index_add_with_ids      <- index.add_with_ids(vectors, ids)          build_phrase_index.py:145-150,156-279
+ *   dph_index_add_int8          <- index.add_with_ids(int8_to_float(start, offset, scale), ids)   build_phrase_index.py:207-226
  *   dph_index_encode            <- the assignment + PQ encoding inside add_with_ids (IndexIVFPQ::encode_vectors)
  *   dph_index_copy_lists        <- the inverted lists faiss.write_index stores (invlists->get_codes / get_ids)
  *   dph_index_remove_ids        <- index.remove_ids(IDSelectorBatch(ids) | IDSelectorRange(lo, hi)) (faiss 1.6.x IndexIVF)
@@ -87,6 +88,12 @@ int dph_index_encode(dph_index* ix, const float* x, int64_t n, int64_t* list_no_
  * non-finite input value, too little device memory for the old and the new code buffers at once (a host index with a reserved
  * capacity: for two staging buffers), a host index whose capacity the new layout exceeds.  Synchronises the stream. */
 int dph_index_add_with_ids(dph_index* ix, const float* x, int64_t n, const int64_t* ids, int mem);
+/* add_with_ids of the rows x = fl32(fl32(q / scale) + offset) of int8 q [n,d] (a phrase dump's `start` rows with its group's offset and
+ * scale attributes cast to fp32): byte-identical to add_with_ids of those fp32 rows.  mem DPH_MEM_DEVICE: q and ids are device
+ * pointers.  DPH_MEM_HOST: page-locked q is read in place through its device mapping, pageable q through a bounded device staging
+ * chunk of int8; no fp32 copy of the rows is made on the host.  q may start at any byte offset.  Rejected, with the index
+ * unchanged: scale zero or not finite, offset not finite, and every case add_with_ids rejects.  Synchronises the stream. */
+int dph_index_add_int8(dph_index* ix, const int8_t* q, int64_t n, float offset, float scale, const int64_t* ids, int mem);
 /* This shard's lists as list-major host arrays: codes_out [ntotal_local,96], ids_out [ntotal_local] (may be NULL); the inverse of
  * set_lists, for writing a grown index back to a faiss file (artifacts.write_faiss_index). */
 int dph_index_copy_lists(dph_index* ix, uint8_t* codes_out, int64_t* ids_out);
